@@ -38,12 +38,14 @@ MODELS = {
 
 
 def metric_label(model):
-    """ONE metric string per model, shared by the B200 arm and the reference arm (the driver matches the two lines on it)."""
+    """ONE metric string per model, shared by the GPU arm and the reference arm (the two lines are matched on it)."""
     return f"images/sec ({MODELS[model]['label']} training step)"
 
 
 ADAMW_MODELS = ("convnext_tiny", "swin_tiny")   # AdamW(lr 5e-4, wd 5e-2): convNext/train.py:96,102; swin config.py:133-162
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+# H100 SXM data-sheet figures (HBM3 bandwidth, dense BF16; a card allowed 700 W) for the roofline fractions when no measured
+# peaks are supplied
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}
 
 
 def load_peaks():
@@ -230,7 +232,7 @@ def run_reference(args):
     emit(line)
 
 
-# ------------------------------------------------------------------------------------------------------- B200 arm
+# ------------------------------------------------------------------------------------------------------- GPU arm
 def build_model(name, dev):
     if name == "resnet50":
         from deeplearning_b200.classification.resnet.models.networks import resnet50
@@ -253,6 +255,27 @@ def build_model(name, dev):
 def optimizer_desc(name):
     return ("AdamW(lr=5e-4, wd=5e-2, decay groups, clip_grad_norm 5.0)" if name == "swin_tiny" else
             "AdamW(lr=5e-4, wd=5e-2, decay groups)" if name in ADAMW_MODELS else "SGD(momentum=0.9, weight_decay=5e-5)")
+
+
+DUMP_PARAM_SAMPLE = 4_000_000   # parameters per model written by --dump-outputs (16 MB of float32)
+
+
+def dump_outputs(dirpath, name, loss, correct, trainer):
+    """What the timed path hands its caller after its last step: the loss, the count of correct predictions and the updated
+    parameters (float32; a fixed, seeded sample of DUMP_PARAM_SAMPLE of them, the same indices on every run)."""
+    import numpy as np
+    import torch
+
+    os.makedirs(dirpath, exist_ok=True)
+    flat = trainer.arena.flat_p.detach().float()
+    n = flat.numel()
+    if n > DUMP_PARAM_SAMPLE:
+        idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:DUMP_PARAM_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    arrays = {"loss": loss.detach().float().reshape(1), "correct": torch.as_tensor(correct).detach().float().reshape(-1),
+              "params": flat}
+    for key, t in arrays.items():
+        np.save(os.path.join(dirpath, f"{name}_{key}.npy"), t.cpu().numpy().astype(np.float32))
 
 
 def measure(name, args, dev, world, rank, local_rank, batch=None):
@@ -299,20 +322,22 @@ def measure(name, args, dev, world, rank, local_rank, batch=None):
     if not args.eager:
         trainer.capture(images, labels)         # whole step (fwd+CE+bwd+all-reduce+update)
     for _ in range(warmup):
-        loss, _ = trainer.step(images, labels)
+        loss, correct = trainer.step(images, labels)
     sync_all()
     sampler = ClockSampler(local_rank)
     sampler.start()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        loss, _ = trainer.step(images, labels)
+        loss, correct = trainer.step(images, labels)
     e1.record()
     sync_all()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     launches = launches_per_step * args.steps   # graph replays launch the same kernels the eager step does
     clocks = sampler.stop()
     final_loss = float(loss)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, name, loss, correct, trainer)
     ms_step = ms_total / args.steps
     value = world * B * args.steps / (ms_total / 1e3)
 
@@ -405,7 +430,7 @@ def measure(name, args, dev, world, rank, local_rank, batch=None):
                        "optimizer": optimizer_desc(name),
                        "step": "fwd+CE+bwd+allreduce+optimizer",
                        "launch": "eager" if args.eager else "CUDA graph replay",
-                       "l2": "working set (>10 GB of activations per step) is far larger than the 126 MB L2; no flush needed"},
+                       "l2": "working set (>10 GB of activations per step) is far larger than the 50 MB L2; no flush needed"},
             "e2e": {"value": e2e_value, "unit": "images/sec", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
                     "ms_per_step": e2e_ms / args.steps},
             "gpu_launches": int(launches), "clocks": clocks, "final_loss": final_loss}
@@ -470,7 +495,7 @@ def run_b200(args):
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py needs a B200: no CUDA device visible (there is no CPU fallback; use --impl reference)")
+        raise RuntimeError("bench.py needs an H100: no CUDA device visible (there is no CPU fallback; use --impl reference)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -504,6 +529,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the ViT-B/16 block of the default (resnet50) line")
     ap.add_argument("--eager", action="store_true", help="do not capture the step into CUDA graphs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (loss, correct count, a fixed sample of the "
+                         "updated parameters) as DIR/<model>_<name>.npy, float32")
     args = ap.parse_args()
     global _JSON_FD
     sys.stdout.flush()

@@ -1,7 +1,7 @@
-"""deeplearning_b200: a B200-native (sm_100a) implementation of the KKKSQJ/DeepLearning classification training step.
+"""deeplearning_b200: an H100-native (sm_90a) implementation of the KKKSQJ/DeepLearning classification training step.
 
 Layout
-  csrc/            hand-written CUDA (tcgen05 / TMA / TMEM) + the C-ABI (include/b200cls.h) -> lib/libb200cls.so
+  csrc/            hand-written CUDA (wgmma / TMA / mbarrier) + the C-ABI (include/b200cls.h) -> lib/libb200cls.so
   _lib.py, ops.py  ctypes binding and tensor-level wrappers (PyTorch = device memory + streams only)
   engine/          forward/backward schedules of the backbones, gradient arena + data-parallel step
   classification/  host-side mirrors of the reference constructors (same names, signatures, state_dict keys)

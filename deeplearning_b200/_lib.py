@@ -117,7 +117,7 @@ SIGNATURES = {
     "b200_conv1x1_bn_fwd": (_I, [_P, _P, _P, _P, _P, _L, _I, _I, _P]),
     "b200_subsample2": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "b200_add_even_pixels": (_I, [_P, _P, _I, _I, _I, _I, _P]),
-    "b200_conv1x1_dgrad_masked_stats_rows": (_I, [_L, _I]),
+    "b200_conv1x1_dgrad_masked_stats_rows": (_I, [_L, _I, _I]),
     "b200_conv1x1_dgrad_masked": (_I, [_P, _P, _P, _L, _I, _I, _P, _P, _P, _P]),
     "b200_bn_conv1x1_bwd_scratch_bytes": (c_size_t, [_I, _I]),
     "b200_bn_conv1x1_bwd": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _D, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, c_size_t, _P, _P]),

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference ConvNeXt constructors, backed by the sm_100a engine.
+"""Host-side mirror of the reference ConvNeXt constructors, backed by the sm_90a engine.
 
 Drop-in for ``classification/convNext/models/networks.py`` of KKKSQJ/DeepLearning (ConvNeXt ``:108``, Block ``:70``,
 LayerNorm ``:41``, ``convnext_tiny`` ``:173`` ...): same constructor signatures, parameter names / shapes and the same

@@ -1,8 +1,8 @@
 """Host-side mirror of the reference's MNIST toy nets (classification/mnist/models/network.py:7 ``mnist_cnn``, :34 ``mnist_fcn``).
 
 BASELINE.json's config 0 is *CPU plumbing, no GPU*: it exists to exercise the host loop (constructor -> forward -> loss ->
-backward -> optimizer) end to end where no B200 is present, so these two nets are ordinary PyTorch modules with the
-reference's layer structure, parameter names and initialisation order.  They are not part of the sm_100a hot path.
+backward -> optimizer) end to end where no GPU is present, so these two nets are ordinary PyTorch modules with the
+reference's layer structure, parameter names and initialisation order.  They are not part of the sm_90a hot path.
 """
 import torch
 import torch.nn as nn

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference ResNet constructors, backed by the sm_100a engine.
+"""Host-side mirror of the reference ResNet constructors, backed by the sm_90a engine.
 
 Drop-in for ``classification/resnet/models/networks.py`` of KKKSQJ/DeepLearning (ResNet ``:127``, Bottleneck ``:78``,
 BasicBlock ``:38``, resnet50 ``:259``; the training script builds the identical torchvision model, train.py:14,74):

@@ -2,7 +2,7 @@
 
 Replaces ``swin_window_process`` (the pybind module built by kernels/window_process/setup.py from swin_window_process.cpp:1-132
 and swin_window_process_kernel.cu:1-354) and the two autograd Functions of kernels/window_process/window_process.py:11-63 with
-the same names, argument order and semantics, on top of the 16-byte-vectorised sm_100a permutation kernels behind
+the same names, argument order and semantics, on top of the 16-byte-vectorised sm_90a permutation kernels behind
 ``b200_window_partition`` / ``b200_window_merge`` (include/b200cls.h):
 
     roll_and_window_partition_forward(x, B, H, W, C, shift, ws)   == window_partition(torch.roll(x, (shift, shift), (1, 2)), ws)
@@ -19,7 +19,7 @@ from deeplearning_b200 import ops
 
 def _chk(t):
     if not t.is_cuda:
-        raise RuntimeError("swin_window_process: CUDA (sm_100a) tensors only; there is no CPU fallback")
+        raise RuntimeError("swin_window_process: CUDA (sm_90a) tensors only; there is no CPU fallback")
     return t.contiguous()
 
 

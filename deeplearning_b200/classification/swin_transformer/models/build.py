@@ -8,7 +8,7 @@ from .swin_transformer import SwinTransformer
 def build_model(config, is_pretrain=False):
     model_type = config.MODEL.TYPE
     if model_type != 'swin':
-        raise NotImplementedError(f"Unkown model: {model_type} (the B200 engine implements MODEL.TYPE 'swin')")
+        raise NotImplementedError(f"Unkown model: {model_type} (this engine implements MODEL.TYPE 'swin')")
     s = config.MODEL.SWIN
     return SwinTransformer(img_size=config.DATA.IMG_SIZE, patch_size=s.PATCH_SIZE, in_chans=s.IN_CHANS,
                            num_classes=config.MODEL.NUM_CLASSES, embed_dim=s.EMBED_DIM, depths=s.DEPTHS,

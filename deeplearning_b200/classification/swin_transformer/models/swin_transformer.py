@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference Swin Transformer constructors, backed by the sm_100a engine.
+"""Host-side mirror of the reference Swin Transformer constructors, backed by the sm_90a engine.
 
 Drop-in for ``classification/swin_transformer/models/swin_transformer.py`` of KKKSQJ/DeepLearning (SwinTransformer ``:478``,
 BasicLayer ``:353``, SwinTransformerBlock ``:168``, WindowAttention ``:70``, PatchMerging ``:308``, PatchEmbed ``:430``,
@@ -6,7 +6,7 @@ Mlp ``:19``): same constructor signatures, parameter / buffer names (``relative_
 ``relative_position_index``, ``attn_mask`` ...), shapes and initialisation RNG order, so reference checkpoints load with
 ``strict=True``.  No timm dependency (``DropPath`` / ``to_2tuple`` / ``trunc_normal_`` are local).  Sub-modules only hold
 parameters; ``SwinTransformer.forward`` runs the whole network through ``deeplearning_b200.engine.swin``: the cyclic shift,
-window partition / reverse, relative-position bias and shift mask all live inside one tcgen05 window-attention kernel.
+window partition / reverse, relative-position bias and shift mask all live inside one wgmma window-attention kernel.
 """
 import torch
 import torch.nn as nn

@@ -1,11 +1,11 @@
-"""Host-side mirror of the reference ViT constructors, backed by the sm_100a engine.
+"""Host-side mirror of the reference ViT constructors, backed by the sm_90a engine.
 
 Drop-in for ``classification/vision_transformer/vit_model.py`` of KKKSQJ/DeepLearning (VisionTransformer ``:164``,
 Block ``:136``, Attention ``:71``, Mlp ``:114``, PatchEmbed ``:43``, ``vit_base_patch16_224_in21k`` ``:290`` ...): same
 constructor signatures, attribute / state_dict names, shapes and initialisation RNG order (``trunc_normal_`` on pos/cls,
 then ``apply(_init_vit_weights)``), so reference checkpoints load unchanged and ``torch.manual_seed(s)`` gives bit-identical
 initial weights.  The sub-modules only hold parameters: ``VisionTransformer.forward`` runs the whole network through
-``deeplearning_b200.engine.vit`` (fused patch-embed GEMM, LayerNorm, tcgen05 attention, GEMMs with bias/GELU/residual
+``deeplearning_b200.engine.vit`` (fused patch-embed GEMM, LayerNorm, wgmma attention, GEMMs with bias/GELU/residual
 epilogues) as one autograd Function.  No CPU path.
 """
 from collections import OrderedDict

@@ -1,4 +1,4 @@
-// C-ABI entry points for the tcgen05 implicit-GEMM kernels (forward / dgrad / wgrad). Host side only builds tensor maps,
+// C-ABI entry points for the wgmma implicit-GEMM kernels (forward / dgrad / wgrad). Host side only builds tensor maps,
 // tap tables and tile geometry; see conv_gemm.cuh / wgrad_gemm.cuh for the device code.
 #include <stdlib.h>
 #include <string.h>
@@ -101,7 +101,7 @@ int encode_view(CUtensorMap* m, const View& v, const Box3& bx) {
   return encode_tmap_bf16(m, v.base, 4, v.dims, v.strides, box);
 }
 
-// The epilogue stores one TMEM lane quadrant (32 consecutive tile rows) per warp: split the 128-pixel box into 4 slabs along
+// The epilogue stores one quadrant (32 consecutive tile rows) per warp: split the 128-pixel box into 4 slabs along
 // its slowest-varying dimensions (all box dims are powers of two, rows are ordered w fastest).
 void quarter_box(const Box3& bx, Box3* qb, int (&o1)[4], int (&o2)[4], int (&o3)[4]) {
   for (int q = 0; q < 4; ++q) o1[q] = o2[q] = o3[q] = 0;
@@ -147,7 +147,7 @@ int setup_output(ConvGemmParams& p, const View& dv, int N, int out_f32, const Vi
   p.tiles2 = static_cast<int>((d2 + bx.b2 - 1) / bx.b2);
   p.tiles3 = static_cast<int>((d3 + bx.b3 - 1) / bx.b3);
   p.N = N;
-  const int BN = N <= 64 ? 64 : (N <= 128 ? 128 : 256);
+  const int BN = N <= 64 ? 64 : 128;
   p.n_tiles = (N + BN - 1) / BN;
   Box3 qb;
   quarter_box(bx, &qb, p.qoff1, p.qoff2, p.qoff3);
@@ -229,63 +229,6 @@ int epilogue_flags(const ConvGemmParams& p) {
   X(kEpiBnMask)                                           /* 3x3 dgrad + reduce half of the producer's BN backward */ \
   X(kEpiBnMask | kEpiBias)                                /* the same behind the BN-algebra dual GEMM (bias = k W) */
 
-// ---- CTA-pair GEMM (tcgen05 cta_group::2): the 256-wide linear layers of the transformer / ConvNeXt paths run as pairs
-// of CTAs on one 256-pixel x 256-channel tile (each CTA stages half of the B tile).  Validated on B200 in round 2 (bit-exact
-// against the single-CTA kernel in tools/experiments/gemm_2cta_test.cu; the transformer GPU tests run through it): ViT-B/16
-// linear layers 1058 -> 1144 TFLOP/s.  B200_GEMM_PAIR=0 in the environment switches back to the single-CTA kernels.
-bool gemm_pair_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("B200_GEMM_PAIR");
-    return e == nullptr || e[0] != '0';
-  }();
-  return on;
-}
-
-template <int EPI>
-int launch_conv_gemm_pair(const ConvGemmParams& q, cudaStream_t st) {
-  using Cfg = ConvGemmCfg<256, true>;
-  static bool configured = false;
-  if (!configured) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<256, EPI, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES));
-    configured = true;
-  }
-  const int items = (q.tiles1 * q.tiles2 * q.tiles3 + 1) / 2 * q.n_tiles;   // pairs of pixel tiles x channel blocks
-  int pairs = device_sm_count() / 2;
-  if (items < pairs) pairs = items;
-  if (q.stats != nullptr) pairs = pairs / q.n_tiles * q.n_tiles;   // a pair must keep seeing the same channel block
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(Cfg::THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 2 : 1;
-  B200_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<256, EPI, true>, q));
-  B200_LAUNCHED();
-  return OK;
-}
-
-// the epilogues of the transformer / ConvNeXt linear layers
-#define B200_PAIR_EPI_LIST(X)                            \
-  X(0)                                                   \
-  X(kEpiBias)                                            \
-  X(kEpiBias | kEpiResF32 | kEpiOutF32)                  \
-  X(kEpiBias | kEpiColscale | kEpiResF32 | kEpiOutF32)   \
-  X(kEpiBias | (2 << kEpiActShift) | kEpiAux)            \
-  X(3 << kEpiActShift)                                   \
-  X((3 << kEpiActShift) | kEpiStats)                     \
-  X(kEpiOutF32)                                          \
-  X(kEpiBias | kEpiOutF32)
-
 // ---- 64 -> 64 channel convolutions with the weights resident in shared memory (conv_tap64.cuh): ResNet layer1's 3x3
 // forward / dgrad and the space-to-depth stem.  B200_TAP64=0 in the environment switches back to the generic kernel.
 bool tap64_enabled() {
@@ -308,7 +251,7 @@ int launch_tap64(const ConvGemmParams& q, int grid, cudaStream_t st) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tap64_kernel<kStats>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTap64SmemBytes));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(conv_tap64_kernel<kStats>, dim3(grid), dim3(192), kTap64SmemBytes, st, q));
+  B200_CHECK_CUDA(launch_pdl(conv_tap64_kernel<kStats>, dim3(grid), dim3(384), kTap64SmemBytes, st, q));
   B200_LAUNCHED();
   return OK;
 }
@@ -323,19 +266,6 @@ int launch_conv_gemm(const ConvGemmParams& p, cudaStream_t st) {
   q.desc_sbo = g_fwd_sbo;
   if constexpr (BLOCK_N == 64) {
     if (tap64_ok(p)) return p.stats != nullptr ? launch_tap64<true>(q, grid, st) : launch_tap64<false>(q, grid, st);
-  }
-  if constexpr (BLOCK_N == 256) {
-    if (p.pair) {
-      switch (epilogue_flags(p)) {
-#define B200_PAIR_CASE(F) \
-  case (F):               \
-    return launch_conv_gemm_pair<(F)>(q, st);
-        B200_PAIR_EPI_LIST(B200_PAIR_CASE)
-#undef B200_PAIR_CASE
-        default:
-          break;   // no pair kernel for this epilogue: the single-CTA kernels below
-      }
-    }
   }
   switch (epilogue_flags(p)) {
 #define B200_EPI_CASE(F) \
@@ -403,7 +333,7 @@ int run_stream(int mode, const void* a, const void* w, void* out, const void* re
   {
     uint64_t dims[2] = {static_cast<uint64_t>(N), static_cast<uint64_t>(pixels)};
     uint64_t strides[2] = {1, static_cast<uint64_t>(N)};
-    uint32_t box[2] = {64, 32};
+    uint32_t box[2] = {64, 16};
     if ((rc = encode_tmap_bf16(&q.out_map, out, 2, dims, strides, box))) return rc;
     if (res != nullptr && (rc = encode_tmap_bf16(&q.res_map, res, 2, dims, strides, box))) return rc;
     if (mask != nullptr && (rc = encode_tmap_bf16(&q.mask_map, mask, 2, dims, strides, box))) return rc;
@@ -425,10 +355,9 @@ int run_stream(int mode, const void* a, const void* w, void* out, const void* re
 
 int dispatch_conv_gemm(ConvGemmParams& p, int N, cudaStream_t st) {
   if (N <= 64) return launch_conv_gemm<64>(p, st);
-  if (N <= 128) return launch_conv_gemm<128>(p, st);
-  return launch_conv_gemm<256>(p, st);
+  return launch_conv_gemm<128>(p, st);
 }
-int block_n_for(int N) { return N <= 64 ? 64 : (N <= 128 ? 128 : 256); }
+int block_n_for(int N) { return N <= 64 ? 64 : 128; }
 
 template <int BLOCK_NG>
 int launch_wgrad(const WgradParams& p, cudaStream_t st) {
@@ -448,9 +377,9 @@ int launch_wgrad(const WgradParams& p, cudaStream_t st) {
   q.desc_sbo = g_wg_sbo;
   q.desc_kstep = g_wg_kstep;
   if (q.bias_partial != nullptr)   // + four warps that sum the dY tiles' columns (the layer's bias gradient)
-    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, true>, dim3(grid), dim3(320), Cfg::SMEM_BYTES, st, q));
+    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
   else
-    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, false>, dim3(grid), dim3(192), Cfg::SMEM_BYTES, st, q));
+    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, false>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
   B200_LAUNCHED();
   return OK;
 }
@@ -506,7 +435,7 @@ WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int
   pl.tiles3 = static_cast<int>((d3 + pl.box.b3 - 1) / pl.box.b3);
   pl.kb_total = pl.tiles1 * pl.tiles2 * pl.tiles3;
   // Split-K factor: minimise (waves x pixel blocks per item x time per block) + the fp32 partial traffic it causes. The
-  // per-block times are the measured, L2-operand-bandwidth-bound rates of the kernel (us per 64-pixel block and tile width).
+  // per-block times are estimates of the kernel's L2-operand-bound time (us per 64-pixel block, by tile width).
   const int items_per_split = pl.mg_tiles * pl.ng_tiles * (pl.merge_atoms ? 1 : pl.taps);
   const int sms = device_sm_count();
   const double t_kb = pl.block_ng == 256 ? 0.45 : (pl.block_ng == 192 ? 0.36 : (pl.block_ng == 128 ? 0.30 : 0.25));
@@ -519,6 +448,7 @@ WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int
     const int s2 = (pl.kb_total + kps - 1) / kps;
     if (s2 != s) continue;
     const int waves = (items_per_split * s + sms - 1) / sms;
+    if (waves > 2 && items_per_split <= sms) continue;   // never a third wave when one split's tiles fit on the SMs
     const double cost = waves * (kps * t_kb + 2.0) + s * part_us;
     if (cost < best) best = cost, splits = s;
     if (waves > 4 && s > 8) break;
@@ -573,11 +503,11 @@ int b200_conv2d_fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int str
   const long long d3 = flat ? 1 : B;
   const Box3 bx = choose_box(d1, d2, d3, 128);
   const long long m_tiles = ((d1 + bx.b1 - 1) / bx.b1) * ((d2 + bx.b2 - 1) / bx.b2) * ((d3 + bx.b3 - 1) / bx.b3);
-  const int BN = Cout <= 64 ? 64 : (Cout <= 128 ? 128 : 256);
+  const int BN = Cout <= 64 ? 64 : 128;
   const int n_tiles = (Cout + BN - 1) / BN;
   const long long tiles = m_tiles * n_tiles;
   const int grid = conv_grid(tiles > (1 << 30) ? (1 << 30) : static_cast<int>(tiles), n_tiles, true);
-  // one partial row per (CTA group, TMEM quadrant); the two warps of a quadrant write separate rows when they alternate
+  // one partial row per (CTA group, 32-row quadrant); the two warps of a quadrant write separate rows when they alternate
   // tiles (64-channel tiles) and disjoint column units of one row otherwise
   return grid / n_tiles * (BN == 64 ? 8 : 4);
 }
@@ -826,25 +756,6 @@ int b200_gemm_ex(const b200_view_t* a, const b200_view_t* out, const b200_gemm_a
     uint64_t strides[2] = {1, static_cast<uint64_t>(g->K)};
     uint32_t box[2] = {64, static_cast<uint32_t>(BN)};
     if ((rc = encode_tmap_bf16(&p.b_map, g->w, 2, dims, strides, box))) return rc;
-    bool pair_ok = BN == 256 && gemm_pair_enabled();
-    if (pair_ok && g->stats != nullptr) {
-      // the pair kernel writes (2 * pairs / n_tiles) * 4 partial rows; use it only when that is exactly what the caller
-      // allocated from b200_conv2d_fwd_stats_rows (the single-CTA grid), e.g. the fc2 dgrad of ViT-B/16 (N = 3072: 48 rows)
-      const int n_tiles = (g->N + 255) / 256;
-      const long long m_tiles = static_cast<long long>(p.tiles1) * p.tiles2 * p.tiles3;
-      const long long items = (m_tiles + 1) / 2 * n_tiles;
-      long long pairs = device_sm_count() / 2;
-      if (items < pairs) pairs = items;
-      pairs = pairs / n_tiles * n_tiles;
-      const long long tiles = m_tiles * n_tiles;
-      const int single = conv_grid(tiles > (1 << 30) ? (1 << 30) : static_cast<int>(tiles), n_tiles, true);
-      pair_ok = pairs > 0 && 2 * pairs == single && g->act == B200_ACT_GELU_GRAD;
-    }
-    if (pair_ok) {
-      uint32_t half[2] = {64, 128};
-      if ((rc = encode_tmap_bf16(&p.b_map_half, g->w, 2, dims, strides, half))) return rc;
-      p.pair = 1;
-    }
   }
   p.stats = g->stats;
   p.bias = g->bias;
@@ -859,7 +770,6 @@ int b200_gemm_ex(const b200_view_t* a, const b200_view_t* out, const b200_gemm_a
     B200_REQUIRE(g->rows_per_sample > 0, "gemm_ex: rowscale needs rows_per_sample > 0");
     p.rowscale = g->rowscale;
     p.rows_per_sample = g->rows_per_sample;
-    p.pair = 0;   // the per-sample multiplier lives in the generic single-CTA epilogue
   }
   if (g->act == B200_ACT_GELU_GRAD) {
     B200_REQUIRE(g->aux_in != nullptr, "gemm_ex: B200_ACT_GELU_GRAD needs aux_in");
@@ -1083,8 +993,10 @@ int b200_conv1x1_bn_fwd(const void* x, const void* w, const float* scale, const 
   return b200_conv2d_fwd(x, w, y, 1, 1, static_cast<int>(pixels), Cin, Cout, 1, 1, nullptr, nullptr, 0, nullptr, nullptr, 0, stream);
 }
 
-int b200_conv1x1_dgrad_masked_stats_rows(long long pixels, int Cin) {
-  // (the streaming kernel and the generic one write the same number of partial rows: one per CTA group and TMEM quadrant)
+int b200_conv1x1_dgrad_masked_stats_rows(long long pixels, int Cin, int Cout) {
+  // one partial row per CTA group and 32-row quadrant of the kernel b200_conv1x1_dgrad_masked dispatches to: the streaming
+  // kernel's groups own 256 channels, the generic kernel's 64 or 128
+  if (stream_ok(pixels, Cout, Cin)) return stream_grid(pixels, Cin) / (Cin / 256) * 4;
   return b200_conv2d_fwd_stats_rows(1, 1, static_cast<int>(pixels), Cin, 1, 1);
 }
 

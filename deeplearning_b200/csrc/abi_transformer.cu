@@ -1,4 +1,4 @@
-// C-ABI entry points of the transformer-side kernels: LayerNorm, patch extraction, attention (tcgen05) forward/backward.
+// C-ABI entry points of the transformer-side kernels: LayerNorm, patch extraction, attention (wgmma) forward/backward.
 #include <string.h>
 
 #include "../../include/b200cls.h"
@@ -472,6 +472,23 @@ int b200_patch_merge_ln_bwd(const void* dy, const float* x, const float* mean, c
   return OK;
 }
 
+}  // extern "C"
+
+namespace {
+template <int NT>
+int launch_attn_fwd(const AttnFwdParams& p, int grid, cudaStream_t st) {
+  static bool configured = false;
+  if (!configured) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd2_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn2SmemBytes));
+    configured = true;
+  }
+  B200_CHECK_CUDA(launch_pdl(attn_fwd2_kernel<NT>, dim3(grid), dim3(kAttn2Threads), kAttn2SmemBytes, st, p));
+  return OK;
+}
+}  // namespace
+
+extern "C" {
+
 int b200_attention_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, float scale, void* stream) {
   B200_REQUIRE(T >= 1 && T <= 256, "attention_fwd: T=%d unsupported (1..256 tokens)", T);
   B200_REQUIRE(B > 0 && H > 0, "attention_fwd: empty problem");
@@ -479,7 +496,7 @@ int b200_attention_fwd(const void* qkv, void* out, float* lse, int B, int T, int
   AttnFwdParams p;
   memset(&p, 0, sizeof(p));
   p.B = B, p.H = H, p.T = T;
-  p.Tpad = (T + 15) / 16 * 16;
+  p.Tpad = (T + 63) / 64 * 64;
   p.mblocks = (T + 127) / 128;
   p.scale = scale;
   p.scale_log2e = scale * 1.4426950408889634f;
@@ -489,24 +506,15 @@ int b200_attention_fwd(const void* qkv, void* out, float* lse, int B, int T, int
   if ((rc = encode3(&p.q_map, qkv, 3 * HD, T, B, 128))) return rc;
   if ((rc = encode3(&p.kv_map, qkv, 3 * HD, T, B, p.Tpad))) return rc;
   if ((rc = encode3(&p.o_map, out, HD, T, B, 128))) return rc;
-  static bool cfg = false;
-  static int version = 0;
-  if (!cfg) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
-    B200_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn2SmemBytes));
-    // default: the persistent kernel (attention_fwd2.cuh; ViT-B/16 layer at bs 256: 101 us);  B200_ATTN_FWD=1 selects the
-    // one-CTA-per-(batch, head, query block) kernel it replaced (attention.cuh; 148 us), kept as the A/B reference
-    const char* e = getenv("B200_ATTN_FWD");
-    version = (e != nullptr && e[0] == '1') ? 1 : 2;
-    cfg = true;
+  const int items = B * H;
+  const int grid = items < device_sm_count() ? items : device_sm_count();
+  switch (p.Tpad) {
+    case 64: rc = launch_attn_fwd<64>(p, grid, st); break;
+    case 128: rc = launch_attn_fwd<128>(p, grid, st); break;
+    case 192: rc = launch_attn_fwd<192>(p, grid, st); break;
+    default: rc = launch_attn_fwd<256>(p, grid, st); break;
   }
-  if (version == 2) {
-    const int items = B * H;
-    const int grid = items < device_sm_count() ? items : device_sm_count();
-    B200_CHECK_CUDA(launch_pdl(attn_fwd2_kernel, dim3(grid), dim3(kAttn2Threads), kAttn2SmemBytes, st, p));
-  } else {
-    B200_CHECK_CUDA(launch_pdl(attn_fwd_kernel, dim3(B * H * p.mblocks), dim3(160), kAttnSmemBytes, st, p));
-  }
+  if (rc) return rc;
   B200_LAUNCHED();
   return OK;
 }
@@ -539,7 +547,7 @@ int b200_attention_bwd(const void* qkv, const void* out, const void* dout, const
     B200_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnBwdSmemBytes));
     cfg = true;
   }
-  B200_CHECK_CUDA(launch_pdl(attn_bwd_kernel, dim3(B * H), dim3(288), kAttnBwdSmemBytes, st, p));
+  B200_CHECK_CUDA(launch_pdl(attn_bwd_kernel, dim3(B * H), dim3(kAttnBwdThreads), kAttnBwdSmemBytes, st, p));
   B200_LAUNCHED();
   return OK;
 }

@@ -1,19 +1,5 @@
-// Multi-head self-attention for short sequences (T <= 256 tokens, head_dim 64) on tcgen05 - forward.
-//
-//   O[b, t, h, :] = softmax_j( scale * Q[b,t,h,:] . K[b,j,h,:] ) V[b,j,h,:]
-//
-// One CTA per (batch, head, 128-query block); two CTAs are resident per SM so one CTA's soft-max overlaps the other's MMAs.
-// Q/K/V tiles of the packed qkv tensor [B][T][3][H][64] are fetched with 3-D TMA boxes (rows beyond T are zero-filled),
-// S = Q K^T (M=128, N=Tpad, K=64) accumulates in TMEM, the 128 soft-max threads own one query row each (tcgen05.ld gives
-// a thread its whole row: no shuffles), P is written as bf16 into the 128B-swizzled K-major layout and multiplied with V
-// (used in place as an MN-major operand - no transpose) into TMEM columns that S has vacated. S / P never touch HBM; only
-// the per-row log-sum-exp is kept for the backward pass.
-//
-// (Since late round 2 the product's forward is the persistent attn_fwd2_kernel of attention_fwd2.cuh - same parameters, math and
-// outputs, 148 -> 101 us per ViT-B/16 layer; this kernel is selected with B200_ATTN_FWD=1 and is the op's A/B reference.)
-//
-// Replaces the eager sequence of vit_model.py:95-108 (classification/vision_transformer): qkv split, (q@k^T)*scale, softmax,
-// attn@v, transpose/reshape, which materialises the [B,12,197,197] score tensor three times in HBM.
+// Multi-head self-attention for short sequences (T <= 256 tokens, head_dim 64): the parameters shared by the forward kernel
+// (attention_fwd2.cuh) and the backward kernels (attention_bwd.cuh, attn_delta_kernel below).
 #pragma once
 #include "common.cuh"
 
@@ -27,209 +13,20 @@ __device__ __forceinline__ float attn_ex2(float x) {  // MUFU.EX2; exp2f() adds 
 
 struct alignas(64) AttnFwdParams {
   CUtensorMap q_map;    // qkv as (3*H*64, T, B), box (64, 128, 1)
-  CUtensorMap kv_map;   // same tensor, box (64, Tpad, 1)
+  CUtensorMap kv_map;   // same tensor, box (64, Tpad, 1): keys beyond T are zero-filled
   CUtensorMap o_map;    // out as (H*64, T, B), box (64, 128, 1)
-  int B, H, T, Tpad, mblocks;
+  int B, H, T, Tpad, mblocks;   // Tpad = T rounded up to 64 (the key tile), mblocks = 128-query blocks
   float scale_log2e;    // scale * log2(e)
   float scale;
   float* lse;           // [B][H][T] natural-log LSE of the scaled scores
 };
-
-constexpr int kAttnSmemBytes = 16384 /*Q*/ + 32768 /*K*/ + 16384 /*pad so that P (64 KB) can alias Q+K+pad*/ + 32768 /*V*/ +
-                               256 + 1024;
-
-__global__ void __launch_bounds__(160, 2) attn_fwd_kernel(const __grid_constant__ AttnFwdParams p) {
-  pdl_launch_dependents();
-  pdl_wait();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;                 // [128][128B]
-  uint8_t* sK = smem + 16384;         // [Tpad][128B]
-  uint8_t* sP = smem;                 // 4 key blocks x [128][128B]; aliases Q+K once S is complete
-  uint8_t* sV = smem + 65536;         // [Tpad][128B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 65536 + 32768);
-  uint64_t* bar_load = bars;
-  uint64_t* bar_s = bars + 1;
-  uint64_t* bar_p = bars + 2;
-  uint64_t* bar_o = bars + 3;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 4);
-
-  const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int mb = blockIdx.x % p.mblocks;
-  const int h = (blockIdx.x / p.mblocks) % p.H;
-  const int b = blockIdx.x / (p.mblocks * p.H);
-  const int HD = p.H * 64;
-
-  if (warp_idx == 4) {
-    if (lane == 0) {
-      tma_prefetch_desc(&p.q_map);
-      tma_prefetch_desc(&p.kv_map);
-      tma_prefetch_desc(&p.o_map);
-      mbar_init(bar_load, 1);
-      mbar_init(bar_s, 1);
-      mbar_init(bar_p, 4);
-      mbar_init(bar_o, 1);
-      fence_mbar_init();
-    }
-    __syncwarp();
-    tmem_alloc<256>(tmem_ptr_smem);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp_idx == 4) {
-    if (lane == 0) {
-      mbar_expect_tx(bar_load, 16384 + 2 * p.Tpad * 128);
-      tma_load_3d(sQ, &p.q_map, bar_load, h * 64, mb * 128, b);
-      tma_load_3d(sK, &p.kv_map, bar_load, HD + h * 64, 0, b);
-      tma_load_3d(sV, &p.kv_map, bar_load, 2 * HD + h * 64, 0, b);
-      mbar_wait(bar_load, 0);
-      tc_fence_after();
-      // ---- S = Q K^T : A = Q (K-major), B = K (K-major, N = Tpad key rows), K = 64 (4 steps)
-      const uint32_t idesc_s = make_idesc_bf16(128, p.Tpad, 0, 0);
-      const uint32_t q_addr = smem_u32(sQ), k_addr = smem_u32(sK);
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        umma_f16(tmem_base, make_smem_desc_sw128(q_addr + k * 32, 16, 1024), make_smem_desc_sw128(k_addr + k * 32, 16, 1024),
-                 idesc_s, k > 0 ? 1u : 0u);
-      umma_commit(bar_s);
-      // ---- O = P V : A = P (K-major, key blocks of 64), B = V (MN-major: rows = keys, 64 contiguous d), K = Tpad keys
-      mbar_wait(bar_p, 0);
-      tc_fence_after();
-      const uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-      const uint32_t p_addr = smem_u32(sP), v_addr = smem_u32(sV);
-      const int ksteps = p.Tpad / 16;
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const uint64_t da = make_smem_desc_sw128(p_addr + (ks >> 2) * 16384 + (ks & 3) * 32, 16, 1024);
-        const uint64_t db = make_smem_desc_sw128(v_addr + ks * 2048, 8192, 1024);
-        umma_f16(tmem_base, da, db, idesc_o, ks > 0 ? 1u : 0u);  // O reuses the TMEM columns S has vacated
-      }
-      umma_commit(bar_o);
-    }
-  } else {
-    // ---------------- soft-max / epilogue: thread = query row
-    const int row = warp_idx * 32 + lane;
-    const int t = mb * 128 + row;
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp_idx * 32) << 16);
-    mbar_wait(bar_s, 0);
-    tc_fence_after();
-    const int nfull = p.Tpad / 32;          // 32-column chunks
-    const bool tail16 = (p.Tpad & 31) != 0;  // one extra 16-column chunk
-    float mx = -INFINITY;
-    for (int c = 0; c < nfull; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32(taddr + c * 32, v);
-      tmem_ld_wait();
-      if (c * 32 + 32 <= p.T) {   // warp-uniform: only the chunk that crosses T needs per-column masks
-#pragma unroll
-        for (int j = 0; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if (c * 32 + j < p.T) mx = fmaxf(mx, __uint_as_float(v[j]));
-      }
-    }
-    if (tail16) {
-      uint32_t v[16];
-      tmem_ld_32x16(taddr + nfull * 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-        if (nfull * 32 + j < p.T) mx = fmaxf(mx, __uint_as_float(v[j]));
-    }
-    const float mxs = mx * p.scale_log2e;
-    float sum = 0.f;
-    // second pass: exponentiate, accumulate the row sum, write P (bf16, unnormalised) into the swizzled K-major tile.
-    // (Q and K are dead once bar_s has fired, so P may overwrite them.)
-    auto emit = [&](const uint32_t* v, int col0, int n) {
-      // n is 32 or 16; col0 multiple of 16
-      const bool crosses = col0 + n > p.T;   // warp-uniform
-      for (int g = 0; g < n / 8; ++g) {
-        float e[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) e[j] = attn_ex2(fmaf(__uint_as_float(v[g * 8 + j]), p.scale_log2e, -mxs));
-        if (crosses) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (col0 + g * 8 + j >= p.T) e[j] = 0.f;
-        }
-        uint4 w;
-        w.x = pack_bf16x2(e[0], e[1]);
-        w.y = pack_bf16x2(e[2], e[3]);
-        w.z = pack_bf16x2(e[4], e[5]);
-        w.w = pack_bf16x2(e[6], e[7]);
-        // the row sum must match what the tensor core will see: accumulate the bf16-rounded values
-        sum += bf16_lo(w.x) + bf16_hi(w.x) + bf16_lo(w.y) + bf16_hi(w.y) + bf16_lo(w.z) + bf16_hi(w.z) + bf16_lo(w.w) +
-               bf16_hi(w.w);
-        const int col = col0 + g * 8;
-        const int kb = col >> 6, chunk = (col & 63) >> 3;
-        *reinterpret_cast<uint4*>(sP + kb * 16384 + row * 128 + ((chunk ^ (row & 7)) << 4)) = w;
-      }
-    };
-    for (int c = 0; c < nfull; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32(taddr + c * 32, v);
-      tmem_ld_wait();
-      emit(v, c * 32, 32);
-    }
-    if (tail16) {
-      uint32_t v[16];
-      tmem_ld_32x16(taddr + nfull * 32, v);
-      tmem_ld_wait();
-      emit(v, nfull * 32, 16);
-    }
-    tc_fence_before();
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_p);
-    // ---- epilogue: O / sum -> bf16 -> staging (P block 3 region is free: O MMA done) -> TMA store
-    mbar_wait(bar_o, 0);
-    tc_fence_after();
-    const float inv = 1.0f / sum;
-    uint8_t* stg = sP;  // all P blocks are dead once bar_o has fired
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32(taddr + c * 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint4 w;
-        w.x = pack_bf16x2(__uint_as_float(v[g * 8 + 0]) * inv, __uint_as_float(v[g * 8 + 1]) * inv);
-        w.y = pack_bf16x2(__uint_as_float(v[g * 8 + 2]) * inv, __uint_as_float(v[g * 8 + 3]) * inv);
-        w.z = pack_bf16x2(__uint_as_float(v[g * 8 + 4]) * inv, __uint_as_float(v[g * 8 + 5]) * inv);
-        w.w = pack_bf16x2(__uint_as_float(v[g * 8 + 6]) * inv, __uint_as_float(v[g * 8 + 7]) * inv);
-        const int chunk = c * 4 + g;
-        *reinterpret_cast<uint4*>(stg + row * 128 + ((chunk ^ (row & 7)) << 4)) = w;
-      }
-    }
-    if (t < p.T && p.lse != nullptr)
-      p.lse[(static_cast<long long>(b) * p.H + h) * p.T + t] = mx * p.scale + logf(sum);
-    tc_fence_before();
-    fence_proxy_async_smem();
-    named_bar_sync(1, 128);
-    if (threadIdx.x == 0) {
-      tma_store_3d(&p.o_map, stg, h * 64, mb * 128, b);
-      tma_store_commit();
-      tma_store_wait_all<0>();
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 4) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
-  }
-}
 
 }  // namespace b200
 
 namespace b200 {
 
 // ------------------------------------------------------------------------------------------------------------------
-// Backward: attention_bwd.cuh (attn_bwd_kernel, two CTAs per SM); the row term delta_i = sum_d dO[i,d] O[i,d] it needs is
+// Backward: attention_bwd.cuh (attn_bwd_kernel); the row term delta_i = sum_d dO[i,d] O[i,d] it needs is
 // produced by attn_delta_kernel below.
 
 // delta[b][h][t] = sum_d dO[b,t,h,d] * O[b,t,h,d].  Eight lanes per (b,t,h) row (one 16-byte vector of dO and of O each, the

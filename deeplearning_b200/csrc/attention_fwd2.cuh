@@ -1,284 +1,196 @@
-// Multi-head self-attention forward, persistent version (T <= 256 tokens, head dim 64) - same math, operands and outputs as
-// attn_fwd_kernel (attention.cuh), which stays in the library as the reference implementation of the op.
+// Multi-head self-attention forward for short sequences (T <= 256 tokens, head dim 64), persistent, with wgmma:
 //
-// attn_fwd_kernel is one short-lived CTA per (batch, head, 128-query block): TMEM allocation, barrier set-up, an exposed TMA
-// round trip for Q / K / V and a strictly serial S -> soft-max -> PV -> store chain per CTA, with only the second resident
-// CTA to overlap with (TMEM: 256 columns each, so never more than two).  A ViT-B/16 layer at bs 256 is 6144 such CTAs:
-// 153 us, 1.9 TB/s of DRAM traffic and ~200 TFLOP/s - bound by none of the machine's limits, only by those latencies.
+//   O[b, t, h, :] = softmax_j( scale * Q[b,t,h,:] . K[b,j,h,:] ) V[b,j,h,:]
 //
-// Here ONE CTA per SM walks (batch, head) items:
-//   * K and V of an item are fetched once and shared by both query blocks (the per-block CTAs each fetched their own copy);
-//   * a producer warp prefetches: Q / K of item i+1 land while item i is in its soft-max (they are dead as soon as both
-//     S = Q K^T products have retired), V of item i+1 as soon as the PV products of item i have retired;
-//   * the two query blocks are two independent chains - their own soft-max warp group (4 warps), MMA-issuing warp, TMEM
-//     columns (S / O of block g at columns g*256) and P buffer - so one block's MMAs and stores overlap the other's soft-max;
-//   * set-up (TMEM allocation, barrier init, descriptor prefetch) is paid once per SM instead of 41 times.
+// ONE CTA per SM walks (batch, head) items:
+//   * a producer warp fetches Q (both 128-query blocks) and K of an item, and V, with TMA (rows beyond T are zero-filled);
+//     Q / K of item i+1 land as soon as every S product of item i has retired, V once its P V products have;
+//   * query block g is owned by warpgroup 1 + g, which works through its 128 rows as two 64-row halves:
+//     S = Q K^T (m64 x NT keys, K = 64) in registers, the soft-max on the accumulator fragment (a row lives in the four
+//     lanes of a quad: two shuffles per row reduction), P as bf16 into the 128B-swizzled K-major layout, O = P V (V used in
+//     place as an MN-major operand), O / rowsum -> bf16 -> staging -> one TMA store per block;
+//   * S / P never touch HBM; only the per-row log-sum-exp is kept for the backward pass.
 //
-// Shared memory: Q 2 x 16 KB, K 32 KB, V 32 KB, P 2 x 64 KB (bf16, key-blocked 128B-swizzled K-major: the A operand of
-// O = P V; its first 16 KB double as the O staging slab of the TMA store) = 224 KB.  Warps 0-3 / 4-7: soft-max groups of
-// query block 0 / 1 (thread = query row, TMEM lane = row), warp 8: TMA producer, warps 9 / 10: MMA issuers of block 0 / 1.
+// Shared memory: Q 2 x 16 KB, K 32 KB, V 32 KB, P 2 x 64 KB (the first 16 KB of a block's P double as its O staging slab).
 //
-// The single-lane producer / issuer roles wait with a 40 ns back-off (a third of all issued instructions of the first version
-// were their mbarrier polls: profiles/r02_attn_fwd2_ncu.md).
-//
-// Replaces the eager sequence of vit_model.py:95-108 (classification/vision_transformer), as attn_fwd_kernel does.
+// Replaces the eager sequence of vit_model.py:95-108 (classification/vision_transformer): qkv split, (q@k^T)*scale, softmax,
+// attn@v, transpose/reshape, which materialises the [B,12,197,197] score tensor three times in HBM.
 #pragma once
 #include "attention.cuh"
 
 namespace b200 {
 
 constexpr int kAttn2SmemBytes = 2 * 16384 /*Q*/ + 32768 /*K*/ + 32768 /*V*/ + 2 * 65536 /*P*/ + 256 + 1024;
-constexpr int kAttn2Threads = 11 * 32;
+constexpr int kAttn2Threads = 384;   // warpgroup 0: TMA producer (warp 0), warpgroups 1-2: query blocks 0 / 1
+static_assert(kAttn2SmemBytes <= 227 * 1024, "shared memory of one H100 block");
 
+// NT = the key tile (p.Tpad: T rounded up to 64, <= 256)
+template <int NT>
 __global__ void __launch_bounds__(kAttn2Threads, 1) attn_fwd2_kernel(const __grid_constant__ AttnFwdParams p) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                       // [2][128][128B]
-  uint8_t* sK = smem + 32768;               // [Tpad][128B]
-  uint8_t* sV = smem + 65536;               // [Tpad][128B]
+  uint8_t* sK = smem + 32768;               // [NT][128B]
+  uint8_t* sV = smem + 65536;               // [NT][128B]
   uint8_t* sP = smem + 98304;               // [2 blocks][4 key blocks][128][128B]
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 98304 + 131072);
   uint64_t* bar_qk_full = bars + 0;         // Q (all blocks) and K of the current item landed
-  uint64_t* bar_qk_empty = bars + 1;        // every block's S MMAs retired: Q / K may be overwritten   (count = mblocks)
+  uint64_t* bar_qk_empty = bars + 1;        // every block's S products retired: Q / K may be overwritten (count = mblocks)
   uint64_t* bar_v_full = bars + 2;
-  uint64_t* bar_v_empty = bars + 3;         // every block's PV MMAs retired                              (count = mblocks)
-  uint64_t* bar_s = bars + 4;               // [2] S of block g complete in TMEM
-  uint64_t* bar_p = bars + 6;               // [2] P of block g complete in shared memory               (4 warp arrivals)
-  uint64_t* bar_o = bars + 8;               // [2] O of block g complete in TMEM
-  uint64_t* bar_free = bars + 10;           // [2] block g has read O out of TMEM: columns reusable       (4 warp arrivals)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 12);
+  uint64_t* bar_v_empty = bars + 3;         // every block's P V products retired                           (count = mblocks)
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int items = p.B * p.H;
   const int HD = p.H * 64;
   const int mblocks = p.mblocks;
 
-  if (warp_idx == 8) {
-    if (lane == 0) {
-      tma_prefetch_desc(&p.q_map);
-      tma_prefetch_desc(&p.kv_map);
-      tma_prefetch_desc(&p.o_map);
-      mbar_init(bar_qk_full, 1);
-      mbar_init(bar_qk_empty, mblocks);
-      mbar_init(bar_v_full, 1);
-      mbar_init(bar_v_empty, mblocks);
-      for (int g = 0; g < 2; ++g) {
-        mbar_init(bar_s + g, 1);
-        mbar_init(bar_p + g, 4);
-        mbar_init(bar_o + g, 1);
-        mbar_init(bar_free + g, 4);
-      }
-      fence_mbar_init();
-    }
-    __syncwarp();
-    tmem_alloc<512>(tmem_ptr_smem);   // one CTA per SM (224 KB of shared memory): all 512 columns
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&p.q_map);
+    tma_prefetch_desc(&p.kv_map);
+    tma_prefetch_desc(&p.o_map);
+    mbar_init(bar_qk_full, 1);
+    mbar_init(bar_qk_empty, mblocks);
+    mbar_init(bar_v_full, 1);
+    mbar_init(bar_v_empty, mblocks);
+    fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp_idx == 8) {
+  if (warp_idx < 4) {
     // ---------------- TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       int it = 0;
       for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
         const int h = item % p.H, b = item / p.H;
         if (it > 0) mbar_wait_backoff(bar_qk_empty, (it - 1) & 1);
-        mbar_expect_tx(bar_qk_full, mblocks * 16384 + p.Tpad * 128);
+        mbar_expect_tx(bar_qk_full, mblocks * 16384 + NT * 128);
         for (int g = 0; g < mblocks; ++g) tma_load_3d(sQ + g * 16384, &p.q_map, bar_qk_full, h * 64, g * 128, b);
         tma_load_3d(sK, &p.kv_map, bar_qk_full, HD + h * 64, 0, b);
         if (it > 0) mbar_wait_backoff(bar_v_empty, (it - 1) & 1);
-        mbar_expect_tx(bar_v_full, p.Tpad * 128);
+        mbar_expect_tx(bar_v_full, NT * 128);
         tma_load_3d(sV, &p.kv_map, bar_v_full, 2 * HD + h * 64, 0, b);
       }
     }
-  } else if (warp_idx >= 9) {
-    // ---------------- MMA issuer of query block g
-    const int g = warp_idx - 9;
-    if (lane == 0 && g < mblocks) {
-      const uint32_t tmem_g = tmem_base + g * 256;
+  } else {
+    setmaxnreg_inc<232>();
+    const int g = (warp_idx >> 2) - 1;
+    if (g < mblocks) {
+      // ---------------- query block g: S -> soft-max -> P -> P V -> O, in two halves of 64 rows
+      const int t = threadIdx.x & 127;
+      const bool leader = t == 0;
+      const int r0 = 16 * (t >> 5) + (lane >> 2);   // fragment rows r0, r0 + 8 of a half
+      const int cq = 2 * (lane & 3);                // fragment column offset inside an 8-column group
+      uint8_t* sPg = sP + g * 65536;
       const uint32_t q_addr = smem_u32(sQ + g * 16384), k_addr = smem_u32(sK), v_addr = smem_u32(sV);
-      const uint32_t p_addr = smem_u32(sP + g * 65536);
-      const uint32_t idesc_s = make_idesc_bf16(128, p.Tpad, 0, 0);
-      const uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-      const int ksteps = p.Tpad / 16;
+      const uint32_t p_addr = smem_u32(sPg);
       int it = 0;
       for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
         const uint32_t ph = it & 1;
-        mbar_wait_backoff(bar_qk_full, ph);
-        if (it > 0) mbar_wait_backoff(bar_free + g, (it - 1) & 1);   // the previous item's O has left these TMEM columns
-        tc_fence_after();
-        // ---- S = Q K^T : A = Q block (K-major), B = K (K-major, N = Tpad key rows), K = 64 (4 steps)
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_f16(tmem_g, make_smem_desc_sw128(q_addr + k * 32, 16, 1024), make_smem_desc_sw128(k_addr + k * 32, 16, 1024),
-                   idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(bar_s + g);
-        umma_commit(bar_qk_empty);
-        // ---- O = P V : A = P (K-major, key blocks of 64), B = V (MN-major: rows = keys, 64 contiguous d), K = Tpad keys
-        mbar_wait_backoff(bar_v_full, ph);
-        mbar_wait_backoff(bar_p + g, ph);
-        tc_fence_after();
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const uint64_t da = make_smem_desc_sw128(p_addr + (ks >> 2) * 16384 + (ks & 3) * 32, 16, 1024);
-          const uint64_t db = make_smem_desc_sw128(v_addr + ks * 2048, 8192, 1024);
-          umma_f16(tmem_g, da, db, idesc_o, ks > 0 ? 1u : 0u);   // O reuses the first 64 columns S has vacated
+        const int h = item % p.H, b = item / p.H;
+        // The first 16 KB of this block's P buffer were the staging slab of the previous item's O store: that store must
+        // have finished READING shared memory before P is written again.
+        if (it > 0) {
+          if (leader) tma_store_wait_read<0>();
+          named_bar_sync(2 + g, 128);
         }
-        umma_commit(bar_o + g);
-        umma_commit(bar_v_empty);
-      }
-    }
-  } else if ((warp_idx >> 2) < mblocks) {
-    // ---------------- soft-max / epilogue group of query block g: thread = query row
-    const int g = warp_idx >> 2;
-    const int wq = warp_idx & 3;            // TMEM lane quadrant
-    const int row = wq * 32 + lane;
-    const int t = g * 128 + row;
-    const uint32_t taddr = tmem_base + g * 256 + (static_cast<uint32_t>(wq * 32) << 16);
-    uint8_t* sPg = sP + g * 65536;
-    const int nfull = p.Tpad / 32;           // 32-column chunks
-    const bool tail16 = (p.Tpad & 31) != 0;  // one extra 16-column chunk
-    // a warp whose 32 query rows all lie beyond T (ViT: rows 224-255 of the 197 tokens) only keeps the barrier protocol
-    // alive: its S / P / O rows are never stored (TMA clips them) and cannot leak into other rows of P V
-    const bool warp_live = g * 128 + wq * 32 < p.T;
-    const bool pingpong = mblocks == 2;
-    int it = 0;
-    for (int item = blockIdx.x; item < items; item += gridDim.x, ++it) {
-      const uint32_t ph = it & 1;
-      const int h = item % p.H, b = item / p.H;
-      mbar_wait(bar_s + g, ph);
-      tc_fence_after();
-      float mx = -INFINITY;
-      for (int c = 0; warp_live && c < nfull; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(taddr + c * 32, v);
-        tmem_ld_wait();
-        if (c * 32 + 32 <= p.T) {   // warp-uniform: only the chunk that crosses T needs per-column masks
+        mbar_wait(bar_qk_full, ph);
+#pragma unroll 1
+        for (int hf = 0; hf < 2; ++hf) {
+          // a half whose 64 query rows all lie beyond T only keeps the barrier protocol alive (TMA clips its O rows)
+          const bool live = g * 128 + hf * 64 < p.T;
+          float mx[2] = {-INFINITY, -INFINITY}, sum[2] = {0.f, 0.f};
+          if (live) {
+            float sacc[NT / 2];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
-        } else {
+            for (int i = 0; i < NT / 2; ++i) sacc[i] = 0.f;
+            wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (c * 32 + j < p.T) mx = fmaxf(mx, __uint_as_float(v[j]));
-        }
-      }
-      if (warp_live && tail16) {
-        uint32_t v[16];
-        tmem_ld_32x16(taddr + nfull * 32, v);
-        tmem_ld_wait();
+            for (int k = 0; k < 4; ++k)
+              Wgmma<NT, 0, 0>::mma(sacc, make_smem_desc_sw128(q_addr + hf * 8192 + k * 32, 16, 1024),
+                                   make_smem_desc_sw128(k_addr + k * 32, 16, 1024), 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_reg_fence(sacc);
+            // row maxima over the valid keys, then P = exp2(scale * log2e * s - max) (bf16, unnormalised), keys >= T zero
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
-          if (nfull * 32 + j < p.T) mx = fmaxf(mx, __uint_as_float(v[j]));
-      }
-      // The exponential pass is bound by the SM's MUFU rate: the two groups take turns at it (block 1 of item i after
-      // block 0 of item i, block 0 of item i+1 after block 1 of item i), so that one group's pass overlaps the other's
-      // MMA round trips, max pass and epilogue instead of both passes colliding and both waits idling the SM.
-      if (pingpong) {
-        if (g == 1)
-          mbar_wait(bar_p + 0, ph);
-        else if (it > 0)
-          mbar_wait(bar_p + 1, (it - 1) & 1);
-      }
-      // The first 16 KB of this block's P buffer were the staging slab of the previous item's O store: that store must have
-      // finished READING shared memory before P is written again (the PV MMAs that read the old P retired before bar_o).
-      if (it > 0) {
-        if (wq == 0 && lane == 0) tma_store_wait_read<0>();
-        named_bar_sync(1 + g, 128);
-      }
-      const float mxs = mx * p.scale_log2e;
-      float sum = 0.f;
-      // second pass: exponentiate, accumulate the row sum, write P (bf16, unnormalised) into the swizzled K-major tile
-      auto emit = [&](const uint32_t* v, int col0, int n) {
-        const bool crosses = col0 + n > p.T;   // warp-uniform
-        for (int q8 = 0; q8 < n / 8; ++q8) {
-          float e[8];
+            for (int j = 0; j < NT / 8; ++j) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) e[j] = attn_ex2(fmaf(__uint_as_float(v[q8 * 8 + j]), p.scale_log2e, -mxs));
-          if (crosses) {
+              for (int i = 0; i < 4; ++i) {
+                if (8 * j + cq + (i & 1) < p.T) mx[i >> 1] = fmaxf(mx[i >> 1], sacc[4 * j + i]);
+              }
+            }
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-              if (col0 + q8 * 8 + j >= p.T) e[j] = 0.f;
+            for (int hh = 0; hh < 2; ++hh) {
+              mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+              mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+            }
+            const float mxs[2] = {mx[0] * p.scale_log2e, mx[1] * p.scale_log2e};
+#pragma unroll
+            for (int j = 0; j < NT / 8; ++j) {
+#pragma unroll
+              for (int hh = 0; hh < 2; ++hh) {
+                const int c = 8 * j + cq;
+                const float e0 = c < p.T ? attn_ex2(fmaf(sacc[4 * j + 2 * hh], p.scale_log2e, -mxs[hh])) : 0.f;
+                const float e1 = c + 1 < p.T ? attn_ex2(fmaf(sacc[4 * j + 2 * hh + 1], p.scale_log2e, -mxs[hh])) : 0.f;
+                // row sum of the unrounded exponentials (differs from the sum of the bf16-rounded P the tensor core sees
+                // by ~2^-9 / sqrt(T) relative, far below the bf16 output)
+                sum[hh] += e0 + e1;
+                const int R = hf * 64 + r0 + 8 * hh;
+                *reinterpret_cast<uint32_t*>(sPg + (j >> 3) * 16384 + R * 128 + (((j & 7) ^ (R & 7)) << 4) + (lane & 3) * 4) =
+                    pack_bf16x2(e0, e1);
+              }
+            }
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              sum[hh] += __shfl_xor_sync(0xffffffffu, sum[hh], 1);
+              sum[hh] += __shfl_xor_sync(0xffffffffu, sum[hh], 2);
+            }
           }
-          uint4 w;
-          w.x = pack_bf16x2(e[0], e[1]);
-          w.y = pack_bf16x2(e[2], e[3]);
-          w.z = pack_bf16x2(e[4], e[5]);
-          w.w = pack_bf16x2(e[6], e[7]);
-          // row sum of the unrounded exponentials (attn_fwd_kernel sums the bf16-rounded values the tensor core sees, at
-          // three instructions per element; the two sums differ by ~2^-9 / sqrt(T) relative, far below the bf16 output)
-          sum += ((e[0] + e[1]) + (e[2] + e[3])) + ((e[4] + e[5]) + (e[6] + e[7]));
-          const int col = col0 + q8 * 8;
-          const int kb = col >> 6, chunk = (col & 63) >> 3;
-          *reinterpret_cast<uint4*>(sPg + kb * 16384 + row * 128 + ((chunk ^ (row & 7)) << 4)) = w;
+          if (hf == 1 && leader) mbar_arrive(bar_qk_empty);   // both S products of this block have retired
+          fence_proxy_async_smem();
+          named_bar_sync(2 + g, 128);   // P of this half complete
+          if (live) {
+            // ---- O = P V : A = P (K-major, key blocks of 64), B = V (MN-major: rows = keys, 64 contiguous d), K = NT keys
+            if (hf == 0) mbar_wait(bar_v_full, ph);
+            float o[32];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) o[i] = 0.f;
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < NT / 16; ++ks)
+              Wgmma<64, 0, 1>::mma(o, make_smem_desc_sw128(p_addr + (ks >> 2) * 16384 + hf * 8192 + (ks & 3) * 32, 16, 1024),
+                                   make_smem_desc_sw128(v_addr + ks * 2048, 8192, 1024), 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_reg_fence(o);
+            // O / sum -> bf16 -> staging rows of this half (their P rows in key block 0 have just been consumed)
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const float inv = 1.0f / sum[hh];
+              const int R = hf * 64 + r0 + 8 * hh;
+#pragma unroll
+              for (int j = 0; j < 8; ++j)
+                *reinterpret_cast<uint32_t*>(sPg + R * 128 + ((j ^ (R & 7)) << 4) + (lane & 3) * 4) =
+                    pack_bf16x2(o[4 * j + 2 * hh] * inv, o[4 * j + 2 * hh + 1] * inv);
+              const int tq = g * 128 + R;
+              if ((lane & 3) == 0 && tq < p.T && p.lse != nullptr)
+                p.lse[(static_cast<long long>(b) * p.H + h) * p.T + tq] = mx[hh] * p.scale + logf(sum[hh]);
+            }
+          }
         }
-      };
-      for (int c = 0; warp_live && c < nfull; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(taddr + c * 32, v);
-        tmem_ld_wait();
-        emit(v, c * 32, 32);
+        if (leader) mbar_arrive(bar_v_empty);   // both P V products of this block have retired
+        fence_proxy_async_smem();
+        named_bar_sync(2 + g, 128);
+        if (leader) {
+          tma_store_3d(&p.o_map, sPg, h * 64, g * 128, b);
+          tma_store_commit();
+        }
       }
-      if (warp_live && tail16) {
-        uint32_t v[16];
-        tmem_ld_32x16(taddr + nfull * 32, v);
-        tmem_ld_wait();
-        emit(v, nfull * 32, 16);
-      }
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p + g);
-      // ---- epilogue: O out of TMEM (the columns go back to the issuer at once), / sum -> bf16 -> staging -> TMA store
-      mbar_wait(bar_o + g, ph);
-      tc_fence_after();
-      uint32_t o0[32], o1[32];
-      if (warp_live) {
-        tmem_ld_32x32(taddr, o0);
-        tmem_ld_32x32(taddr + 32, o1);
-        tmem_ld_wait();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_free + g);
-      const float inv = 1.0f / sum;
-      uint8_t* stg = sPg;   // P is dead once bar_o has fired
-#pragma unroll
-      for (int q8 = 0; warp_live && q8 < 4; ++q8) {
-        uint4 w;
-        w.x = pack_bf16x2(__uint_as_float(o0[q8 * 8 + 0]) * inv, __uint_as_float(o0[q8 * 8 + 1]) * inv);
-        w.y = pack_bf16x2(__uint_as_float(o0[q8 * 8 + 2]) * inv, __uint_as_float(o0[q8 * 8 + 3]) * inv);
-        w.z = pack_bf16x2(__uint_as_float(o0[q8 * 8 + 4]) * inv, __uint_as_float(o0[q8 * 8 + 5]) * inv);
-        w.w = pack_bf16x2(__uint_as_float(o0[q8 * 8 + 6]) * inv, __uint_as_float(o0[q8 * 8 + 7]) * inv);
-        *reinterpret_cast<uint4*>(stg + row * 128 + ((q8 ^ (row & 7)) << 4)) = w;
-      }
-#pragma unroll
-      for (int q8 = 0; warp_live && q8 < 4; ++q8) {
-        uint4 w;
-        w.x = pack_bf16x2(__uint_as_float(o1[q8 * 8 + 0]) * inv, __uint_as_float(o1[q8 * 8 + 1]) * inv);
-        w.y = pack_bf16x2(__uint_as_float(o1[q8 * 8 + 2]) * inv, __uint_as_float(o1[q8 * 8 + 3]) * inv);
-        w.z = pack_bf16x2(__uint_as_float(o1[q8 * 8 + 4]) * inv, __uint_as_float(o1[q8 * 8 + 5]) * inv);
-        w.w = pack_bf16x2(__uint_as_float(o1[q8 * 8 + 6]) * inv, __uint_as_float(o1[q8 * 8 + 7]) * inv);
-        *reinterpret_cast<uint4*>(stg + row * 128 + (((4 + q8) ^ (row & 7)) << 4)) = w;
-      }
-      if (t < p.T && p.lse != nullptr)
-        p.lse[(static_cast<long long>(b) * p.H + h) * p.T + t] = mx * p.scale + logf(sum);
-      fence_proxy_async_smem();
-      named_bar_sync(1 + g, 128);
-      if (wq == 0 && lane == 0) {
-        tma_store_3d(&p.o_map, stg, h * 64, g * 128, b);
-        tma_store_commit();
-      }
+      if (leader) tma_store_wait_all<0>();
     }
-    if (wq == 0 && lane == 0) tma_store_wait_all<0>();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 8) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 

@@ -1,25 +1,25 @@
-// Shared device-side primitives for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM wrappers.
-// Everything here is inline PTX for Blackwell (compile with -gencode arch=compute_100a,code=sm_100a).
+// Shared device-side primitives for the sm_90a kernels: mbarrier, TMA, wgmma and the shared-memory accumulator image.
+// Everything here is inline PTX for Hopper (compile with -gencode arch=compute_90a,code=sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <cuda.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace b200 {
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;
 
 // ---- Programmatic dependent launch.  Every kernel of the library is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization (host_utils.h launch_pdl): the next kernel of the stream is scheduled
 // when the CTAs of its predecessor have finished, without waiting for the grid's completion / memory flush to be processed
-// by the launch path; its CTAs run their prologue (barrier init, TMEM allocation, descriptor prefetch) and then block in
+// by the launch path; its CTAs run their prologue (barrier init, descriptor prefetch) and then block in
 // pdl_wait() until the PREVIOUS kernel has completed and its memory is visible.  Every kernel executes the wait before it
 // touches global memory (and before it can exit), so completion stays transitive along the stream: the data dependencies
 // are exactly those of plain stream order, only launch latency and prologues overlap the predecessor's end.
-// Measured on B200, ResNet-50 step (same box, ms): plain launches 16.92; attribute + implicit trigger at grid completion
-// 16.70 (default); explicit griddepcontrol.launch_dependents right after the wait 17.14; at kernel entry 17.70 - dependents
-// scheduled early pile onto the SMs that drain first and unbalance the next grid, so no kernel triggers explicitly.
+// No kernel triggers its dependents explicitly: dependents scheduled early pile onto the SMs that drain first and unbalance
+// the next grid (B200_PDL_TRIGGER selects the other two placements for experiments).
 #ifndef B200_PDL_TRIGGER
 #define B200_PDL_TRIGGER 0   // 0: never (implicit at grid completion), 1: at kernel entry, 2: right after the wait
 #endif
@@ -101,7 +101,7 @@ __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
 }
-// packed fp32x2 arithmetic (Blackwell): two lanes of a 64-bit register
+// fp32x2 values in one 64-bit register: the arithmetic is per lane (the same IEEE fp32 results as two scalar operations)
 __device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -111,31 +111,29 @@ __device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  return f2_pack(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t f2_bcast(float c) { return f2_pack(c, c); }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  f2_unpack(a, a0, a1);
+  f2_unpack(b, b0, b1);
+  f2_unpack(c, c0, c1);
+  return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 // ---------------------------------------------------------------- proxies / fences
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -189,148 +187,78 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+// Every tensor-core kernel of the library follows one scheme: a warpgroup (128 threads, warps 4k .. 4k+3) issues
+// wgmma.mma_async for 64 rows of the tile (Wgmma<N, TA, TB>::mma of wgmma.cuh) with the fp32 accumulators in its registers.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate. One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// Register split of the warp-specialised kernels (384 threads: a TMA producer warpgroup and two consumer warpgroups): the
+// producer gives registers back, the consumers, which hold the accumulators, take them.
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+// the registers of an accumulator written by wgmma may only be read once wgmma_wait has retired it
+template <int R>
+__device__ __forceinline__ void wgmma_reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- CTA pairs (tcgen05 cta_group::2) - bring-up, see
-// conv_gemm.cuh kPair: two CTAs of a cluster compute one 256-row tile, each stages its own 128 rows of A and HALF of B.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same shared-memory offset in CTA 0 (the MMA leader) of the cluster
-__device__ __forceinline__ uint32_t mapa_leader(uint32_t local_addr) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(local_addr));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads of a CTA pair: the data lands in THIS CTA, the transaction bytes complete on the barrier at `bar_cluster_addr`
-__device__ __forceinline__ void tma_load_2d_2cta(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2cta(void* dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1,
-                                                 int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_dst) {   // the same warp of BOTH CTAs executes this
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// M = 256 across the pair (128 TMEM lanes in each CTA); issued by one thread of the leader CTA only
-__device__ __forceinline__ void umma_f16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive, once the MMAs issued so far have completed, on the barrier at this shared-memory offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  const uint16_t mask = 0x3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
 // Shared-memory matrix descriptor for a 128B-swizzled tile (rows of 128 bytes, 8-row swizzle atoms of 1024 B).
 //   K-major  : rows = M/N index, 128 B of K per row.   SBO = 1024 (next 8 rows), LBO unused.
 //   MN-major : rows = K index, 128 B (64 bf16) of M/N per row. SBO = 1024 (next 8 K rows),
 //              LBO = byte distance to the next 64-wide M/N atom.
-// Bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                         uint32_t sbo_bytes) {
+// Bits: [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [62,64) layout (1 = SWIZZLE_128B). Tiles are 1024-byte aligned, so
+// the base-offset field stays 0; a K step of 16 bf16 (32 B) inside the atom adds 2 to the address field.
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 accumulation.
-//  [4,6) c_format=1 (F32) | [7,10) a_format=1 (BF16) | [10,13) b_format=1 | [15] a_major | [16] b_major
-//  [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
+// ---------------------------------------------------------------- accumulator image in shared memory
+// The epilogues own one tile row per thread (32 consecutive columns at a time). A warpgroup hands its accumulator fragment
+// to them through a row-major fp32 image whose 16-byte chunks are XOR-swizzled by (row & 7) inside each 32-column group:
+// the 128-bit row reads of a warp are conflict-free, the 64-bit fragment stores cost two passes.
+__device__ __forceinline__ uint32_t img_addr(uint32_t img, int ld, int row, int col) {
+  return img + static_cast<uint32_t>(row * ld + (col & 3)) * 4u +
+         (static_cast<uint32_t>((col >> 2) ^ (row & 7)) << 4);
 }
+// fragment of an m64nN accumulator (wgmma.cuh layout) -> image rows row0 .. row0 + 63, columns col0 .. col0 + N - 1
+template <int N>
+__device__ __forceinline__ void acc_to_img(const float (&d)[N / 2], uint32_t img, int ld, int row0, int col0) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+  const int c = col0 + 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(img_addr(img, ld, r + 8 * h, c + 8 * j)),
+                   "f"(d[4 * j + 2 * h]), "f"(d[4 * j + 2 * h + 1])
+                   : "memory");
+  }
+}
+// one row, columns col .. col + 4 * CH - 1 (col a multiple of 32 for CH = 8, of 16 for CH = 4) -> v[]
+template <int CH>
+__device__ __forceinline__ void img_ld(uint32_t img, int ld, int row, int col, uint32_t (&v)[4 * CH]) {
+#pragma unroll
+  for (int c = 0; c < CH; ++c)
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v[4 * c]), "=r"(v[4 * c + 1]), "=r"(v[4 * c + 2]), "=r"(v[4 * c + 3])
+                 : "r"(img_addr(img, ld, row, col + 4 * c))
+                 : "memory");
+}
+__device__ __forceinline__ void img_ld32(uint32_t img, int ld, int row, int col, uint32_t (&v)[32]) { img_ld<8>(img, ld, row, col, v); }
+__device__ __forceinline__ void img_ld16(uint32_t img, int ld, int row, int col, uint32_t (&v)[16]) { img_ld<4>(img, ld, row, col, v); }
 
 // ---------------------------------------------------------------- misc
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

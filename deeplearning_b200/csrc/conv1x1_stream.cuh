@@ -1,4 +1,4 @@
-// Streaming 1x1-convolution GEMM for the HBM-bound "narrow K -> wide N" layers of a ResNet bottleneck (sm_100a):
+// Streaming 1x1-convolution GEMM for the HBM-bound "narrow K -> wide N" layers of a ResNet bottleneck (sm_90a):
 //
 //   out[P][N] = epilogue( A[P][K] * W[N][K]^T ),   K = 64, 128 or 256 (KB = 1, 2, 4 k-blocks), N a multiple of 256, P a multiple of 128
 //
@@ -8,16 +8,15 @@
 //                   the ReLU of the block input; the sums are sum(dz) of the previous block's BatchNorm backward
 //   kStreamAffine : out = acc * scale[n] + shift[n]                            downsample conv -> BatchNorm (no residual, no ReLU)
 //
-// These layers move 9 bytes of activations per byte of operand: per 128-pixel tile the tensor core needs ~512 clocks, HBM
-// ~7000.  The generic implicit-GEMM kernel (conv_gemm.cuh) runs them at ~3 TB/s because its epilogue fetches the residual
-// with per-lane LDG.128 (32 scattered rows per instruction, two column groups in flight) and spends ~10 instructions per
-// output value on predicates and register shuffling.  Here everything that touches HBM is a bulk tensor copy:
+// These layers move far more bytes of activations than they do arithmetic per byte, so everything that touches HBM is a bulk
+// tensor copy:
 //   * K <= 128: W (32 / 64 KB) is loaded ONCE per CTA and stays in shared memory (a CTA always works on the same 256-channel
 //     block) and the A tiles (16 / 32 KB) stream through a 4- / 2-deep TMA ring;  K = 256 (layer3): W no longer fits beside
 //     the slab rings, so (A, W) k-blocks of 16 + 32 KB stream through a 3-deep ring as in the generic kernel;
-//   * every epilogue warp (one per TMEM lane quadrant) prefetches its own 32-row x 64-channel residual / mask slabs by TMA
-//     into a private ring (no cross-warp synchronisation), two or three slabs ahead, reads them back with conflict-free
-//     128-bit shared loads, and stores its output slab by TMA;
+//   * two consumer warpgroups multiply 64 rows x 256 columns each with wgmma; the epilogue is elementwise, so it works on the
+//     accumulator fragment in place: every consumer warp owns 16 rows of the tile, prefetches its own 16-row x 64-channel
+//     residual / mask slabs by TMA into a private ring (no cross-warp synchronisation), two or three slabs ahead, and
+//     stores its output slab by TMA;
 //   * full tiles only: no row / column predicates anywhere.
 #pragma once
 #include "common.cuh"
@@ -29,14 +28,15 @@ enum : int { kStreamBnRelu = 0, kStreamMask = 1, kStreamAffine = 2 };
 struct alignas(64) StreamParams {
   CUtensorMap a_map;     // A   [P][K] bf16, box {64, 128}
   CUtensorMap b_map;     // W   [N][K] bf16, box {64, 256}
-  CUtensorMap out_map;   // out [P][N] bf16, box {64, 32}
-  CUtensorMap res_map;   // residual [P][N] bf16, box {64, 32}
-  CUtensorMap mask_map;  // kStreamMask: ReLU output whose zeros kill the gradient [P][N] bf16, box {64, 32}
+  CUtensorMap out_map;   // out [P][N] bf16, box {64, 16}
+  CUtensorMap res_map;   // residual [P][N] bf16, box {64, 16}
+  CUtensorMap mask_map;  // kStreamMask: ReLU output whose zeros kill the gradient [P][N] bf16, box {64, 16}
   int m_tiles, n_tiles;  // P / 128, N / 256
   int N;
   const float* scale;    // kStreamBnRelu: [N]
   const float* shift;
-  float* stats;          // kStreamMask: [gridDim.x / n_tiles * 4][2][N] (plane 0 = column sums of `out` as stored, plane 1 = 0)
+  float* stats;          // kStreamMask: [gridDim.x / n_tiles * 4][2][N] (plane 0 = column sums of `out` as stored, plane 1 = 0):
+                         // one row per 32-row quadrant of the tile, as conv_gemm_kernel writes them
 };
 
 template <int KB, int MODE>
@@ -46,15 +46,16 @@ struct StreamCfg {
   static constexpr int STAGES = STREAM_B ? 3 : (KB == 1 ? 4 : 2);
   static constexpr int B_BYTES = STREAM_B ? 0 : KB * 32768;
   static constexpr int NBUF = (KB >= 2 && (MODE == kStreamMask || STREAM_B)) ? 2 : 3;   // slabs in flight per warp and source
-  static constexpr int SLAB = 4096;                                        // 32 rows x 128 B
-  static constexpr int RES_BYTES = MODE == kStreamAffine ? 0 : 4 * NBUF * SLAB;
+  static constexpr int SLAB = 2048;                                        // 16 rows x 128 B
+  static constexpr int RES_BYTES = MODE == kStreamAffine ? 0 : 8 * NBUF * SLAB;
   static constexpr int MASK_BYTES = MODE == kStreamMask ? RES_BYTES : 0;
   static constexpr int OUT_SLABS = (STREAM_B && MODE == kStreamMask) ? 1 : 2;   // output slabs per warp (shared memory is full)
-  static constexpr int OUT_BYTES = 4 * OUT_SLABS * SLAB;
+  static constexpr int OUT_BYTES = 8 * OUT_SLABS * SLAB;
   static constexpr int COEF_BYTES = MODE != kStreamMask ? 2 * 256 * 4 : 0;
   static constexpr int BAR_BYTES = 512;
   static constexpr int SMEM_BYTES = B_BYTES + STAGES * A_STAGE + RES_BYTES + MASK_BYTES + OUT_BYTES + COEF_BYTES + BAR_BYTES + 1024;
-  static constexpr int THREADS = 192;   // warp 0: TMA producer, warp 1: MMA issuer, warps 2-5: epilogue (one per TMEM quadrant)
+  static constexpr int THREADS = 384;   // warpgroup 0: TMA producer (warp 0), warpgroups 1-2: consumers
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 };
 
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
@@ -70,7 +71,7 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src_
 }
 
 template <int KB, int MODE>
-__global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_constant__ StreamParams p) {
+__global__ void __launch_bounds__(384, 1) conv1x1_stream_kernel(const __grid_constant__ StreamParams p) {
   pdl_launch_dependents();
   using Cfg = StreamCfg<KB, MODE>;
   constexpr int STAGES = Cfg::STAGES, NBUF = Cfg::NBUF;
@@ -86,10 +87,7 @@ __global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_con
   uint64_t* a_full = bars;                        // [STAGES]
   uint64_t* a_empty = bars + STAGES;              // [STAGES]
   uint64_t* b_full = bars + 2 * STAGES;           // [1]
-  uint64_t* tmem_full = bars + 2 * STAGES + 1;    // [2]
-  uint64_t* tmem_empty = bars + 2 * STAGES + 3;   // [2]
-  uint64_t* slab_full = bars + 2 * STAGES + 5;    // [4 warps][NBUF]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 5 + 4 * NBUF);
+  uint64_t* slab_full = bars + 2 * STAGES + 1;    // [8 warps][NBUF]
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tile = blockIdx.x % p.n_tiles;
@@ -104,18 +102,13 @@ __global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_con
     if constexpr (MODE == kStreamMask) tma_prefetch_desc(&p.mask_map);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
+      mbar_init(&a_empty[i], 2);   // one arrive per consumer warpgroup
     }
     mbar_init(b_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
-    }
-    for (int i = 0; i < 4 * NBUF; ++i) mbar_init(&slab_full[i], 1);
+    for (int i = 0; i < 8 * NBUF; ++i) mbar_init(&slab_full[i], 1);
     fence_mbar_init();
   }
-  if (warp_idx == 1) tmem_alloc<512>(tmem_ptr_smem);
-  pdl_wait();   // everything above touched only this CTA's shared memory / TMEM and the kernel parameters
+  pdl_wait();   // everything above touched only this CTA's shared memory and the kernel parameters
   if constexpr (MODE != kStreamMask) {
     // this CTA's 256 scale / shift values (its channel block never changes)
     for (int i = threadIdx.x; i < 256; i += blockDim.x) {
@@ -123,14 +116,12 @@ __global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_con
       sCoef[256 + i] = __ldg(p.shift + n_tile * 256 + i);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp_idx == 0) {
-    // ===================== TMA producer: W once, then the A tiles =====================
-    if (lane == 0) {
+  if (warp_idx < 4) {
+    // ===================== TMA producer (warp 0): W once, then the A tiles =====================
+    setmaxnreg_dec<40>();
+    if (warp_idx == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       if constexpr (Cfg::STREAM_B) {
@@ -163,72 +154,29 @@ __global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_con
         }
       }
     }
-  } else if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(128, 256, 0, 0);
-      const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(sB), 16, 1024);
-      const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(sA), 16, 1024);
-      if constexpr (!Cfg::STREAM_B) mbar_wait_backoff(b_full, 0);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int t = 0; t < my_tiles; ++t) {
-        mbar_wait_backoff(&tmem_empty[acc], acc_phase ^ 1);
-        const uint32_t tmem_d = tmem_base + acc * 256;
-        if constexpr (Cfg::STREAM_B) {
-          for (int kb = 0; kb < KB; ++kb) {
-            mbar_wait_backoff(&a_full[stage], phase);
-            tc_fence_after();
-            const uint64_t da = desc_a0 + static_cast<uint64_t>((stage * Cfg::A_STAGE) >> 4);
-            const uint64_t db = da + static_cast<uint64_t>(16384 >> 4);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-            umma_commit(&a_empty[stage]);
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-        } else {
-          mbar_wait_backoff(&a_full[stage], phase);
-          tc_fence_after();
-#pragma unroll
-          for (int kb = 0; kb < KB; ++kb) {
-            const uint64_t da = desc_a0 + static_cast<uint64_t>((stage * Cfg::A_STAGE + kb * 16384) >> 4);
-            const uint64_t db = desc_b0 + static_cast<uint64_t>((kb * 32768) >> 4);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&a_empty[stage]);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
   } else {
-    // ===================== Epilogue: one warp per TMEM lane quadrant, private slab rings =====================
-    const int q = warp_idx & 3;
-    const int ew = warp_idx - 2;
+    // ===================== consumers: warpgroup wg multiplies rows 64 wg .. + 63, warp ew drains 16 of them ===============
+    setmaxnreg_inc<232>();
+    const int ew = warp_idx - 4;       // 0..7: rows 16 ew .. 16 ew + 15 of the tile
+    const int wg = ew >> 2;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(sB), 16, 1024);
+    const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(sA) + wg * 8192, 16, 1024);
     const uint32_t res_s = smem_u32(sRes + ew * NBUF * Cfg::SLAB);
     const uint32_t mask_s = smem_u32(sMask + ew * NBUF * Cfg::SLAB);
     const uint32_t out_s = smem_u32(sOut + ew * Cfg::OUT_SLABS * Cfg::SLAB);
     uint64_t* my_full = slab_full + ew * NBUF;
-    const uint32_t row_s = lane * 128;
-    const uint32_t sw = (lane & 7) << 4;
+    // the fragment element pair (row lane / 4 + 8 h, columns 8 jj + 2 (lane % 4) + {0, 1}) of a 64-column unit sits at
+    // byte frag_off + h * 1024 + ((jj ^ (lane / 4)) << 4) of a 16-row x 128 B swizzled slab
+    const uint32_t frag_off = (lane >> 2) * 128 + (lane & 3) * 4;
+    const uint32_t fsw = lane >> 2;
     const int col0 = n_tile * 256;
     const int total_units = my_tiles * 4;
     constexpr uint32_t kSlabTx = MODE == kStreamMask ? 2 * Cfg::SLAB : Cfg::SLAB;
 
     auto issue_unit = [&](int g) {   // lane 0: TMA loads of unit g (tile g / 4, 64-column unit g % 4) into ring slot g % NBUF
       const int slot = g % NBUF;
-      const int row = (m_first + (g >> 2) * m_step) * 128 + q * 32;
+      const int row = (m_first + (g >> 2) * m_step) * 128 + ew * 16;
       const int col = col0 + (g & 3) * 64;
       mbar_expect_tx(&my_full[slot], kSlabTx);
       tma_load_2d(reinterpret_cast<void*>(sRes + (ew * NBUF + slot) * Cfg::SLAB), &p.res_map, &my_full[slot], col, row);
@@ -245,15 +193,54 @@ __global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_con
 #pragma unroll
     for (int m = 0; m < 8; ++m) stat_off[m] = m * 128 + ((((lane >> 2) ^ m) << 4) | ((lane & 3) << 2));
     uint64_t run_s[4] = {0, 0, 0, 0};
+    if constexpr (!Cfg::STREAM_B) mbar_wait(b_full, 0);
 
-    int g = 0;
+    int g = 0, stage = 0;
+    uint32_t phase = 0;
     for (int t = 0; t < my_tiles; ++t) {
-      const int acc = t & 1;
-      const uint32_t acc_phase = (t >> 1) & 1;
-      const int row0 = (m_first + t * m_step) * 128 + q * 32;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + acc * 256 + (static_cast<uint32_t>(q * 32) << 16);
+      const int row0 = (m_first + t * m_step) * 128 + ew * 16;
+      float acc[128];
+#pragma unroll
+      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      if constexpr (Cfg::STREAM_B) {
+        int prev = -1;
+        for (int kb = 0; kb < KB; ++kb) {
+          mbar_wait(&a_full[stage], phase);
+          wgmma_fence();
+          const uint64_t da = desc_a0 + static_cast<uint64_t>((stage * Cfg::A_STAGE) >> 4);
+          const uint64_t db = da - static_cast<uint64_t>((wg * 8192) >> 4) + static_cast<uint64_t>(16384 >> 4);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) Wgmma<256, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && leader) mbar_arrive(&a_empty[prev]);
+          prev = stage;
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        if (leader) mbar_arrive(&a_empty[prev]);
+      } else {
+        mbar_wait(&a_full[stage], phase);
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < KB; ++kb) {
+          const uint64_t da = desc_a0 + static_cast<uint64_t>((stage * Cfg::A_STAGE + kb * 16384) >> 4);
+          const uint64_t db = desc_b0 + static_cast<uint64_t>((kb * 32768) >> 4);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) Wgmma<256, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (leader) mbar_arrive(&a_empty[stage]);
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_reg_fence(acc);
 #pragma unroll
       for (int u = 0; u < 4; ++u, ++g) {
         const int slot = g % NBUF;
@@ -267,56 +254,36 @@ __global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_con
         __syncwarp();
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_acc + u * 64 + h * 32, v);
-          uint4 r4[4], m4[4];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if constexpr (MODE != kStreamAffine) r4[j] = lds128(rs + row_s + (((h * 4 + j) << 4) ^ sw));
-            else r4[j] = make_uint4(0u, 0u, 0u, 0u);
-            if constexpr (MODE == kStreamMask) m4[j] = lds128(ms + row_s + (((h * 4 + j) << 4) ^ sw));
-          }
-          tmem_ld_wait();
-          if (u == 3 && h == 1) {
-            // every TMEM read of this accumulator by this warp is done: hand it back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t rw[4] = {r4[j].x, r4[j].y, r4[j].z, r4[j].w};
-            uint32_t ow[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              float f0 = __uint_as_float(v[j * 8 + 2 * i]), f1 = __uint_as_float(v[j * 8 + 2 * i + 1]);
-              if constexpr (MODE == kStreamBnRelu) {
-                const int c = u * 64 + h * 32 + j * 8 + 2 * i;
-                const float2 sc = *reinterpret_cast<const float2*>(sCoef + c);
-                const float2 sh = *reinterpret_cast<const float2*>(sCoef + 256 + c);
-                f0 = fmaxf(fmaf(f0, sc.x, sh.x) + bf16_lo(rw[i]), 0.0f);
-                f1 = fmaxf(fmaf(f1, sc.y, sh.y) + bf16_hi(rw[i]), 0.0f);
-              } else if constexpr (MODE == kStreamAffine) {
-                const int c = u * 64 + h * 32 + j * 8 + 2 * i;
-                const float2 sc = *reinterpret_cast<const float2*>(sCoef + c);
-                const float2 sh = *reinterpret_cast<const float2*>(sCoef + 256 + c);
-                f0 = fmaf(f0, sc.x, sh.x);
-                f1 = fmaf(f1, sc.y, sh.y);
-              } else {
-                const uint32_t mw = i == 0 ? m4[j].x : (i == 1 ? m4[j].y : (i == 2 ? m4[j].z : m4[j].w));
-                f0 = (mw & 0x7fffu) ? f0 + bf16_lo(rw[i]) : 0.0f;
-                f1 = (mw & 0x7fff0000u) ? f1 + bf16_hi(rw[i]) : 0.0f;
-              }
-              ow[i] = pack_bf16x2(f0, f1);
+          for (int jj = 0; jj < 8; ++jj) {
+            const uint32_t off = frag_off + h * 1024 + ((jj ^ fsw) << 4);
+            const int j = u * 8 + jj;
+            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+            const uint32_t rw = MODE != kStreamAffine ? lds32(rs + off) : 0u;
+            const int c = u * 64 + jj * 8 + 2 * (lane & 3);
+            if constexpr (MODE == kStreamBnRelu) {
+              const float2 sc = *reinterpret_cast<const float2*>(sCoef + c);
+              const float2 sh = *reinterpret_cast<const float2*>(sCoef + 256 + c);
+              f0 = fmaxf(fmaf(f0, sc.x, sh.x) + bf16_lo(rw), 0.0f);
+              f1 = fmaxf(fmaf(f1, sc.y, sh.y) + bf16_hi(rw), 0.0f);
+            } else if constexpr (MODE == kStreamAffine) {
+              const float2 sc = *reinterpret_cast<const float2*>(sCoef + c);
+              const float2 sh = *reinterpret_cast<const float2*>(sCoef + 256 + c);
+              f0 = fmaf(f0, sc.x, sh.x);
+              f1 = fmaf(f1, sc.y, sh.y);
+            } else {
+              const uint32_t mw = lds32(ms + off);
+              f0 = (mw & 0x7fffu) ? f0 + bf16_lo(rw) : 0.0f;
+              f1 = (mw & 0x7fff0000u) ? f1 + bf16_hi(rw) : 0.0f;
             }
-            sts128(os + row_s + (((h * 4 + j) << 4) ^ sw), ow[0], ow[1], ow[2], ow[3]);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(os + off), "r"(pack_bf16x2(f0, f1)) : "memory");
           }
         }
         __syncwarp();
         if constexpr (MODE == kStreamMask) {
           uint64_t a_s = 0;
 #pragma unroll
-          for (int r = 0; r < 32; ++r) {
+          for (int r = 0; r < 16; ++r) {
             const uint32_t w = lds32(os + (r >> 3) * 1024 + stat_off[r & 7]);
             a_s = f2_add(a_s, f2_pack(bf16_lo(w), bf16_hi(w)));
           }
@@ -334,24 +301,32 @@ __global__ void __launch_bounds__(192, 1) conv1x1_stream_kernel(const __grid_con
       }
     }
     if constexpr (MODE == kStreamMask) {
-      const int srow = (blockIdx.x / p.n_tiles) * 4 + q;
+      // one statistics row per 32-row quadrant q = ew / 2: the two warps of a quadrant add up through the (now idle) residual
+      // ring of the odd warp (every slab loaded into it has been consumed: the loads were waited for)
+      float2* xch = reinterpret_cast<float2*>(sRes + (ew | 1) * NBUF * Cfg::SLAB);
+      if (ew & 1) {
 #pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        float lo, hi;
-        f2_unpack(run_s[u], lo, hi);
-        float* sp = p.stats + static_cast<long long>(srow) * 2 * p.N + col0 + u * 64 + 2 * lane;
-        *reinterpret_cast<float2*>(sp) = make_float2(lo, hi);
-        *reinterpret_cast<float2*>(sp + p.N) = make_float2(0.f, 0.f);
+        for (int u = 0; u < 4; ++u) {
+          float lo, hi;
+          f2_unpack(run_s[u], lo, hi);
+          xch[u * 32 + lane] = make_float2(lo, hi);
+        }
+      }
+      named_bar_sync(1, 256);
+      if (!(ew & 1)) {
+        const int srow = (blockIdx.x / p.n_tiles) * 4 + (ew >> 1);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          float lo, hi;
+          f2_unpack(run_s[u], lo, hi);
+          const float2 o = xch[u * 32 + lane];
+          float* sp = p.stats + static_cast<long long>(srow) * 2 * p.N + col0 + u * 64 + 2 * lane;
+          *reinterpret_cast<float2*>(sp) = make_float2(lo + o.x, hi + o.y);
+          *reinterpret_cast<float2*>(sp + p.N) = make_float2(0.f, 0.f);
+        }
       }
     }
     if (lane == 0) tma_store_wait_all<0>();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 

@@ -1,16 +1,18 @@
-// Implicit-GEMM convolution / linear forward kernel for sm_100a.
+// Implicit-GEMM convolution / linear forward kernel for sm_90a.
 //
 //   D[pixel, n] = sum_{tap, c} A_tap[pixel (+tap offset), c] * Wt[n, tap*Cin + c]        (bf16 in, fp32 accumulate)
 //
 // * A (activations, NHWC bf16) is fetched by TMA as 4-D boxes (64 channels x b1 x b2 x b3 pixels = 128 rows of 128 B,
-//   128B-swizzled) straight into the layout tcgen05.mma consumes (K-major). A filter tap is just a coordinate offset;
+//   128B-swizzled) straight into the layout wgmma consumes (K-major). A filter tap is just a coordinate offset;
 //   out-of-image pixels are zero-filled by the TMA unit, which is the convolution's zero padding. Stride-2 convolutions
 //   pass up to four "phase" views (even/odd rows x cols) of the input as separate tensor maps.
 // * B (weights, [Cout][taps*Cin] bf16) is a 2-D TMA box of BLOCK_N rows x 64 k.
-// * One elected thread issues tcgen05.mma (M=128, N=BLOCK_N, K=16) into a double-buffered TMEM accumulator, so the
-//   epilogue of tile i overlaps the main loop of tile i+1. The kernel is persistent: grid = min(tiles, #SM).
-// * Epilogue warps: tcgen05.ld -> (+bias, activation, +residual) -> bf16 -> swizzled smem staging -> TMA store, plus
-//   optional per-channel sum / sum-of-squares partials (train-mode BatchNorm statistics) per 128-row tile.
+// * Two consumer warpgroups each multiply 64 rows of the 128-row tile with wgmma (m64 x BLOCK_N x k16) into registers; the
+//   TMA producer (warpgroup 0) keeps a ring of k-block stages full, also while the consumers run the epilogue of the previous tile.
+//   The kernel is persistent: grid = min(tiles, #SM).
+// * Epilogue: each warpgroup stores its accumulator into a shared-memory image and its four warps drain it one row per
+//   thread: (+bias, activation, +residual) -> bf16 -> swizzled smem staging -> TMA store, plus optional per-channel sum /
+//   sum-of-squares partials (train-mode BatchNorm statistics).
 //
 // Replaces the cuDNN/cuBLAS calls behind nn.Conv2d / nn.Linear on the reference's hot path
 // (classification/resnet/models/networks.py:27-35,104-124; classification/vision_transformer/vit_model.py:95,109,127-133).
@@ -33,7 +35,7 @@ struct alignas(64) ConvGemmParams {
   int tiles1, tiles2, tiles3;
   int box1, box2, box3;
   int dim1, dim2, dim3;  // output pixel extents (row -> pixel mapping of the residual / aux / fp32 paths)
-  int qoff1[4], qoff2[4], qoff3[4];  // pixel offset of TMEM quadrant q's 32-row slab inside the tile box
+  int qoff1[4], qoff2[4], qoff3[4];  // pixel offset of quadrant q's 32-row slab (tile rows 32q ..) inside the tile box
   int n_tiles;
   int N;
   int8_t tap_map[kMaxTaps];  // which activation view (phase) the tap reads
@@ -54,9 +56,6 @@ struct alignas(64) ConvGemmParams {
   uint32_t desc_lbo, desc_sbo;  // K-major smem descriptor strides (bytes): 16 / 1024
   float* out_direct;        // direct fp32 output ([pixels][ld_out]) for tiny N (logits) or null
   long long ld_out;
-  // --- CTA-pair mode (kPair kernels only)
-  CUtensorMap b_map_half;   // weights with a 128-row box: each CTA of a pair stages half of the 256-column tile
-  int pair;                 // host-side: launch the kPair kernel
   // --- stochastic depth (generic epilogue only): per-SAMPLE multiplier applied after bias / act / colscale, before the
   // residual add: sample = flat output pixel / rows_per_sample  (drop_path of the reference: convNext/models/networks.py:11-26)
   const float* rowscale;
@@ -78,21 +77,22 @@ struct alignas(64) ConvGemmParams {
   const float* bn_shift;
 };
 
-template <int BLOCK_N, bool kPair = false>
+template <int BLOCK_N>
 struct ConvGemmCfg {
   static constexpr int BLOCK_M = 128;
   static constexpr int BLOCK_K = 64;
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_BYTES = (kPair ? BLOCK_N / 2 : BLOCK_N) * BLOCK_K * 2;   // a pair member stages half of B
-  static constexpr int STAGES = kPair ? 4 : ((BLOCK_N == 256) ? 3 : (BLOCK_N == 128 ? 4 : 6));
+  static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
+  static constexpr int STAGES = BLOCK_N == 128 ? 3 : 5;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int EPI_WARPS = 8;
   static constexpr int SLAB_BYTES = 32 * 128;                       // one warp's 32 rows x 128 B
   static constexpr int STAGING_BYTES = EPI_WARPS * 2 * SLAB_BYTES;  // double-buffered per warp
+  static constexpr int IMG_BYTES = BLOCK_M * BLOCK_N * 4;           // fp32 accumulator image
   static constexpr int BAR_BYTES = 256;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + BAR_BYTES + 1024;
-  static constexpr int TMEM_COLS = (2 * BLOCK_N <= 128) ? 128 : (2 * BLOCK_N <= 256 ? 256 : 512);
-  static constexpr int THREADS = 64 + EPI_WARPS * 32;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + IMG_BYTES + BAR_BYTES + 1024;
+  static constexpr int THREADS = 384;   // warpgroup 0: TMA producer, warpgroups 1-2: consumers
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 };
 
 // Exact-erf GELU (nn.GELU() of the reference: vit_model.py:121, swin_transformer.py:20, convNext/models/networks.py:84) with
@@ -124,8 +124,7 @@ __device__ __forceinline__ float gelu_erf_grad(float x) {
   return fmaf(x * 0.3989422804014327f, e, cdf);
 }
 
-// Two GELUs at once with packed fp32x2 arithmetic (FFMA2 / FMUL2 / FADD2: same IEEE fp32 results per lane, half the issue
-// slots): 10 instructions per element instead of 18 - the epilogue of the MLP GEMMs is instruction-issue bound.
+// Two GELUs at once on fp32x2 values (common.cuh f2_*: per-lane IEEE fp32 operations, the same results as the scalar version).
 // cdf = 0.5 + sign(x) * (0.5 - tail) replaces the compare / select of the scalar version.
 __device__ __forceinline__ void gelu_parts2(float x0, float x1, uint64_t& cdf, uint64_t& e) {
   const uint64_t az = f2_pack(fabsf(x0) * 0.70710678118654752f, fabsf(x1) * 0.70710678118654752f);
@@ -154,7 +153,7 @@ __device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
 // x <- GELU(x), g <- GELU'(x) = Phi(x) + x phi(x) for two values: the derivative shares the cdf / exp work of the value (two
 // more packed instructions), which is why the FORWARD GEMM of an MLP saves GELU'(pre) for the backward pass instead of the
 // pre-activation itself - the dgrad epilogue of the following layer then only multiplies (it used to re-evaluate the whole
-// erf polynomial per element and was instruction-issue bound: ViT-B/16 fc2 dgrad 282 us against 161 us for the same-size fc1 dgrad).
+// erf polynomial per element, which made that epilogue instruction-issue bound).
 __device__ __forceinline__ void gelu_erf_val_grad2(float& x0, float& x1, float& g0, float& g1) {
   uint64_t cdf, e;
   gelu_parts2(x0, x1, cdf, e);
@@ -187,45 +186,30 @@ constexpr int kEpiBias = 1, kEpiColscale = 2, kEpiActShift = 2 /* 2 bits */, kEp
               //               this gradient, which therefore needs no pass of its own (bn_bwd_reduce in elementwise.cuh)
               kEpiAffine = 2048, kEpiMask = 4096, kEpiBnMask = 8192;
 
-// kPair (validated on B200, default for the 256-wide linear layers, see abi_conv.cu gemm_pair_enabled()): the two CTAs of a cluster
-// compute one 256-pixel x 256-channel tile with tcgen05.mma.cta_group::2. Each CTA stages its own 128 pixels of A and HALF
-// of the B tile (32 KB instead of 48 KB of operands per k-block and SM), the leader (cluster rank 0) issues the MMAs for
-// both and commits to the barriers of both; every CTA drains its own 128 accumulator rows with the unchanged epilogue.
-template <int BLOCK_N, int EPI = kEpiGeneric, bool kPair = false>
-__global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
+template <int BLOCK_N, int EPI = kEpiGeneric>
+__global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   pdl_launch_dependents();
-  static_assert(!kPair || (BLOCK_N == 256 && EPI >= 0 && !(EPI & kEpiDirect)),
-                "pair mode: 256-wide tiles of the linear layers only");
-  using Cfg = ConvGemmCfg<BLOCK_N, kPair>;
+  static_assert(BLOCK_N == 64 || BLOCK_N == 128, "64- or 128-column tiles");
+  using Cfg = ConvGemmCfg<BLOCK_N>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_base = smem;
   uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
+  uint8_t* img = staging + Cfg::STAGING_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(img + Cfg::IMG_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int m_tiles = p.tiles1 * p.tiles2 * p.tiles3;
-  // pair mode: a work item is a PAIR of pixel tiles (2g, 2g + 1) x one channel block; CTA `cta_rank` owns pixel tile 2g + rank
-  const uint32_t cta_rank = kPair ? cluster_ctarank() : 0u;
-  const int num_tiles = (kPair ? (m_tiles + 1) / 2 : m_tiles) * p.n_tiles;
-  // (first work item / stride of this CTA: written as constant-folded ternaries in the loop headers so that the kPair = false
-  //  instantiations compile to exactly the code they had before the pair mode existed - checked by diffing the SASS)
-#define B200_TILE_FIRST (kPair ? (blockIdx.x >> 1) : blockIdx.x)
-#define B200_TILE_STEP (kPair ? (gridDim.x >> 1) : gridDim.x)
+  const int num_tiles = m_tiles * p.n_tiles;
   const int num_kb = p.var_taps ? p.kb_total : p.num_taps * p.k_blocks_per_tap;
-  // Epilogue work units: 64 bf16 (or 32 fp32) channels x one warp's 32 rows. Two warps share a TMEM lane quadrant and
+  // Epilogue work units: 64 bf16 (or 32 fp32) channels x one warp's 32 rows. Two warps share a 32-row quadrant and
   // take alternate units; with a single unit per tile the second warp of each pair has nothing to do.
   const int unit_cols = ((EPI < 0) ? (p.out_f32 != 0) : ((EPI & kEpiOutF32) != 0)) ? 32 : 64;
   const int units = BLOCK_N / unit_cols;
-  // (with one unit per tile the two warps of a pair alternate TILES instead: pair p drains accumulator buffer p)
-  const int arrivals_per_acc = units >= 2 ? 8 : 4;
 
   if (warp_idx == 0 && lane == 0) {
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&p.a_maps[i]);
@@ -233,42 +217,26 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
     tma_prefetch_desc(&p.d_map);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      // one arrive per epilogue warp that drains this buffer (pair mode: the leader's barrier also counts the peer's warps)
-      mbar_init(&tmem_empty[i], kPair ? 2 * arrivals_per_acc : arrivals_per_acc);
+      mbar_init(&empty_bar[i], 2);   // one arrive per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp_idx == 1) {
-    if constexpr (kPair)
-      tmem_alloc_2cta<Cfg::TMEM_COLS>(tmem_ptr_smem);
-    else
-      tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr_smem);
-  }
-  tc_fence_before();
-  if constexpr (kPair)
-    cluster_sync_all();   // the peer's barriers are initialised before any remote arrive / cross-CTA TMA completion
-  else
-    __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();   // everything above touched only this CTA's shared memory / TMEM and the kernel parameters
+  __syncthreads();
+  pdl_wait();   // everything above touched only this CTA's shared memory and the kernel parameters
 
-  if (warp_idx == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (warp_idx < 4) {
+    // ===================== TMA producer (warp 0 of warpgroup 0) =====================
+    setmaxnreg_dec<40>();
+    if (warp_idx == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       CPROF_DECL(2)
-      for (int tile = B200_TILE_FIRST; tile < num_tiles; tile += B200_TILE_STEP) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int n_tile = tile % p.n_tiles;
-        const int m_tile = kPair ? (tile / p.n_tiles) * 2 + static_cast<int>(cta_rank) : tile / p.n_tiles;
+        const int m_tile = tile / p.n_tiles;
         const int t1 = m_tile % p.tiles1;
         const int t2 = (m_tile / p.tiles1) % p.tiles2;
-        const int t3 = m_tile / (p.tiles1 * p.tiles2);   // (an odd tile count leaves the last peer tile past the tensor: zero fill)
+        const int t3 = m_tile / (p.tiles1 * p.tiles2);
         const int c1 = t1 * p.box1, c2 = t2 * p.box2, c3 = t3 * p.box3;
         int tap = 0, cb = 0;   // running (tap, channel block) of k-block kb: no division in the single-thread issue loop
         int kb_in_tap = p.var_taps ? p.tap_kb[0] : p.k_blocks_per_tap;
@@ -284,19 +252,10 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
           CPROF_TICK(0)
           uint8_t* a_dst = stage_base + stage * Cfg::STAGE_BYTES;
           uint8_t* b_dst = a_dst + Cfg::A_BYTES;
-          if constexpr (kPair) {
-            // the bytes of both CTAs complete on the LEADER's barrier, which alone gates the MMAs
-            const uint32_t full_leader = mapa_leader(smem_u32(&full_bar[stage]));
-            if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-            tma_load_4d_2cta(a_dst, &p.a_maps[p.tap_map[tap]], full_leader, cb * 64, c1 + p.tap_o1[tap], c2 + p.tap_o2[tap], c3);
-            tma_load_2d_2cta(b_dst, &p.b_map_half, full_leader, wk,
-                             n_tile * BLOCK_N + static_cast<int>(cta_rank) * (BLOCK_N / 2));
-          } else {
           mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
           tma_load_4d(a_dst, &p.a_maps[p.tap_map[tap]], &full_bar[stage], cb * 64, c1 + p.tap_o1[tap],
                       c2 + p.tap_o2[tap], c3);
           tma_load_2d(b_dst, &p.b_map, &full_bar[stage], wk, n_tile * BLOCK_N);
-          }
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
@@ -310,71 +269,22 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
       }
 #endif
     }
-  } else if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0 && cta_rank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(kPair ? 256 : 128, BLOCK_N, 0, 0);
-      // The shared-memory descriptors of all stages / K steps differ only in the 14-bit (address >> 4) field, so they are
-      // derived from two base descriptors with 64-bit adds: the one thread that issues every MMA of the CTA spends
-      // ~3 instructions per MMA instead of rebuilding two descriptors (what bounds the small-N tiles).
-      const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(stage_base), p.desc_lbo, p.desc_sbo);
-      const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(stage_base) + Cfg::A_BYTES, p.desc_lbo, p.desc_sbo);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      CPROF_DECL(3)
-      for (int tile = B200_TILE_FIRST; tile < num_tiles; tile += B200_TILE_STEP) {
-        CPROF_TICK(2)
-        mbar_wait_backoff(&tmem_empty[acc], acc_phase ^ 1);
-        CPROF_TICK(0)
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          CPROF_TICK(2)
-          mbar_wait_backoff(&full_bar[stage], phase);
-          CPROF_TICK(1)
-          tc_fence_after();
-          const uint64_t soff = static_cast<uint64_t>(stage) * (Cfg::STAGE_BYTES >> 4);
-          const uint64_t da = desc_a0 + soff, db = desc_b0 + soff;
-          if constexpr (kPair) {
-            umma_f16_2cta(tmem_d, da, db, idesc, kb > 0 ? 1u : 0u);
-#pragma unroll
-            for (int k = 1; k < 4; ++k) umma_f16_2cta(tmem_d, da + 2 * k, db + 2 * k, idesc, 1u);
-            umma_commit_2cta(&empty_bar[stage]);  // frees the slot in BOTH CTAs
-          } else {
-          umma_f16(tmem_d, da, db, idesc, kb > 0 ? 1u : 0u);
-#pragma unroll
-          for (int k = 1; k < 4; ++k) umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, 1u);   // +32 B per 16-element K step
-          umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs retire
-          }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if constexpr (kPair)
-          umma_commit_2cta(&tmem_full[acc]);  // wakes the epilogue warps of both CTAs
-        else
-          umma_commit(&tmem_full[acc]);  // accumulator complete
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-#ifdef CONV_PROFILE
-      if (blockIdx.x == 0) {
-        const int nt = (num_tiles - 1) / gridDim.x + 1;
-        printf("conv mma     : wait_tmem_empty %lld wait_full %lld issue %lld  (cycles/tile)\n", cp_t[0] / nt, cp_t[1] / nt, cp_t[2] / nt);
-      }
-#endif
-    }
   } else {
-    // ===================== Epilogue: 8 independent warps, no CTA-level barriers =====================
-    const int ew = warp_idx - 2;
-    const int q = warp_idx & 3;   // TMEM lane quadrant this warp may access
-    const int pair = ew >> 2;     // which of the two warps sharing the quadrant
+    // ===================== Two consumer warpgroups: wgmma main loop, then the epilogue of their 64 rows =====================
+    // Warpgroup wg owns tile rows 64 wg .. 64 wg + 63: it multiplies them into registers, hands the accumulator to its own
+    // four warps through the shared-memory image and drains it: warp `ew` owns the 32-row quadrant q (q = 2 wg, 2 wg + 1)
+    // and, with its partner warp of the same quadrant, alternate 64-column units.
+    setmaxnreg_inc<232>();
+    const int ew = warp_idx - 4;
+    const int wg = ew >> 2;
+    const int q = 2 * wg + (ew & 1);   // 32-row quadrant of the tile this warp drains
+    const int pair = (ew >> 1) & 1;    // which of the two warps sharing the quadrant
     const int row = q * 32 + lane;
+    const uint32_t img_s = smem_u32(img);
+    const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(stage_base) + wg * 8192, p.desc_lbo, p.desc_sbo);
+    const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(stage_base) + Cfg::A_BYTES, p.desc_lbo, p.desc_sbo);
+    int stage = 0;
+    uint32_t phase = 0;
     const uint32_t stage_s = smem_u32(staging + ew * 2 * Cfg::SLAB_BYTES);
     const uint32_t row_s = lane * 128;          // this thread's row inside a slab
     const uint32_t sw = (lane & 7) << 4;        // 128B-swizzle XOR term of that row
@@ -399,32 +309,56 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
     float* const out_direct = (G || (EPI & kEpiDirect)) ? p.out_direct : nullptr;
     float* const stats = (G || (EPI & (kEpiStats | kEpiBnMask))) ? p.stats : nullptr;
     const float* const rowscale = G ? p.rowscale : nullptr;
-    // (pair mode with an odd number of pixel tiles: the last peer tile lies past the tensor and must not touch memory)
     const bool need_rowmap = has_res || act == 3 || kMask || out_direct != nullptr || rowscale != nullptr || p.dim1 % p.box1 != 0 ||
-                             p.dim2 % p.box2 != 0 || p.dim3 % p.box3 != 0 || (kPair && (m_tiles & 1) != 0);
+                             p.dim2 % p.box2 != 0 || p.dim3 % p.box3 != 0;
     const bool full_cols = (N % BLOCK_N) == 0;  // no partially valid 32-column group anywhere
     uint32_t store_counter = 0;
-    const int nsub = out_f32 ? 1 : 2;  // 32-column TMEM loads per unit
+    const int nsub = out_f32 ? 1 : 2;  // 32-column image loads per unit
     const bool split_tiles = units < 2;  // single unit: the pair alternates tiles
     const int u_first = split_tiles ? 0 : pair;
-    int last_unit = u_first;
-    while (last_unit + 2 < units) last_unit += 2;
-    // Train-mode BN statistics: every epilogue warp keeps running column sums of the slabs it stored (its 32 TMEM lanes x
+    // Train-mode BN statistics: every epilogue warp keeps running column sums of the slabs it stored (its 32 rows x
     // its 64-column units; the launch guarantees grid % n_tiles == 0, so a CTA always sees the same channel block) and
-    // writes ONE partial row at the end of the kernel - ~150 x 4 rows per conv instead of one per 32 pixels.
+    // writes ONE partial row at the end of the kernel.
     constexpr int UN = BLOCK_N >= 128 ? BLOCK_N / 128 : 1;
     uint64_t run_s[UN], run_q[UN];
     float run_x[UN][2];   // kBnMask: sum(dz * x) of column (unit k, half h, lane)
 #pragma unroll
     for (int k = 0; k < UN; ++k) run_s[k] = 0, run_q[k] = 0, run_x[k][0] = run_x[k][1] = 0.f;
     int it = 0;
-    CPROF_DECL(2)
-    for (int tile = B200_TILE_FIRST; tile < num_tiles; tile += B200_TILE_STEP, ++it) {
+    CPROF_DECL(3)
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+      // ---- main loop: 64 rows x BLOCK_N of this warpgroup, K in 64-wide k-blocks of four wgmma K steps each
+      float acc[BLOCK_N / 2];
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;   // (also ends the live range of the previous tile's values)
+      int prev = -1;
+      CPROF_TICK(2)
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        wgmma_fence();
+        const uint64_t soff = static_cast<uint64_t>(stage) * (Cfg::STAGE_BYTES >> 4);
+        const uint64_t da = desc_a0 + soff, db = desc_b0 + soff;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) Wgmma<BLOCK_N, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, 1u);   // +32 B per 16-element K step
+        wgmma_commit();
+        wgmma_wait<1>();   // the k-block before this one has been read: release its slot
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      CPROF_TICK(0)
+      named_bar_sync(1 + wg, 128);   // this warpgroup's epilogue of the previous tile has read the image
+      acc_to_img<BLOCK_N>(acc, img_s, BLOCK_N, 64 * wg, 0);
+      named_bar_sync(1 + wg, 128);
       if (split_tiles && (it & 1) != pair) continue;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
       const int n_tile = tile % p.n_tiles;
-      const int m_tile = kPair ? (tile / p.n_tiles) * 2 + static_cast<int>(cta_rank) : tile / p.n_tiles;
+      const int m_tile = tile / p.n_tiles;
       const int t1 = m_tile % p.tiles1;
       const int t2 = (m_tile / p.tiles1) % p.tiles2;
       const int t3 = m_tile / (p.tiles1 * p.tiles2);
@@ -441,8 +375,8 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
       const int s1 = c1 + p.qoff1[q], s2 = c2 + p.qoff2[q], s3 = c3 + p.qoff3[q];
 
       // Global operands of the epilogue (residual / saved pre-activation) run ONE 32-column group ahead: the group's loads
-      // are issued while the previous group is converted and stored (the first one before the accumulator is even
-      // complete), so every epilogue warp always has 64-128 B per lane in flight towards HBM.
+      // are issued while the previous group is converted and stored, so every epilogue warp always has 64-128 B per lane in
+      // flight towards HBM.
       uint4 nx_b[4];   // bf16 residual or aux_in: 32 x bf16
       float4 nx_f[8];  // fp32 residual: 32 x fp32
       uint4 nx_m[4];   // kMask: 32 x bf16 of the mask tensor
@@ -478,12 +412,6 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
       };
       if (has_res || act == 3 || kMask) issue_pre(u_first, 0);
 
-      CPROF_TICK(1)
-      mbar_wait(&tmem_full[acc], acc_phase);
-      CPROF_TICK(0)
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + acc * BLOCK_N + (static_cast<uint32_t>(q * 32) << 16);
-
 #pragma unroll 1
       for (int u = u_first; u < units; u += 2) {
         const int n0 = n_tile * BLOCK_N + u * unit_cols;
@@ -500,7 +428,7 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
 #pragma unroll 1
         for (int h = 0; h < nsub; ++h) {
           uint32_t v[32];
-          tmem_ld_32x32(tmem_acc + u * unit_cols + h * 32, v);
+          img_ld32(img_s, BLOCK_N, row, u * unit_cols + h * 32, v);
           uint4 pre_b[4];
           float4 pre_f[8];
           uint4 pre_m[4];
@@ -517,18 +445,6 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
               issue_pre(u, h + 1);
             else if (u + 2 < units)
               issue_pre(u + 2, 0);
-          }
-          tmem_ld_wait();
-          if (u == last_unit && h == nsub - 1) {
-            // all TMEM reads of this accumulator by this warp are done -> hand it back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if constexpr (kPair)
-                mbar_arrive_cluster(mapa_leader(smem_u32(&tmem_empty[acc])));   // the leader's barrier gates the next MMAs
-              else
-                mbar_arrive(&tmem_empty[acc]);
-            }
           }
           if (!chunk_live) continue;
           const int nc = n0 + h * 32;  // first channel of this 32-column group
@@ -774,18 +690,15 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
       }
     }
 #ifdef CONV_PROFILE
-    CPROF_TICK(1)
     if (blockIdx.x == 0 && lane == 0 && (ew == 0 || ew == 4)) {
       const int nt = (num_tiles - 1) / gridDim.x + 1;
-      printf("conv epilogue warp %d: wait_tmem_full %lld work %lld  (cycles/tile)\n", ew, cp_t[0] / nt, cp_t[1] / nt);
+      printf("conv consumer warp %d: main loop %lld epilogue %lld  (cycles/tile)\n", ew, cp_t[0] / nt, cp_t[2] / nt);
     }
 #endif
     if (stats != nullptr) {
-      // (pair mode: the host keeps (gridDim.x / 2) % n_tiles == 0, so a CTA pair always works on channel block
-      //  (blockIdx.x >> 1) % n_tiles; each CTA of the pair owns its own 128 accumulator rows and writes its own partial rows)
-      const int cta = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
+      const int cta = static_cast<int>(blockIdx.x);
       const int n_tile = cta % p.n_tiles;
-      const int grp = kPair ? (cta / p.n_tiles) * 2 + static_cast<int>(cta_rank) : cta / p.n_tiles;
+      const int grp = cta / p.n_tiles;
       const int srow = split_tiles ? (grp * 4 + q) * 2 + pair : grp * 4 + q;
 #pragma unroll
       for (int k = 0; k < UN; ++k) {
@@ -809,21 +722,6 @@ __global__ void __launch_bounds__(320, 1) conv_gemm_kernel(const __grid_constant
     }
     if (lane == 0) tma_store_wait_all<0>();
   }
-
-  tc_fence_before();
-  if constexpr (kPair)
-    cluster_sync_all();   // neither CTA frees TMEM or exits while its peer can still reach its barriers / shared memory
-  else
-    __syncthreads();
-  if (warp_idx == 1) {
-    tc_fence_after();
-    if constexpr (kPair)
-      tmem_dealloc_2cta<Cfg::TMEM_COLS>(tmem_base);
-    else
-      tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
-#undef B200_TILE_FIRST
-#undef B200_TILE_STEP
 }
 
 }  // namespace b200

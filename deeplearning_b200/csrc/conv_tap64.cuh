@@ -6,35 +6,35 @@
 // These layers have N = 64 and K = 64 per tap: per 128-pixel tile the generic kernel (conv_gemm.cuh) streams 16 KB of
 // activations AND 8 KB of weights per tap through its ring, so a third of its L2 -> shared-memory traffic is the same
 // 72 KB of weights fetched again for every tile (the layer is L2-bound: nine taps re-read the activation tile).  Here the
-// taps' weight slices (<= 72 KB) are loaded once per CTA, the activation taps stream through a 6-deep ring of 16 KB slots,
-// four epilogue warps (one per TMEM lane quadrant, full tiles only: no predicates) convert, take the BatchNorm statistics
-// from the staged slab and store by TMA.  Same tensor maps, tap tables and statistics layout as conv_gemm_kernel: the host
-// code of b200_conv2d_fwd / b200_conv2d_dgrad / b200_stem_s2d_conv_fwd prepares ONE ConvGemmParams and dispatches here when
-// the shape qualifies (abi_conv.cu tap64_ok).
+// taps' weight slices (<= 72 KB) are loaded once per CTA, the activation taps stream through a 5-deep ring of 16 KB slots,
+// two consumer warpgroups multiply 64 rows each with wgmma (N = 64) and hand the accumulator to their warps through a shared-
+// memory image; the warps of quadrant q take alternate tiles, convert, take the BatchNorm statistics from the staged slab
+// and store by TMA (full tiles only: no predicates).  Same tensor maps, tap tables and statistics layout as
+// conv_gemm_kernel<64>: the host code of b200_conv2d_fwd / b200_conv2d_dgrad / b200_stem_s2d_conv_fwd prepares ONE
+// ConvGemmParams and dispatches here when the shape qualifies (abi_conv.cu tap64_ok).
 #pragma once
 #include "conv_gemm.cuh"
 
 namespace b200 {
 
-constexpr int kTap64Stages = 6;
-constexpr int kTap64SmemBytes = 9 * 8192 + kTap64Stages * 16384 + 4 * 2 * 4096 + 512 + 1024;
+constexpr int kTap64Stages = 5;
+constexpr int kTap64SmemBytes = 9 * 8192 + kTap64Stages * 16384 + 8 * 4096 + 128 * 64 * 4 + 512 + 1024;
+static_assert(kTap64SmemBytes <= 227 * 1024, "shared memory of one H100 block");
 
 template <bool kStats>
-__global__ void __launch_bounds__(192, 1) conv_tap64_kernel(const __grid_constant__ ConvGemmParams p) {
+__global__ void __launch_bounds__(384, 1) conv_tap64_kernel(const __grid_constant__ ConvGemmParams p) {
   pdl_launch_dependents();
   constexpr int STAGES = kTap64Stages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sB = smem;                         // [9 taps][64 rows x 128 B]
   uint8_t* sA = sB + 9 * 8192;                // ring of 128-pixel x 64-channel tap tiles
-  uint8_t* sOut = sA + STAGES * 16384;        // [4 warps][2][32 rows x 128 B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sOut + 4 * 2 * 4096);
+  uint8_t* sOut = sA + STAGES * 16384;        // [8 warps][32 rows x 128 B]
+  uint8_t* sImg = sOut + 8 * 4096;            // fp32 accumulator image [128][64]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sImg + 128 * 64 * 4);
   uint64_t* a_full = bars;                    // [STAGES]
   uint64_t* a_empty = bars + STAGES;          // [STAGES]
   uint64_t* b_full = bars + 2 * STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES + 1;    // [2]
-  uint64_t* tmem_empty = bars + 2 * STAGES + 3;   // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 5);
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tiles = p.tiles1 * p.tiles2 * p.tiles3;
@@ -46,25 +46,18 @@ __global__ void __launch_bounds__(192, 1) conv_tap64_kernel(const __grid_constan
     tma_prefetch_desc(&p.d_map);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
+      mbar_init(&a_empty[i], 2);   // one arrive per consumer warpgroup
     }
     mbar_init(b_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
-    }
     fence_mbar_init();
   }
-  if (warp_idx == 1) tmem_alloc<128>(tmem_ptr_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();   // everything above touched only this CTA's shared memory / TMEM and the kernel parameters
+  pdl_wait();   // everything above touched only this CTA's shared memory and the kernel parameters
 
-  if (warp_idx == 0) {
-    // ===================== TMA producer: the weight slices once, then the activation taps =====================
-    if (lane == 0) {
+  if (warp_idx < 4) {
+    // ===================== TMA producer (warp 0): the weight slices once, then the activation taps =====================
+    setmaxnreg_dec<40>();
+    if (warp_idx == 0 && lane == 0) {
       mbar_expect_tx(b_full, static_cast<uint32_t>(taps) * 8192u);
       for (int t = 0; t < taps; ++t) tma_load_2d(sB + t * 8192, &p.b_map, b_full, p.tap_w[t] * p.k_per_tap, 0);
       int stage = 0;
@@ -85,74 +78,66 @@ __global__ void __launch_bounds__(192, 1) conv_tap64_kernel(const __grid_constan
         }
       }
     }
-  } else if (warp_idx == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(128, 64, 0, 0);
-      const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(sA), p.desc_lbo, p.desc_sbo);
-      const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(sB), p.desc_lbo, p.desc_sbo);
-      mbar_wait_backoff(b_full, 0);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < m_tiles; tile += gridDim.x) {
-        mbar_wait_backoff(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * 64;
-        for (int t = 0; t < taps; ++t) {
-          mbar_wait_backoff(&a_full[stage], phase);
-          tc_fence_after();
-          const uint64_t da = desc_a0 + static_cast<uint64_t>(stage) * (16384 >> 4);
-          const uint64_t db = desc_b0 + static_cast<uint64_t>(t) * (8192 >> 4);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(tmem_d, da + 2 * k, db + 2 * k, idesc, (t > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&a_empty[stage]);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
   } else {
-    // ===================== Epilogue: one warp per TMEM lane quadrant =====================
-    const int q = warp_idx & 3;
-    const int ew = warp_idx - 2;
-    const uint32_t out_s = smem_u32(sOut + ew * 2 * 4096);
+    // ===================== Two consumer warpgroups (rows 64 wg ..): wgmma, then the epilogue of alternate tiles ===========
+    setmaxnreg_inc<232>();
+    const int ew = warp_idx - 4;
+    const int wg = ew >> 2;
+    const int q = 2 * wg + (ew & 1);   // 32-row quadrant of the tile
+    const int pair = (ew >> 1) & 1;    // the two warps of a quadrant take alternate tiles
+    const int row = q * 32 + lane;
+    const uint32_t img_s = smem_u32(sImg);
+    const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(sA) + wg * 8192, p.desc_lbo, p.desc_sbo);
+    const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(sB), p.desc_lbo, p.desc_sbo);
+    const uint32_t os = smem_u32(sOut + ew * 4096);
     const uint32_t row_s = lane * 128;
     const uint32_t sw = (lane & 7) << 4;
     uint32_t stat_off[8];
 #pragma unroll
     for (int m = 0; m < 8; ++m) stat_off[m] = m * 128 + ((((lane >> 2) ^ m) << 4) | ((lane & 3) << 2));
     uint64_t run_s = 0, run_q = 0;
+    mbar_wait(b_full, 0);
+    int stage = 0;
+    uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < m_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
+      float acc[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int t = 0; t < taps; ++t) {
+        mbar_wait(&a_full[stage], phase);
+        wgmma_fence();
+        const uint64_t da = desc_a0 + static_cast<uint64_t>(stage) * (16384 >> 4);
+        const uint64_t db = desc_b0 + static_cast<uint64_t>(t) * (8192 >> 4);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) Wgmma<64, 0, 0>::mma(acc, da + 2 * k, db + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&a_empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&a_empty[prev]);
+      named_bar_sync(1 + wg, 128);   // the previous tile's image has been read
+      acc_to_img<64>(acc, img_s, 64, 64 * wg, 0);
+      named_bar_sync(1 + wg, 128);
+      if ((it & 1) != pair) continue;
       const int t1 = tile % p.tiles1;
       const int t2 = (tile / p.tiles1) % p.tiles2;
       const int t3 = tile / (p.tiles1 * p.tiles2);
       const int s1 = t1 * p.box1 + p.qoff1[q], s2 = t2 * p.box2 + p.qoff2[q], s3 = t3 * p.box3 + p.qoff3[q];
-      const uint32_t os = out_s + (it & 1) * 4096;
-      if (lane == 0) tma_store_wait_read<1>();   // the store that used this slab two tiles ago has finished reading it
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
+      if (lane == 0) tma_store_wait_read<0>();   // this warp's previous store has finished reading the slab
       __syncwarp();
-      const uint32_t tmem_acc = tmem_base + acc * 64 + (static_cast<uint32_t>(q * 32) << 16);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         uint32_t v[32];
-        tmem_ld_32x32(tmem_acc + h * 32, v);
-        tmem_ld_wait();
-        if (h == 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        }
+        img_ld32(img_s, 64, row, h * 32, v);
 #pragma unroll
         for (int j = 0; j < 4; ++j)
           sts128(os + row_s + (((h * 4 + j) << 4) ^ sw),
@@ -186,25 +171,16 @@ __global__ void __launch_bounds__(192, 1) conv_tap64_kernel(const __grid_constan
       }
     }
     if constexpr (kStats) {
-      // the statistics layout of conv_gemm_kernel<64>: two partial rows per (CTA, quadrant) - this kernel fills the first
-      const long long srow = (static_cast<long long>(blockIdx.x) * 4 + q) * 2;
+      // the statistics layout of conv_gemm_kernel<64>: two partial rows per (CTA, quadrant), one per warp of the quadrant
+      const long long srow = (static_cast<long long>(blockIdx.x) * 4 + q) * 2 + pair;
       float s_lo, s_hi, q_lo, q_hi;
       f2_unpack(run_s, s_lo, s_hi);
       f2_unpack(run_q, q_lo, q_hi);
       float* sp = p.stats + srow * 2 * p.N + 2 * lane;
       *reinterpret_cast<float2*>(sp) = make_float2(s_lo, s_hi);
       *reinterpret_cast<float2*>(sp + p.N) = make_float2(q_lo, q_hi);
-      *reinterpret_cast<float2*>(sp + 2 * p.N) = make_float2(0.f, 0.f);
-      *reinterpret_cast<float2*>(sp + 3 * p.N) = make_float2(0.f, 0.f);
     }
     if (lane == 0) tma_store_wait_all<0>();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    tc_fence_after();
-    tmem_dealloc<128>(tmem_base);
   }
 }
 

@@ -101,8 +101,8 @@ int device_sm_count() {
   static int sms = 0;
   if (sms == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }

@@ -1,4 +1,4 @@
-// Weight-gradient GEMM for sm_100a:   dW[cout, tap, cin] = sum_pixels dY[pixel, cout] * X_tap[pixel (+tap offset), cin]
+// Weight-gradient GEMM for sm_90a:   dW[cout, tap, cin] = sum_pixels dY[pixel, cout] * X_tap[pixel (+tap offset), cin]
 //
 // The reduction runs over pixels, so both operands are "MN-major" for the tensor core: a TMA box of 64 pixels x 64 channels
 // (64 rows of 128 B, 128B swizzle) is exactly one canonical MN-major SWIZZLE_128B atom column (K = pixel rows). The same
@@ -8,7 +8,10 @@
 //
 // 64-channel inputs with several taps (ResNet layer1 3x3, the space-to-depth stem) run in MERGED-TAP mode: the 64-column
 // atoms of one B tile belong to DIFFERENT taps (same pixels, shifted TMA coordinates), so one dY tile feeds an N = 192 / 256
-// MMA instead of one N = 64 MMA per tap (tcgen05.mma costs ~100 cycles however small N is).
+// MMA instead of one N = 64 MMA per tap.
+//
+// Two consumer warpgroups multiply with wgmma (64 output channels each: one dY atom) and store their fp32 fragments straight
+// to the partial rows; warp 0 is the TMA producer.
 //
 // Replaces the cuDNN backward-filter / cuBLAS calls autograd issues for nn.Conv2d / nn.Linear in the reference
 // (loss.backward(): classification/resnet/utils.py:43).
@@ -38,7 +41,7 @@ struct alignas(64) WgradParams {
   uint32_t desc_lbo, desc_sbo, desc_kstep;  // MN-major smem descriptor strides (bytes): 8192 / 1024 / 2048
   // kBias kernels: per-split column sums of dY (= the bias gradient of the layer), [splits][2][Cout] (plane 0 = sums,
   // plane 1 = 0: the layout b200_bn_bwd_finalize folds).  The dY tiles are already in shared memory for the tensor core:
-  // four extra warps add up their rows, so the bias gradient costs no pass over dY (it used to be a separate HBM pass).
+  // the consumer warps add up their rows, so the bias gradient costs no pass over dY.
   float* bias_partial;
 };
 
@@ -51,11 +54,12 @@ struct WgradCfg {
   static constexpr int STAGES = (BLOCK_NG == 256) ? 4 : (BLOCK_NG == 192 ? 5 : (BLOCK_NG == 128 ? 6 : 8));
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;
-  static constexpr int TMEM_COLS = (2 * BLOCK_NG <= 128) ? 128 : (2 * BLOCK_NG <= 256 ? 256 : 512);
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 };
+constexpr int kWgradThreads = 384;   // warpgroup 0: TMA producer (warp 0), warpgroups 1-2: consumers
 
 template <int BLOCK_NG, bool kBias = false>
-__global__ void __launch_bounds__(kBias ? 320 : 192, 1) wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
+__global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
   pdl_launch_dependents();
   using Cfg = WgradCfg<BLOCK_NG>;
   constexpr int STAGES = Cfg::STAGES;
@@ -64,10 +68,7 @@ __global__ void __launch_bounds__(kBias ? 320 : 192, 1) wgrad_gemm_kernel(const 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  uint64_t* item_bar = bars + 2 * STAGES + 5;   // kBias: the MMA thread has reached the next item the column-sum warps read
+  __shared__ float bias_red[2][16][64];      // kBias: per-row-group column sums of the two dY atoms
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -80,24 +81,16 @@ __global__ void __launch_bounds__(kBias ? 320 : 192, 1) wgrad_gemm_kernel(const 
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&p.x_maps[i]);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kBias ? 5 : 1);   // the MMA commit (+ the four column-sum warps)
+      mbar_init(&empty_bar[i], kBias ? 8 : 2);   // one arrive per consumer warpgroup (kBias: per consumer warp)
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
-    }
-    mbar_init(item_bar, 1);
     fence_mbar_init();
   }
-  if (warp_idx == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr_smem);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();   // everything above touched only this CTA's shared memory / TMEM and the kernel parameters
+  pdl_wait();   // everything above touched only this CTA's shared memory and the kernel parameters
 
-  if (warp_idx == 0) {
-    if (lane == 0) {
+  if (warp_idx < 4) {
+    setmaxnreg_dec<40>();
+    if (warp_idx == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
@@ -144,76 +137,20 @@ __global__ void __launch_bounds__(kBias ? 320 : 192, 1) wgrad_gemm_kernel(const 
         }
       }
     }
-  } else if (warp_idx == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(128, BLOCK_NG, 1, 1);  // both operands MN-major
-      // descriptors of all stages / K steps by 64-bit adds on two base descriptors (see conv_gemm.cuh)
-      const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(smem), p.desc_lbo, p.desc_sbo);
-      const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(smem) + Cfg::A_BYTES, p.desc_lbo, p.desc_sbo);
-      const uint64_t kstep = p.desc_kstep >> 4;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        const int split = item / items_per_split;
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        bool summed = false;   // kBias: is this the item whose dY tiles the column-sum warps read?
-        if constexpr (kBias) {
-          int r = item - split * items_per_split;
-          const int tap = r % p.num_taps;
-          r /= p.num_taps;
-          summed = (r % p.ng_tiles) == 0 && tap == 0;
-        }
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        if constexpr (kBias) {
-          // every earlier tile has been consumed: the column-sum warps may now start waiting for this item's tiles (an
-          // mbarrier parity wait is only meaningful for a waiter that is less than one phase ahead of the pipeline)
-          if (summed) mbar_arrive(item_bar);
-        }
-        const uint32_t tmem_d = tmem_base + acc * BLOCK_NG;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if constexpr (kBias) {
-            if (!summed) {   // nobody else reads this tile: stand in for the four column-sum warps
-#pragma unroll
-              for (int i = 0; i < 4; ++i) mbar_arrive(&empty_bar[stage]);
-            }
-          }
-          // 16 pixel rows per MMA = 2048 B; LBO = next 64-channel atom (8192 B); SBO = next 8 pixel rows (1024 B)
-          const uint64_t soff = static_cast<uint64_t>(stage) * (Cfg::STAGE_BYTES >> 4);
-          const uint64_t da = desc_a0 + soff, db = desc_b0 + soff;
-          umma_f16(tmem_d, da, db, idesc, kb > kb0 ? 1u : 0u);
-#pragma unroll
-          for (int k = 1; k < 4; ++k) umma_f16(tmem_d, da + k * kstep, db + k * kstep, idesc, 1u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
-  } else if (kBias && warp_idx >= 6) {
-    // ===================== column sums of the dY tiles (bias gradient) =====================
-    // Only the (ng == 0, tap == 0) item of every (split, mg) pair is summed; for all other items the MMA thread supplies
-    // this role's four arrivals itself (below), so the pipeline of those items is untouched.
-    // The dY stage is 64 pixel rows x 2 atoms x 128 B: thread t of the 128 reads 8 rows of ONE 16-byte chunk (8 channels),
-    // chunk cc = t % 16 (atom cc / 8, chunk cc % 8 inside the 128-byte row, XOR-swizzled by row & 7), rows (t / 16) * 8 .. + 8.
-    __shared__ float bias_red[8][128];
-    const int t = (warp_idx - 6) * 32 + lane;
-    const int cc = t & 15, rg = t >> 4;
-    const uint32_t atom_off = static_cast<uint32_t>(cc >> 3) * 8192u;
+  } else {
+    // ===================== consumer warpgroups: rows (output channels) mg * 128 + 64 wg .. + 63 =====================
+    setmaxnreg_inc<232>();
+    const int wg = (warp_idx >> 2) - 1;
+    const bool leader = (threadIdx.x & 127) == 0;
+    // A = dY atom wg (64 output channels, MN-major), B = BLOCK_NG / 64 atoms of X (MN-major): 16 pixel rows per K step
+    const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(smem) + wg * 8192, p.desc_lbo, p.desc_sbo);
+    const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(smem) + Cfg::A_BYTES, p.desc_lbo, p.desc_sbo);
+    const uint64_t kstep = p.desc_kstep >> 4;
+    const int t = threadIdx.x & 127;
+    const int frow = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);   // fragment row of d[4j], d[4j+1]; d[4j+2..3]: + 8
+    const int fcol = 2 * (t & 3);
     int stage = 0;
-    uint32_t phase = 0, item_phase = 0;
+    uint32_t phase = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       const int split = item / items_per_split;
       int r = item - split * items_per_split;
@@ -223,106 +160,88 @@ __global__ void __launch_bounds__(kBias ? 320 : 192, 1) wgrad_gemm_kernel(const 
       const int mg = r / p.ng_tiles;
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-      if (!(ng == 0 && tap == 0)) {
-        // not ours: just keep the ring position in step
-        const int n = kb1 - kb0;
-        const int adv = stage + n;
-        phase ^= static_cast<uint32_t>((adv / STAGES) & 1);
-        stage = adv % STAGES;
-        continue;
-      }
-      float sum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      mbar_wait(item_bar, item_phase);   // the pipeline has reached this item
-      item_phase ^= 1;
+      // kBias: the (ng == 0, tap == 0) item of every (split, mg) pair also sums the columns of its dY tiles (the layer's bias
+      // gradient) while they are in shared memory for the tensor core: thread t of a warpgroup adds up 4 rows of ONE 16-byte
+      // chunk (8 channels) of its atom, chunk cc = t % 8 (XOR-swizzled by row & 7), rows (t / 8) * 4 .. + 4.
+      const bool summed = kBias && ng == 0 && tap == 0;
+      const int cc = t & 7, rg = t >> 3;
+      float bsum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      float acc[BLOCK_NG / 2];
+#pragma unroll
+      for (int i = 0; i < BLOCK_NG / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        const uint32_t base = smem_u32(smem + stage * Cfg::STAGE_BYTES) + atom_off;
-        uint4 v[8];
+        wgmma_fence();
+        const uint64_t soff = static_cast<uint64_t>(stage) * (Cfg::STAGE_BYTES >> 4);
+        const uint64_t da = desc_a0 + soff, db = desc_b0 + soff;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int row = rg * 8 + i;
-          v[i] = lds128(base + row * 128 + ((static_cast<uint32_t>(cc & 7) ^ static_cast<uint32_t>(row & 7)) << 4));
+        for (int k = 0; k < 4; ++k) Wgmma<BLOCK_NG, 1, 1>::mma(acc, da + k * kstep, db + k * kstep, 1u);
+        wgmma_commit();
+        if (summed) {
+          const uint32_t base = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * 8192;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int r = rg * 4 + i;
+            float f[8];
+            unpack8(lds128(base + r * 128 + ((static_cast<uint32_t>(cc) ^ static_cast<uint32_t>(r & 7)) << 4)), f);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) bsum[j] += f[j];
+          }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);   // the tile has been read
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          float f[8];
-          unpack8(v[i], f);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) sum[j] += f[j];
+        wgmma_wait<1>();   // the k-block before this one has been read: release its slot
+        if constexpr (kBias) {
+          __syncwarp();
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        } else {
+          if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
         }
+        prev = stage;
         if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
-      // fold the 8 row groups (fixed order: deterministic) and write this split's partial sums
-      named_bar_sync(2, 128);   // previous item's readers are done with bias_red
-#pragma unroll
-      for (int j = 0; j < 8; ++j) bias_red[rg][cc * 8 + j] = sum[j];
-      named_bar_sync(2, 128);
-      {
-        float tot = 0.f;
-#pragma unroll
-        for (int g2 = 0; g2 < 8; ++g2) tot += bias_red[g2][t];
-        const int cout = mg * 128 + t;
-        if (cout < p.Cout) {
-          p.bias_partial[(static_cast<long long>(split) * 2) * p.Cout + cout] = tot;
-          p.bias_partial[(static_cast<long long>(split) * 2 + 1) * p.Cout + cout] = 0.f;
-        }
-      }
-    }
-  } else {
-    const int q = warp_idx & 3;
-    const int row = q * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      const int split = item / items_per_split;
-      int r = item - split * items_per_split;
-      const int tap = r % p.num_taps;
-      r /= p.num_taps;
-      const int ng = r % p.ng_tiles;
-      const int mg = r / p.ng_tiles;
-      const int cout = mg * 128 + row;
-      float* out_row = p.partial + (static_cast<long long>(split) * p.Cout + cout) * p.ld_partial +
-                       static_cast<long long>(tap) * p.Cin + ng * BLOCK_NG;
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
       // (the host guarantees every split owns at least one pixel block)
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t tmem_acc = tmem_base + acc * BLOCK_NG + (static_cast<uint32_t>(q * 32) << 16);
-#pragma unroll 1
-      for (int ch = 0; ch < BLOCK_NG / 32; ++ch) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_acc + ch * 32, v);
-        tmem_ld_wait();
-        if (cout < p.Cout) {
-          const int cin0 = ng * BLOCK_NG + ch * 32;
+      if constexpr (kBias) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      } else {
+        if (leader) mbar_arrive(&empty_bar[prev]);
+      }
+      if (summed) {
+        // fold the 16 row groups (fixed order: deterministic) and write this split's partial sums
+        named_bar_sync(1 + wg, 128);   // the previous item's readers are done with bias_red
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            if (cin0 + j * 4 < p.n_cols) {  // a multiple of 8
-              uint4 w = make_uint4(v[j * 4], v[j * 4 + 1], v[j * 4 + 2], v[j * 4 + 3]);
-              *reinterpret_cast<uint4*>(out_row + ch * 32 + j * 4) = w;
-            }
+        for (int j = 0; j < 8; ++j) bias_red[wg][rg][cc * 8 + j] = bsum[j];
+        named_bar_sync(1 + wg, 128);
+        if (t < 64) {
+          float tot = 0.f;
+#pragma unroll
+          for (int g2 = 0; g2 < 16; ++g2) tot += bias_red[wg][g2][t];
+          const int cout = mg * 128 + wg * 64 + t;
+          if (cout < p.Cout) {
+            p.bias_partial[(static_cast<long long>(split) * 2) * p.Cout + cout] = tot;
+            p.bias_partial[(static_cast<long long>(split) * 2 + 1) * p.Cout + cout] = 0.f;
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
+      const int ncol = p.n_cols - ng * BLOCK_NG;   // valid columns of this tile (a multiple of 8)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int cout = mg * 128 + frow + 8 * h;
+        if (cout < p.Cout) {
+          float* out_row = p.partial + (static_cast<long long>(split) * p.Cout + cout) * p.ld_partial +
+                           static_cast<long long>(tap) * p.Cin + ng * BLOCK_NG;
+#pragma unroll
+          for (int j = 0; j < BLOCK_NG / 8; ++j)
+            if (8 * j + fcol < ncol)
+              *reinterpret_cast<float2*>(out_row + 8 * j + fcol) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 

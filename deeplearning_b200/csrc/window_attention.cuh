@@ -1,4 +1,4 @@
-// Shifted-window multi-head self-attention (Swin), head_dim 32, 7x7 windows (49 tokens), on tcgen05 - forward and backward.
+// Shifted-window multi-head self-attention (Swin), head_dim 32, 7x7 windows (49 tokens), with wgmma - forward and backward.
 //
 //   attn = softmax( scale * q k^T + relative_position_bias[h] (+ shift mask[window]) ) ;  out = attn v
 //
@@ -6,8 +6,8 @@
 // a window's 49 tokens are gathered with 16-byte cp.async copies straight from the un-rolled qkv tensor [B,H,W,3C]
 // (pixel ((wy*7+i+shift)%H, (wx*7+j+shift)%W)) into the 128B-swizzled operand layout, and the result rows are scattered
 // back to the same pixels, so none of the four full-tensor permutation passes of the reference is executed.
-// Per (batch, window, head): S = Q K^T (M=128 with 49 valid rows, N=64 keys, K=32) in TMEM, the soft-max threads own one
-// query row each, P (bf16) goes through shared memory into O = P V. Scores never touch HBM; only the row log-sum-exp is kept.
+// Per (batch, window, head): S = Q K^T (64 query rows with 49 valid, N=64 keys, K=32) by wgmma, handed to the soft-max
+// threads (one query row each) through a shared-memory image; P (bf16) goes through shared memory into O = P V. Scores never touch HBM; only the row log-sum-exp is kept.
 // CTAs are persistent over (batch, window) pairs of ONE head so that the backward pass can accumulate the gradient of the
 // relative-position bias in registers and flush it with one atomicAdd per element per CTA.
 //
@@ -78,13 +78,16 @@ __device__ __forceinline__ void wattn_gather(uint32_t tile_s, const __nv_bfloat1
 }
 
 // Two windows per step: rows 0..63 of every operand tile belong to window "A" of the pair, rows 64..127 to window "B"
-// (49 real tokens + 15 zero rows each). One M=128 x N=128 MMA produces both score blocks (the off-diagonal blocks are never
-// read), all four soft-max warps own real rows, and P is written block-diagonally (the off-diagonal halves of the P tile
-// are zeroed once and never touched) so that P V, P^T dO, dS K and dS^T Q of both windows are single M=128 MMAs as well.
-constexpr int kWAttnStages = 4;  // operand ring: the gathers run up to three steps ahead of the tensor core
-constexpr int kWAttnFwdSmem = kWAttnStages * 2 * 16384 + 2 * 32768 + 256 + 1024;
-constexpr int kWAttnFwdThreads = 11 * 32;  // 8 soft-max warps (two groups), 1 MMA warp, 2 gather warps
+// (49 real tokens + 15 zero rows each). A soft-max group (one warpgroup) multiplies the two diagonal 64 x 64 blocks with
+// wgmma (one m64 product per window), so every product of a step is two m64 MMAs; P is written block-diagonally into a
+// 128-row tile whose off-diagonal halves are zeroed once and never touched.
+constexpr int kWAttnStages = 3;  // operand ring: the gathers run up to two steps ahead of the tensor core
+constexpr int kWAttnImg = 128 * 64 * 4;   // per group: fp32 image of one 128 x 64 accumulator pair
+constexpr int kWAttnFwdSmem = kWAttnStages * 2 * 16384 + 2 * 32768 + 2 * kWAttnImg + 256 + 1024;
+// warps 0-1: gather, warps 4-7 / 8-11: soft-max groups 0 / 1 (warpgroups 1 and 2)
+constexpr int kWAttnFwdThreads = 12 * 32;
 constexpr int kWAttnGatherThreads = 64;
+static_assert(kWAttnFwdSmem <= 227 * 1024, "shared memory of one H100 block");
 
 __device__ __forceinline__ void wattn_item(const WAttnParams& p, int item, int nW, int nWx, int& b, int& win, int& wy, int& wx) {
   b = item / nW;
@@ -93,12 +96,30 @@ __device__ __forceinline__ void wattn_item(const WAttnParams& p, int item, int n
   wx = win - wy * nWx;
 }
 
-// Forward, warp specialised and double buffered. A step = one PAIR of windows of this CTA's head (see above).
-//   gather warps (9, 10): tokens i and i+64 of the pair -> 12 cp.async (q, k, v x 4 chunks) into ring stage n%3, then arrive full
-//   MMA warp (8):         S(n) = Q K^T into TMEM buffer n&1 as soon as the stage is full; O(n-1) = P V once group (n-1)&1
-//                         has written P; the commit of O also releases the stage to the gather warps
-//   soft-max group g (warps 4g..4g+3) owns the steps with n&1 == g: S -> P (bf16, block diagonal) -> wait O -> write out
-// so the gathers of step n+1, the soft-max of step n and the P V product / output of step n-1 overlap.
+// Both m64 products of a step for one group: window w (rows 64 w ..) of D = A B, K = 16 * KSTEPS. A / B descriptors of
+// window w: (a0 + w * a_win + k * a_k, b0 + w * b_win + k * b_k) in 16-byte units.
+template <int N, int TA, int TB, int KSTEPS>
+__device__ __forceinline__ void wattn_mma2(float (&d0)[N / 2], float (&d1)[N / 2], uint64_t a0, uint64_t a_win, uint64_t a_k,
+                                           uint64_t b0, uint64_t b_win, uint64_t b_k) {
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d0[i] = 0.f, d1[i] = 0.f;
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < KSTEPS; ++k) {
+    Wgmma<N, TA, TB>::mma(d0, a0 + k * a_k, b0 + k * b_k, 1u);
+    Wgmma<N, TA, TB>::mma(d1, a0 + a_win + k * a_k, b0 + b_win + k * b_k, 1u);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_reg_fence(d0);
+  wgmma_reg_fence(d1);
+}
+__device__ __forceinline__ uint64_t wdesc(uint32_t addr, uint32_t lbo) { return make_smem_desc_sw128(addr, lbo, 1024); }
+
+// Forward, warp specialised. A step = one PAIR of windows of this CTA's head (see above).
+//   gather warps (0, 1): tokens i and i+64 of the pair -> 12 cp.async (q, k, v x 4 chunks) into ring stage n%3, then arrive full
+//   soft-max group g (warpgroup 1 + g) owns the steps with n&1 == g: S = Q K^T -> P (bf16, block diagonal) -> O = P V ->
+//   write out, so the gathers of step n+1 and the two groups' steps overlap.
 __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WAttnParams p) {
   pdl_launch_dependents();
   pdl_wait();
@@ -106,18 +127,14 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WA
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // stage s: two tiles [128][128B] (rows 0..48: window A, 64..112: window B). A head row is only 64 B, so Q and K share
   // a tile (Q = 16-byte chunks 0..3 of a row, K = chunks 4..7: the K descriptor simply starts 64 B later) and V takes the
-  // first half of the second tile; then P[g]
+  // first half of the second tile; then P[g], then the accumulator images
   constexpr int kStage = 2 * 16384;
   constexpr int NS = kWAttnStages;
   uint8_t* sP = smem + NS * kStage;   // [2 groups][2 key atoms][128][128B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NS * kStage + 2 * 32768);
-  uint64_t* full = bars;        // [NS] gather complete (128 arrivals)
-  uint64_t* empty = bars + 4;   // [NS] stage consumed (commit of P V)
-  uint64_t* bar_s = bars + 8;   // [2] S in TMEM
-  uint64_t* bar_p = bars + 10;  // [2] P in smem (4 warp arrivals)
-  uint64_t* bar_o = bars + 12;  // [2] O in TMEM
-  uint64_t* tfree = bars + 14;  // [2] group done with its TMEM buffers and P tile (4 warp arrivals)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 16);
+  uint8_t* sImg = sP + 2 * 32768;     // [2 groups][128][64] fp32
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sImg + 2 * kWAttnImg);
+  uint64_t* full = bars;        // [NS] gather complete (64 arrivals)
+  uint64_t* empty = bars + 4;   // [NS] stage consumed (the group's P V product retired)
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int C = p.nH * 32;
   const int nWy = p.H / kWS, nWx = p.W / kWS, nW = nWy * nWx;
@@ -125,29 +142,15 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WA
   // zero everything once: pad rows of K / V and the off-diagonal halves of P must be finite zeros for every step
   for (int i = threadIdx.x; i < (NS * kStage + 2 * 32768) / 16; i += blockDim.x)
     reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  if (warp_idx == 8) {
-    if (lane == 0) {
-      for (int i = 0; i < NS; ++i) {
-        mbar_init(&full[i], kWAttnGatherThreads);
-        mbar_init(&empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&bar_s[i], 1);
-        mbar_init(&bar_p[i], 4);
-        mbar_init(&bar_o[i], 1);
-        mbar_init(&tfree[i], 4);
-      }
-      fence_mbar_init();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < NS; ++i) {
+      mbar_init(&full[i], kWAttnGatherThreads);
+      mbar_init(&empty[i], 1);
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_ptr_smem);
+    fence_mbar_init();
   }
   fence_proxy_async_smem();   // the zero fill above must be visible to the tensor core (async proxy)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  constexpr uint32_t kColS = 0, kColO = 256;   // S[g] at g*128, O[g] at 256 + g*32
 
   const int head = blockIdx.x % p.nH;
   const int lanes = gridDim.x / p.nH;           // CTAs sharing this head
@@ -156,9 +159,9 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WA
   const int first = blockIdx.x / p.nH;
   const int nsteps = first < npairs ? (npairs - first + lanes - 1) / lanes : 0;
 
-  if (warp_idx >= 9) {
+  if (warp_idx < 2) {
     // ===================== gather warps: one thread per token of the pair =====================
-    const int i0 = threadIdx.x - 9 * 32;   // 0..63; tokens i0 and i0 + 64 of the 98
+    const int i0 = threadIdx.x;   // 0..63; tokens i0 and i0 + 64 of the 98
     for (int n = 0; n < nsteps; ++n) {
       const int s = n % NS;
       const uint32_t ph = (n / NS) & 1;
@@ -186,47 +189,16 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WA
       fence_proxy_async_smem();
       mbar_arrive(&full[s]);
     }
-  } else if (warp_idx == 8) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);  // S[128 x 128 keys] = Q K^T, both K-major, K = 32
-      const uint32_t idesc_o = make_idesc_bf16(128, 32, 0, 1);   // O[128 x 32] = P (K-major) V (MN-major), K = 128 keys
-      for (int n = 0; n <= nsteps; ++n) {
-        if (n < nsteps) {
-          const int s = n % NS, g = n & 1;
-          mbar_wait(&tfree[g], ((n >> 1) & 1) ^ 1);   // group g has drained S/O of step n-2
-          mbar_wait(&full[s], (n / NS) & 1);
-          tc_fence_after();
-          const uint32_t q_s = smem_u32(smem + s * kStage), k_s = q_s + 64;
-#pragma unroll
-          for (int k = 0; k < 2; ++k)
-            umma_f16(tmem_base + kColS + g * 128, make_smem_desc_sw128(q_s + k * 32, 16, 1024),
-                     make_smem_desc_sw128(k_s + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-          umma_commit(&bar_s[g]);
-        }
-        if (n > 0) {
-          const int m = n - 1, s = m % NS, g = m & 1;
-          mbar_wait(&bar_p[g], (m >> 1) & 1);
-          tc_fence_after();
-          const uint32_t v_s = smem_u32(smem + s * kStage) + 16384, p_s = smem_u32(sP + g * 32768);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)
-            umma_f16(tmem_base + kColO + g * 32, make_smem_desc_sw128(p_s + (ks >> 2) * 16384 + (ks & 3) * 32, 16, 1024),
-                     make_smem_desc_sw128(v_s + ks * 2048, 8192, 1024), idesc_o, ks > 0 ? 1u : 0u);
-          umma_commit(&bar_o[g]);
-          umma_commit(&empty[s]);
-        }
-      }
-    }
-  } else {
+  } else if (warp_idx >= 4) {
     // ===================== soft-max groups: thread = query row of window `slot` =====================
-    const int g = warp_idx >> 2;
+    const int g = (warp_idx >> 2) - 1;
     const int row = (warp_idx & 3) * 32 + lane;
     const int slot = row >> 6, tok = row & 63;
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>((warp_idx & 3) * 32) << 16);
-    const uint32_t p_s = smem_u32(sP + g * 32768) + slot * 16384 + row * 128;  // this row's 64 keys (key atom `slot`)
+    const uint32_t img = smem_u32(sImg + g * kWAttnImg);
+    const uint32_t p_g = smem_u32(sP + g * 32768);
+    const uint32_t p_s = p_g + slot * 16384 + row * 128;  // this row's 64 keys (key atom `slot`)
     for (int n = g; n < nsteps; n += 2) {
-      const uint32_t ph = (n >> 1) & 1;
+      const int s = n % NS;
       const int item = 2 * (first + n * lanes) + slot;
       const bool valid = tok < kWT && item < total;
       int b = 0, win = 0, wy = 0, wx = 0;
@@ -238,15 +210,23 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WA
 #pragma unroll
       for (int c = 0; c < 13; ++c) bv[c] = __ldg(brow + c);
       const float* bf = reinterpret_cast<const float*>(bv);
-      mbar_wait(&bar_s[g], ph);
-      tc_fence_after();
+      mbar_wait(&full[s], (n / NS) & 1);
+      const uint32_t q_s = smem_u32(smem + s * kStage), k_s = q_s + 64, v_s = q_s + 16384;
+      {
+        // S = Q K^T of both windows (K = 32: two steps), into the image
+        float s0[32], s1[32];
+        wattn_mma2<64, 0, 0, 2>(s0, s1, wdesc(q_s, 16), 8192 >> 4, 2, wdesc(k_s, 16), 8192 >> 4, 2);
+        named_bar_sync(1 + g, 128);   // the previous step's O has been read out of the image
+        acc_to_img<64>(s0, img, 64, 0, 0);
+        acc_to_img<64>(s1, img, 64, 64, 0);
+        named_bar_sync(1 + g, 128);
+      }
       uint32_t v[64];
       {
         uint32_t(&lo)[32] = *reinterpret_cast<uint32_t(*)[32]>(&v[0]);
         uint32_t(&hi)[32] = *reinterpret_cast<uint32_t(*)[32]>(&v[32]);
-        tmem_ld_32x32(taddr + kColS + g * 128 + slot * 64, lo);
-        tmem_ld_32x32(taddr + kColS + g * 128 + slot * 64 + 32, hi);
-        tmem_ld_wait();
+        img_ld32(img, 64, row, 0, lo);
+        img_ld32(img, 64, row, 32, hi);
       }
       // log2 domain, branch free: rows outside the window (zero Q rows -> finite scores) get max = +inf -> all-zero P
       const float scale2 = p.scale * 1.4426950408889634f;
@@ -270,18 +250,19 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WA
 #pragma unroll
       for (int c = 0; c < 8; ++c) sts128(p_s + ((c ^ (row & 7)) << 4), v[c * 4], v[c * 4 + 1], v[c * 4 + 2], v[c * 4 + 3]);
       if (valid) p.lse[((static_cast<long long>(b) * nW + win) * p.nH + head) * kWT + tok] = mx + __log2f(sum);  // log2 units
-      tc_fence_before();
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_p[g]);
-      mbar_wait(&bar_o[g], ph);
-      tc_fence_after();
+      named_bar_sync(1 + g, 128);   // P complete; every row has read S out of the image
+      {
+        // O = P V of both windows: A = P (K-major, the window's own key atom), B = V (MN-major), K = 64 keys
+        float o0[16], o1[16];
+        wattn_mma2<32, 0, 1, 4>(o0, o1, wdesc(p_g, 16), (16384 + 8192) >> 4, 2, wdesc(v_s, 8192), 8192 >> 4, 2048 >> 4);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[s]);   // Q / K / V of this stage are no longer read
+        acc_to_img<32>(o0, img, 64, 0, 0);
+        acc_to_img<32>(o1, img, 64, 64, 0);
+        named_bar_sync(1 + g, 128);
+      }
       uint32_t ov[32];
-      tmem_ld_32x32(taddr + kColO + g * 32, ov);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tfree[g]);   // S / O columns and the P tile of this group may be reused
+      img_ld32(img, 64, row, 0, ov);
       if (valid) {
         const float inv = 1.0f / sum;
         __nv_bfloat16* dst = p.out + wattn_pixel(p, b, wy, wx, tok) * C + head * 32;
@@ -297,23 +278,17 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WA
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 8) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // Backward. Per (batch, window, head), two windows per step as in the forward kernel:
 //   P = exp(scale*S + bias + mask - lse);  dP = dO V^T;  dS = P*(dP - delta), delta_i = <dO_i, O_i>;  dbias += dS
 //   dV = P^T dO;  dQ = scale * dS K;  dK = scale * dS^T Q          (dS is stored pre-multiplied by scale)
-constexpr int kWAttnBwdSmem = kWAttnStages * 2 * 16384 + 2 * 32768 + 256 + 1024;
+constexpr int kWAttnBwdSmem = kWAttnFwdSmem;
 
-// Same warp-specialised pipeline as the forward kernel (two-stage Q/K/V/dO ring, two soft-max groups with their own TMEM
-// columns and P/dS tile). Per step m the MMA warp issues   A(m): S = Q K^T   B(m): dP = dO V^T, dV = P^T dO   C(m): dQ = dS K,
-// dK = dS^T Q   in the order  B(n-1), A(n), C(n-1)  so that one group computes P while the other computes dS / stores.
+// Same warp-specialised pipeline as the forward kernel (Q/K/V/dO ring, two soft-max groups with their own P/dS tile and
+// accumulator image); each group issues its step's products itself: S = Q K^T, then dP = dO V^T with dV = P^T dO, then
+// dQ = dS K with dK = dS^T Q (block diagonal: only the two 64 x 64 window blocks are multiplied).
 __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WAttnParams p) {
   pdl_launch_dependents();
   pdl_wait();
@@ -322,47 +297,25 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
   constexpr int kStage = 2 * 16384;   // tile 0: Q (chunks 0..3 of a row) | K (chunks 4..7); tile 1: V | dO
   constexpr int NS = kWAttnStages;
   uint8_t* sP = smem + NS * kStage;   // [2 groups][2 key atoms][128][128B]: P, then dS in place (block diagonal)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NS * kStage + 2 * 32768);
+  uint8_t* sImg = sP + 2 * 32768;     // [2 groups][128][64] fp32
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sImg + 2 * kWAttnImg);
   uint64_t* full = bars;         // [NS]
   uint64_t* empty = bars + 4;    // [NS]
-  uint64_t* bar_s = bars + 8;    // [2] S in TMEM
-  uint64_t* bar_p = bars + 10;   // [2] P in smem (4 warp arrivals)
-  uint64_t* bar_dp = bars + 12;  // [2] dP (and dV) in TMEM
-  uint64_t* bar_ds = bars + 14;  // [2] dS in smem (4 warp arrivals)
-  uint64_t* bar_dq = bars + 16;  // [2] dQ, dK in TMEM
-  uint64_t* tfree = bars + 18;   // [2] group done with its TMEM columns and P tile
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 20);
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int C = p.nH * 32;
   const int nWy = p.H / kWS, nWx = p.W / kWS, nW = nWy * nWx;
 
   for (int i = threadIdx.x; i < (NS * kStage + 2 * 32768) / 16; i += blockDim.x)
     reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-  if (warp_idx == 8) {
-    if (lane == 0) {
-      for (int i = 0; i < NS; ++i) {
-        mbar_init(&full[i], kWAttnGatherThreads);
-        mbar_init(&empty[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&bar_s[i], 1);
-        mbar_init(&bar_p[i], 4);
-        mbar_init(&bar_dp[i], 1);
-        mbar_init(&bar_ds[i], 4);
-        mbar_init(&bar_dq[i], 1);
-        mbar_init(&tfree[i], 4);
-      }
-      fence_mbar_init();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < NS; ++i) {
+      mbar_init(&full[i], kWAttnGatherThreads);
+      mbar_init(&empty[i], 1);
     }
-    __syncwarp();
-    tmem_alloc<512>(tmem_ptr_smem);
+    fence_mbar_init();
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  constexpr uint32_t kColS = 0, kColDV = 256, kColDK = 320;   // S[g] at g*128; dV[g] / dK[g] at +g*32
 
   const int head = blockIdx.x % p.nH;
   const int lanes = gridDim.x / p.nH;
@@ -371,9 +324,11 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
   const int first = blockIdx.x / p.nH;
   const int nsteps = first < npairs ? (npairs - first + lanes - 1) / lanes : 0;
 
-  if (warp_idx >= 9) {
+  if (warp_idx < 4) {
+    setmaxnreg_dec<56>();
+    if (warp_idx < 2) {
     // ===================== gather warps: one thread per token of the pair (q, k, v, dO rows) =====================
-    const int i0 = threadIdx.x - 9 * 32;
+    const int i0 = threadIdx.x;
     WPROF_DECL(3)
     for (int n = 0; n < nsteps; ++n) {
       const int s = n % NS;
@@ -408,82 +363,18 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
       mbar_arrive(&full[s]);
     }
 #ifdef WATTN_PROFILE
-    if (blockIdx.x == 0 && threadIdx.x == 9 * 32 && nsteps > 0)
+    if (blockIdx.x == 0 && threadIdx.x == 0 && nsteps > 0)
       printf("bwd gather : wait_empty %lld  issue %lld  wait_data %lld\n", wp_t[0] / nsteps, wp_t[1] / nsteps, wp_t[2] / nsteps);
-#endif
-  } else if (warp_idx == 8) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);  // [128 q] x [128 keys], K = 32
-      const uint32_t idesc_t = make_idesc_bf16(128, 32, 1, 1);   // A^T B, both MN-major (P^T dO, dS^T Q), K = 128 query rows
-      const uint32_t idesc_q = make_idesc_bf16(128, 32, 0, 1);   // dS (K-major) x K (MN-major), K = 128 keys
-      WPROF_DECL(5)
-      for (int n = 0; n <= nsteps; ++n) {
-        if (n > 0) {  // B(n-1): dP = dO V^T (into the S columns) and dV = P^T dO
-          const int m = n - 1, s = m % NS, g = m & 1;
-          WPROF_TICK(4)
-          mbar_wait(&bar_p[g], (m >> 1) & 1);
-          WPROF_TICK(0)
-          tc_fence_after();
-          const uint32_t base = smem_u32(smem + s * kStage), v_s = base + 16384, do_s = v_s + 64;
-          const uint32_t p_s = smem_u32(sP + g * 32768);
-#pragma unroll
-          for (int k = 0; k < 2; ++k)
-            umma_f16(tmem_base + kColS + g * 128, make_smem_desc_sw128(do_s + k * 32, 16, 1024),
-                     make_smem_desc_sw128(v_s + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)  // 128 query rows = 8 steps of 16; A = P^T: two 64-key atoms 16384 B apart
-            umma_f16(tmem_base + kColDV + g * 32, make_smem_desc_sw128(p_s + ks * 2048, 16384, 1024),
-                     make_smem_desc_sw128(do_s + ks * 2048, 8192, 1024), idesc_t, ks > 0 ? 1u : 0u);
-          umma_commit(&bar_dp[g]);
-        }
-        if (n < nsteps) {  // A(n): S = Q K^T
-          const int s = n % NS, g = n & 1;
-          WPROF_TICK(4)
-          mbar_wait(&tfree[g], ((n >> 1) & 1) ^ 1);
-          WPROF_TICK(1)
-          mbar_wait(&full[s], (n / NS) & 1);
-          WPROF_TICK(2)
-          tc_fence_after();
-          const uint32_t q_s = smem_u32(smem + s * kStage), k_s = q_s + 64;
-#pragma unroll
-          for (int k = 0; k < 2; ++k)
-            umma_f16(tmem_base + kColS + g * 128, make_smem_desc_sw128(q_s + k * 32, 16, 1024),
-                     make_smem_desc_sw128(k_s + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-          umma_commit(&bar_s[g]);
-        }
-        if (n > 0) {  // C(n-1): dQ = dS K (S columns again) and dK = dS^T Q
-          const int m = n - 1, s = m % NS, g = m & 1;
-          WPROF_TICK(4)
-          mbar_wait(&bar_ds[g], (m >> 1) & 1);
-          WPROF_TICK(3)
-          tc_fence_after();
-          const uint32_t q_s = smem_u32(smem + s * kStage), k_s = q_s + 64;
-          const uint32_t p_s = smem_u32(sP + g * 32768);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)
-            umma_f16(tmem_base + kColS + g * 128, make_smem_desc_sw128(p_s + (ks >> 2) * 16384 + (ks & 3) * 32, 16, 1024),
-                     make_smem_desc_sw128(k_s + ks * 2048, 8192, 1024), idesc_q, ks > 0 ? 1u : 0u);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)
-            umma_f16(tmem_base + kColDK + g * 32, make_smem_desc_sw128(p_s + ks * 2048, 16384, 1024),
-                     make_smem_desc_sw128(q_s + ks * 2048, 8192, 1024), idesc_t, ks > 0 ? 1u : 0u);
-          umma_commit(&bar_dq[g]);
-          umma_commit(&empty[s]);
-        }
-      }
-#ifdef WATTN_PROFILE
-      if (blockIdx.x == 0 && nsteps > 0)
-        printf("bwd mma    : wait_p %lld  wait_tfree %lld  wait_full %lld  wait_ds %lld  issue %lld\n", wp_t[0] / nsteps,
-               wp_t[1] / nsteps, wp_t[2] / nsteps, wp_t[3] / nsteps, wp_t[4] / nsteps);
 #endif
     }
   } else {
     // ===================== soft-max groups =====================
-    const int g = warp_idx >> 2;
+    setmaxnreg_inc<224>();
+    const int g = (warp_idx >> 2) - 1;
     const int row = (warp_idx & 3) * 32 + lane;
     const int slot = row >> 6, tok = row & 63;
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>((warp_idx & 3) * 32) << 16);
+    const uint32_t img = smem_u32(sImg + g * kWAttnImg);
+    const uint32_t p_g = smem_u32(sP + g * 32768);
     uint8_t* const prow = sP + g * 32768 + slot * 16384 + row * 128;   // this row's 64 keys (key atom `slot`)
     const uint32_t prow_s = smem_u32(prow);
     WPROF_DECL(14)
@@ -491,7 +382,6 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
 #pragma unroll
     for (int j = 0; j < kWT; ++j) db[j] = 0.f;
     for (int n = g; n < nsteps; n += 2) {
-      const uint32_t ph = (n >> 1) & 1;
       const int s = n % NS;
       const int item = 2 * (first + n * lanes) + slot;
       const bool valid = tok < kWT && item < total;
@@ -507,22 +397,30 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
 #pragma unroll
       for (int c = 0; c < 13; ++c) bv[c] = __ldg(brow + c);
       const float* bf = reinterpret_cast<const float*>(bv);
-      uint4 orow[4];  // forward output row (64 B), requested early: only needed for delta after the first MMA wait
+      uint4 orow[4];  // forward output row (64 B), requested early: only needed for delta
       if (valid) {
         const uint4* op = reinterpret_cast<const uint4*>(p.o + pix * C + head * 32);
 #pragma unroll
         for (int c = 0; c < 4; ++c) orow[c] = __ldg(op + c);
       }
-      // ---- P
       WPROF_TICK(13)
-      mbar_wait(&bar_s[g], ph);
+      mbar_wait(&full[s], (n / NS) & 1);
       WPROF_TICK(0)
-      tc_fence_after();
+      const uint32_t q_s = smem_u32(smem + s * kStage), k_s = q_s + 64, v_s = q_s + 16384, do_s = v_s + 64;
+      {
+        // S = Q K^T (both windows) into the image
+        float s0[32], s1[32];
+        wattn_mma2<64, 0, 0, 2>(s0, s1, wdesc(q_s, 16), 8192 >> 4, 2, wdesc(k_s, 16), 8192 >> 4, 2);
+        named_bar_sync(1 + g, 128);   // the previous step's gradients have been read out of the image
+        acc_to_img<64>(s0, img, 64, 0, 0);
+        acc_to_img<64>(s1, img, 64, 64, 0);
+        named_bar_sync(1 + g, 128);
+      }
+      // ---- P
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {   // two 32-key halves keep the live register set small
         uint32_t v[32];
-        tmem_ld_32x32(taddr + kColS + g * 128 + slot * 64 + hf * 32, v);
-        tmem_ld_wait();
+        img_ld32(img, 64, row, hf * 32, v);
         WPROF_TICK(1)
 #pragma unroll
         for (int jj = 0; jj < 32; jj += 2) {
@@ -538,12 +436,20 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
           sts128(prow_s + (((hf * 4 + c) ^ (row & 7)) << 4), v[c * 4], v[c * 4 + 1], v[c * 4 + 2], v[c * 4 + 3]);
         WPROF_TICK(3)
       }
-      tc_fence_before();
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_p[g]);
+      named_bar_sync(1 + g, 128);   // P complete; S read out of the image
       WPROF_TICK(4)
-      // delta_i = <dO_i, O_i>: dO from the gathered tile (stage s stays valid until C(n) retires)
+      // dP = dO V^T (both windows) into the image, dV = P^T dO (A = P^T: the window's key atom, MN-major) kept in registers
+      float gv0[16], gv1[16];
+      {
+        float d0[32], d1[32];
+        wattn_mma2<64, 0, 0, 2>(d0, d1, wdesc(do_s, 16), 8192 >> 4, 2, wdesc(v_s, 16), 8192 >> 4, 2);
+        acc_to_img<64>(d0, img, 64, 0, 0);
+        acc_to_img<64>(d1, img, 64, 64, 0);
+        wattn_mma2<32, 1, 1, 4>(gv0, gv1, wdesc(p_g, 16384), (16384 + 8192) >> 4, 2048 >> 4, wdesc(do_s, 8192), 8192 >> 4,
+                             2048 >> 4);
+      }
+      // delta_i = <dO_i, O_i>: dO from the gathered tile (stage s stays valid until this step's last products retire)
       float delta = 0.f;
       if (valid) {
         const uint8_t* drow = smem + s * kStage + 16384 + row * 128;   // dO = chunks 4..7 of the V|dO tile row
@@ -556,18 +462,15 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
           for (int e = 0; e < 8; ++e) delta = fmaf(a[e], o[e], delta);
         }
       }
+      named_bar_sync(1 + g, 128);   // dP in the image
       // ---- dS (in place over P)
-      WPROF_TICK(5)
-      mbar_wait(&bar_dp[g], ph);
       WPROF_TICK(6)
-      tc_fence_after();
       {
         uint32_t v[64];
         uint32_t(&lo)[32] = *reinterpret_cast<uint32_t(*)[32]>(&v[0]);
         uint32_t(&hi)[32] = *reinterpret_cast<uint32_t(*)[32]>(&v[32]);
-        tmem_ld_32x32(taddr + kColS + g * 128 + slot * 64, lo);
-        tmem_ld_32x32(taddr + kColS + g * 128 + slot * 64 + 32, hi);
-        tmem_ld_wait();
+        img_ld32(img, 64, row, 0, lo);
+        img_ld32(img, 64, row, 32, hi);
         WPROF_TICK(7)
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
@@ -586,24 +489,36 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
         }
       }
       WPROF_TICK(8)
-      tc_fence_before();
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_ds[g]);
-      // ---- write dq (row = query), dk / dv (row = key) of this token
-      WPROF_TICK(9)
-      mbar_wait(&bar_dq[g], ph);
+      named_bar_sync(1 + g, 128);   // dS complete; dP read out of the image
+      // dQ = dS K (A = dS K-major, B = K MN-major) and dK = dS^T Q (both MN-major), then the gradients through the image
+      {
+        float q0[16], q1[16], k0[16], k1[16];
+        wattn_mma2<32, 0, 1, 4>(q0, q1, wdesc(p_g, 16), (16384 + 8192) >> 4, 2, wdesc(k_s, 8192), 8192 >> 4, 2048 >> 4);
+        wattn_mma2<32, 1, 1, 4>(k0, k1, wdesc(p_g, 16384), (16384 + 8192) >> 4, 2048 >> 4, wdesc(q_s, 8192), 8192 >> 4,
+                             2048 >> 4);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[s]);   // the stage is no longer read
+        acc_to_img<32>(q0, img, 64, 0, 0);
+        acc_to_img<32>(q1, img, 64, 64, 0);
+        acc_to_img<32>(k0, img, 64, 0, 32);
+        acc_to_img<32>(k1, img, 64, 64, 32);
+      }
+      named_bar_sync(1 + g, 128);
       WPROF_TICK(10)
-      tc_fence_after();
       uint32_t gq[32], gk[32], gv[32];
-      tmem_ld_32x32(taddr + kColS + g * 128, gq);
-      tmem_ld_32x32(taddr + kColDK + g * 32, gk);
-      tmem_ld_32x32(taddr + kColDV + g * 32, gv);
-      tmem_ld_wait();
+      img_ld32(img, 64, row, 0, gq);
+      {
+        uint32_t t2[32];
+        img_ld32(img, 64, row, 32, t2);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) gk[i] = t2[i];
+      }
+      named_bar_sync(1 + g, 128);
+      acc_to_img<32>(gv0, img, 64, 0, 0);
+      acc_to_img<32>(gv1, img, 64, 64, 0);
+      named_bar_sync(1 + g, 128);
+      img_ld32(img, 64, row, 0, gv);
       WPROF_TICK(11)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tfree[g]);
       if (valid) {
         __nv_bfloat16* dst = p.dqkv + pix * 3 * C + head * 32;
 #pragma unroll
@@ -626,9 +541,9 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
     WPROF_TICK(12)
     if (blockIdx.x == 0 && lane == 0 && (warp_idx & 3) == 0 && nsteps > 1) {
       const int ns = (nsteps - g + 1) / 2;
-      printf("bwd softmax g%d: wait_s %lld | P: ld %lld math %lld sts %lld fence %lld | delta %lld wait_dp %lld | dS: ld %lld math %lld fence %lld | "
-             "wait_dq %lld | epi: ld %lld store %lld | prologue %lld\n", g, wp_t[0] / ns, wp_t[1] / ns, wp_t[2] / ns, wp_t[3] / ns, wp_t[4] / ns,
-             wp_t[5] / ns, wp_t[6] / ns, wp_t[7] / ns, wp_t[8] / ns, wp_t[9] / ns, wp_t[10] / ns, wp_t[11] / ns, wp_t[12] / ns, wp_t[13] / ns);
+      printf("bwd softmax g%d: wait_s %lld | P: ld %lld math %lld sts %lld fence %lld | dS: ld %lld math %lld | "
+             "grad: mma %lld ld %lld store %lld | prologue %lld\n", g, wp_t[0] / ns, wp_t[1] / ns, wp_t[2] / ns, wp_t[3] / ns,
+             wp_t[4] / ns, wp_t[7] / ns, wp_t[8] / ns, wp_t[10] / ns, wp_t[11] / ns, wp_t[12] / ns, wp_t[13] / ns);
     }
 #endif
     if (tok < kWT) {
@@ -636,12 +551,6 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
 #pragma unroll
       for (int j = 0; j < kWT; ++j) atomicAdd(dbp + j, db[j]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 8) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 

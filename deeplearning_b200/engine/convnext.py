@@ -1,4 +1,4 @@
-"""Forward / backward schedule of the ConvNeXt family on the sm_100a kernels (one autograd.Function for the whole network).
+"""Forward / backward schedule of the ConvNeXt family on the sm_90a kernels (one autograd.Function for the whole network).
 
 Mirrors ``ConvNeXt.forward_features`` / ``Block.forward`` of the reference (classification/convNext/models/networks.py:160-170,
 :92-105).  The residual stream ``x`` is fp32 NHWC; everything feeding a tensor core is bf16:
@@ -285,7 +285,7 @@ class _Function(torch.autograd.Function):
 
 def apply(model, x):
     if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 ConvNeXt runs on CUDA (sm_100a) tensors only; there is no CPU fallback")
+        raise RuntimeError("deeplearning_b200 ConvNeXt runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
     params = tuple(model.parameters())
     if torch.is_grad_enabled() and any(p.requires_grad for p in params):
         return _Function.apply(x, model, *params)

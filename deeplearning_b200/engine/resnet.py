@@ -1,8 +1,8 @@
-"""Forward / backward schedule of the ResNet family on the sm_100a kernels.
+"""Forward / backward schedule of the ResNet family on the sm_90a kernels.
 
 The whole network is ONE ``torch.autograd.Function``: forward runs conv(+BN statistics in the GEMM epilogue) -> finalize ->
 apply(+ReLU)(+residual) per layer and records the tensors the backward needs on a tape; backward replays the tape with
-BN-backward reduce/apply passes, tcgen05 dgrad and wgrad GEMMs.  Residual additions never get their own pass: the identity
+BN-backward reduce/apply passes, wgmma dgrad and wgrad GEMMs.  Residual additions never get their own pass: the identity
 gradient is added in the epilogue of the first conv's dgrad GEMM.
 
 Mirrors ``ResNet._forward_impl`` / ``Bottleneck.forward`` / ``BasicBlock.forward`` of the reference
@@ -35,13 +35,13 @@ def _check_conv(conv, name):
     if (conv.groups != 1 or conv.dilation != (1, 1) or conv.kernel_size[0] != conv.kernel_size[1] or conv.bias is not None
             or conv.padding != (k // 2, k // 2) or conv.stride[0] != conv.stride[1] or conv.stride[0] not in (1, 2)):
         raise NotImplementedError(f"{name}: only dense k x k convolutions with pad=k//2, stride 1/2, no bias run on the "
-                                  f"B200 engine (got {conv})")
+                                  f"GPU engine (got {conv})")
 
 
 def _check_bn(bn, name):
     if (not isinstance(bn, (nn.BatchNorm2d, nn.SyncBatchNorm)) or not bn.affine or not bn.track_running_stats
             or bn.momentum is None):
-        raise NotImplementedError(f"{name}: the B200 engine implements affine nn.BatchNorm2d / nn.SyncBatchNorm with running "
+        raise NotImplementedError(f"{name}: this engine implements affine nn.BatchNorm2d / nn.SyncBatchNorm with running "
                                   f"statistics (got {bn})")
 
 
@@ -478,7 +478,7 @@ class _ResNetFunction(torch.autograd.Function):
 
 def apply(model, x):
     if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 ResNet runs on CUDA (sm_100a) tensors only; there is no CPU fallback")
+        raise RuntimeError("deeplearning_b200 ResNet runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
     params = tuple(model.parameters())
     if torch.is_grad_enabled() and any(p.requires_grad for p in params):
         return _ResNetFunction.apply(x, model, *params)

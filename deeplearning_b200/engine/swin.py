@@ -1,4 +1,4 @@
-"""Forward / backward schedule of the Swin Transformer on the sm_100a kernels (one autograd.Function for the whole network).
+"""Forward / backward schedule of the Swin Transformer on the sm_90a kernels (one autograd.Function for the whole network).
 
 Mirrors ``SwinTransformer.forward_features`` / ``BasicLayer.forward`` / ``SwinTransformerBlock.forward`` /
 ``WindowAttention.forward`` / ``PatchMerging.forward`` of the reference
@@ -6,7 +6,7 @@ Mirrors ``SwinTransformer.forward_features`` / ``BasicLayer.forward`` / ``SwinTr
 
 Data flow per block (residual stream ``h`` fp32 [B, H*W, C] in natural pixel order; tensor-core operands bf16):
     LN1(h) -> qkv GEMM(+bias) -> shifted-window attention (roll, partition, bias, mask, softmax, reverse, un-roll all inside
-    one tcgen05 kernel that gathers its 49-token windows straight from the pixel-ordered qkv tensor)
+    one wgmma kernel that gathers its 49-token windows straight from the pixel-ordered qkv tensor)
     -> proj GEMM(+bias, +h, fp32 out) = h2 -> LN2 -> fc1 GEMM(+bias, GELU, keeps GELU'(pre)) -> fc2 GEMM(+bias, +h2) = h3
 PatchMerging = one gather+LayerNorm kernel (the 2x2 concat never exists in HBM) + the bias-free reduction GEMM (fp32 out).
 """
@@ -61,15 +61,15 @@ _pack_spec = _PackSpec()
 
 def _check(model):
     if model.ape:
-        raise NotImplementedError("absolute position embedding (ape=True) is not implemented on the B200 engine")
+        raise NotImplementedError("absolute position embedding (ape=True) is not implemented on this engine")
     if model.patch_embed.norm is None:
-        raise NotImplementedError("patch_norm=False is not implemented on the B200 engine")
+        raise NotImplementedError("patch_norm=False is not implemented on this engine")
     if not isinstance(model.head, nn.Linear):
         raise NotImplementedError("model.head must be an nn.Linear (num_classes > 0)")
     if model.training:
         for m in model.modules():
             if isinstance(m, nn.Dropout) and m.p != 0:
-                raise NotImplementedError("dropout > 0 is not implemented on the B200 engine")
+                raise NotImplementedError("dropout > 0 is not implemented on this engine")
     for blk in _blocks(model):
         if blk.window_size != 7 or blk.dim // blk.num_heads != 32:
             raise NotImplementedError("the window-attention kernel is built for window_size 7 and head_dim 32")
@@ -265,7 +265,7 @@ class _SwinFunction(torch.autograd.Function):
 
 def apply(model, x):
     if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 Swin runs on CUDA (sm_100a) tensors only; there is no CPU fallback")
+        raise RuntimeError("deeplearning_b200 Swin runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
     params = tuple(model.parameters())
     if torch.is_grad_enabled() and any(p.requires_grad for p in params):
         return _SwinFunction.apply(x, model, *params)

@@ -1,6 +1,6 @@
 """Data-parallel training step: flat parameter / gradient arenas, ONE gradient all-reduce, one fused optimizer launch.
 
-B200-native counterpart of the reference's DDP recipe (others/train_with_DDP/train.py:106-111,188-201,245-253 and
+H100-native counterpart of the reference's DDP recipe (others/train_with_DDP/train.py:106-111,188-201,245-253 and
 classification/swin_transformer/main.py:101-103): one process per GPU, identical replicas, per-GPU BatchNorm statistics
 (DDP *without* SyncBN, as the north-star asks), gradients averaged across ranks after backward, identical update on every
 rank.  The backward kernels write straight into one contiguous fp32 arena; like DDP's bucketed reducer the all-reduce is
@@ -46,7 +46,7 @@ def _engine_for(model):
         from . import swin
 
         return swin
-    raise NotImplementedError(f"no B200 engine schedule for {type(model).__name__}")
+    raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 
 def ops_clip_blocks():
@@ -219,7 +219,7 @@ class TrainStep:
         self.arena = FlatArena(model.parameters(), process_group, world_size, bucket_mb=bucket_mb)
         self.overlap = overlap   # bucketed all-reduce on a side stream during the backward pass (False: one call after it)
         if self.arena.flat_p.device.type != "cuda":
-            raise RuntimeError("TrainStep needs the model on a CUDA (sm_100a) device; there is no CPU fallback")
+            raise RuntimeError("TrainStep needs the model on a CUDA (sm_90a) device; there is no CPU fallback")
         self.world = self.arena.world
         self.steps = 0
         self.label_smoothing = float(label_smoothing)

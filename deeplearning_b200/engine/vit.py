@@ -1,10 +1,10 @@
-"""Forward / backward schedule of the ViT family on the sm_100a kernels (one autograd.Function for the whole network).
+"""Forward / backward schedule of the ViT family on the sm_90a kernels (one autograd.Function for the whole network).
 
 Mirrors ``VisionTransformer.forward_features`` / ``Block.forward`` / ``Attention.forward`` / ``Mlp.forward`` of the
 reference (classification/vision_transformer/vit_model.py:240-268, :158-161, :88-111, :127-133).
 
 Data flow per block (residual stream ``h`` fp32 [B,T,D], everything feeding a tensor core bf16):
-    LN1(h) -> qkv GEMM(+bias) -> tcgen05 attention -> proj GEMM(+bias, +h, fp32 out) = h2
+    LN1(h) -> qkv GEMM(+bias) -> wgmma attention -> proj GEMM(+bias, +h, fp32 out) = h2
     LN2(h2) -> fc1 GEMM(+bias, GELU; also writes GELU'(pre) for the backward) -> fc2 GEMM(+bias, +h2, fp32 out) = h3
 Residual adds, biases, GELU, GELU' (backward) and the pos-embed add of the patch embedding all live in GEMM epilogues; the
 attention scores never touch HBM.  The gradient of the residual stream is carried in bf16 and accumulated inside the
@@ -57,7 +57,7 @@ _pack_spec = _PackSpec()
 
 def _check(model):
     if model.dist_token is not None:
-        raise NotImplementedError("distilled ViT (dist_token) is not implemented on the B200 engine")
+        raise NotImplementedError("distilled ViT (dist_token) is not implemented on this engine")
     if model.has_logits and not (isinstance(getattr(model.pre_logits, "fc", None), nn.Linear)
                                  and isinstance(getattr(model.pre_logits, "act", None), nn.Tanh)):
         raise NotImplementedError("pre_logits must be the reference's Sequential(fc=Linear, act=Tanh) (vit_model.py:218-221)")
@@ -65,7 +65,7 @@ def _check(model):
         raise NotImplementedError("model.head must be an nn.Linear (num_classes > 0)")
     for m in model.modules():
         if isinstance(m, nn.Dropout) and m.p != 0 and model.training:
-            raise NotImplementedError("dropout > 0 is not implemented on the B200 engine")
+            raise NotImplementedError("dropout > 0 is not implemented on this engine")
     for blk in model.blocks:
         if blk.attn.qkv.in_features // blk.attn.num_heads != 64:
             raise NotImplementedError("the attention kernel is built for head_dim 64")
@@ -278,7 +278,7 @@ class _VitFunction(torch.autograd.Function):
 
 def apply(model, x):
     if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 ViT runs on CUDA (sm_100a) tensors only; there is no CPU fallback")
+        raise RuntimeError("deeplearning_b200 ViT runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
     params = tuple(model.parameters())
     if torch.is_grad_enabled() and any(p.requires_grad for p in params):
         return _VitFunction.apply(x, model, *params)

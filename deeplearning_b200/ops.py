@@ -1,6 +1,6 @@
 """Tensor-level wrappers over the C ABI (include/b200cls.h).
 
-PyTorch is used for device memory and streams only; every arithmetic op below is a hand-written sm_100a kernel.
+PyTorch is used for device memory and streams only; every arithmetic op below is a hand-written sm_90a kernel.
 Activations are NHWC bf16 tensors ``[B, H, W, C]`` (``[rows, C]`` for linear layers); parameters and statistics fp32.
 """
 import os
@@ -503,7 +503,7 @@ def conv1x1_dgrad_masked(dy, wd_packed, residual, mask_src):
     Cin = wd_packed.shape[0]
     pixels = dy.numel() // Cout
     dz = torch.empty(*dy.shape[:-1], Cin, dtype=BF16, device=dy.device)
-    T = lib.b200_conv1x1_dgrad_masked_stats_rows(pixels, Cin)
+    T = lib.b200_conv1x1_dgrad_masked_stats_rows(pixels, Cin, Cout)
     stats = torch.empty(T, 2, Cin, dtype=F32, device=dy.device)
     sp = _span("conv_gemm_dgrad", 2.0 * pixels * Cin * Cout, _nb(dy, wd_packed, residual, mask_src, dz))
     rc = lib.b200_conv1x1_dgrad_masked(_p(dy), _p(wd_packed), _p(dz), pixels, Cin, Cout, _p(residual), _p(mask_src), _p(stats),

@@ -1,4 +1,4 @@
-/* libb200cls.so - C ABI of the B200-native classification training step.
+/* libb200cls.so - C ABI of the H100-native classification training step.
  *
  * The reference (KKKSQJ/DeepLearning) has no operator registry on this path: every op is a stock PyTorch call
  * (nn.Conv2d / nn.BatchNorm2d / nn.Linear / ... -> ATen -> cuDNN / cuBLAS, or oneDNN on CPU), and the only FFI it owns is
@@ -41,11 +41,11 @@ int b200_sm_count(void);
 /* Kernels launched by this library so far in this process (bench.py reports the per-step delta as gpu_launches). */
 unsigned long long b200_launch_count(void);
 
-/* ---- convolution / linear as implicit GEMM on tcgen05 (ksize in {1,3} pad ksize/2, stride in {1,2}; or 2x2/s2 unpadded) ----
+/* ---- convolution / linear as implicit GEMM on wgmma (ksize in {1,3} pad ksize/2, stride in {1,2}; or 2x2/s2 unpadded) ----
  * forward:  y[B,Ho,Wo,Cout] = conv(x[B,H,W,Cin], w) (+bias) (act) (+residual)
  *   w        bf16 [Cout][ksize*ksize*Cin]   (b200_pack_weight mode 0)
  *   stats    optional fp32 [b200_conv2d_fwd_stats_rows()][2][Cout]: partial sum / sum of squares of y (as stored), one row
- *            per (persistent CTA group, 32-lane TMEM quadrant) - a few hundred rows; feed them to b200_bn_finalize
+ *            per (persistent CTA group, 32-row quadrant) - a few hundred rows; feed them to b200_bn_finalize
  *   residual optional bf16, same shape as y, added after bias/act
  *   out_f32  optional fp32 [B*Ho*Wo][ld_out] - when given the result is written there instead of y (ksize 1 only)
  * replaces nn.Conv2d.forward / nn.Linear.forward: classification/resnet/models/networks.py:107,111,115,119,218;
@@ -150,7 +150,7 @@ int b200_copy_rows(const void* src, long long src_pitch_bytes, void* dst, long l
 int b200_colsum_partial_slices(long long rows);
 int b200_colsum_partial(const void* m, long long rows, long long ld, int cols, float* partial, void* stream);
 
-/* ---- multi-head self-attention, head_dim 64, T <= 256 tokens, on tcgen05 (vit_model.py:95-108) ---------------------------------
+/* ---- multi-head self-attention, head_dim 64, T <= 256 tokens, with wgmma (vit_model.py:95-108) ---------------------------------
  * qkv bf16 [B][T][3][H][64] (the qkv Linear output as is), out bf16 [B][T][H*64], lse fp32 [B][H][T].
  * backward: dqkv bf16 [B][T][3][H][64]; delta fp32 [B][H][T] is scratch. Scores / probabilities never touch HBM. */
 int b200_attention_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, float scale, void* stream);
@@ -158,7 +158,7 @@ int b200_attention_bwd(const void* qkv, const void* out, const void* dout, const
                        int B, int T, int H, float scale, void* stream);
 
 /* ---- Swin (classification/swin_transformer/models/swin_transformer.py) -----------------------------------------------------
- * Shifted-window attention, 7x7 windows, head_dim 32, on tcgen05. qkv bf16 [B][H][W][3*nH*32] in natural (un-rolled) pixel
+ * Shifted-window attention, 7x7 windows, head_dim 32, with wgmma. qkv bf16 [B][H][W][3*nH*32] in natural (un-rolled) pixel
  * order; torch.roll / window_partition / window_reverse (:251-280) are folded into the gather / scatter addressing.
  * bias_tab = b200_window_bias_gather(): fp32 [nH][masked ? nW : 1][49 (query i)][64 (key j, 49 used)] holding
  *   log2(e) x ( relative_position_bias_table[relative_position_index[i][j]][h] (:131-134) plus, for shifted blocks, the
@@ -336,7 +336,7 @@ int b200_subsample2(const void* x, void* xs, int B, int H, int W, int C, void* s
 int b200_add_even_pixels(void* gx, const void* gs, int B, int H, int W, int C, void* stream);
 /* dx[pixels][Cin] = (mask_src > 0) ? (dy[pixels][Cout] * wd^T + residual) : 0  (wd bf16 [Cin][Cout], b200_pack_weight mode 1);
  * stats fp32 [b200_conv1x1_dgrad_masked_stats_rows()][2][Cin]: per-CTA column sums (plane 0) of dx as stored */
-int b200_conv1x1_dgrad_masked_stats_rows(long long pixels, int Cin);
+int b200_conv1x1_dgrad_masked_stats_rows(long long pixels, int Cin, int Cout);
 int b200_conv1x1_dgrad_masked(const void* dy, const void* wd, void* dx, long long pixels, int Cin, int Cout,
                               const void* residual, const void* mask_src, float* stats, void* stream);
 /* dz_partial fp32 [T][2][N] (plane 0 = partial column sums of dz); scratch: b200_bn_conv1x1_bwd_scratch_bytes(N, K) bytes;
@@ -361,7 +361,7 @@ int b200_rowscale_bf16(const void* x, const float* scale, void* y, long long n_s
 int b200_tanh_fwd(const float* u, float* t, void* t_bf16, long long n, void* stream);
 int b200_tanh_bwd(const void* dt_bf16, const float* t, void* du_bf16, long long n, void* stream);
 
-/* bring-up only: override the UMMA shared-memory descriptor strides (which: 0 = forward K-major, 1 = wgrad MN-major) */
+/* bring-up only: override the wgmma shared-memory descriptor strides (which: 0 = forward K-major, 1 = wgrad MN-major) */
 int b200_debug_set_desc(int which, unsigned lbo, unsigned sbo, unsigned kstep);
 
 #ifdef __cplusplus

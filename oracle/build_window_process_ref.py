@@ -1,11 +1,11 @@
 """TEST / BASELINE INFRASTRUCTURE - builds the REFERENCE's own CUDA extension `swin_window_process`
 (classification/swin_transformer/kernels/window_process/swin_window_process{.cpp,_kernel.cu}, the only first-party CUDA of
-the reference) for sm_100a, as the beat-this baseline of b200_window_partition / b200_window_merge (SURVEY.md 2.3A).
+the reference) for sm_90a, as the beat-this baseline of b200_window_partition / b200_window_merge (SURVEY.md 2.3A).
 
 The sources are compiled from a scratch copy under /tmp (the reference tree is read-only and must not be copied into the
 repo); the only edit is the one torch 2.x forces: `AT_DISPATCH_*(x.type(), ...)` -> `x.scalar_type()` (the implicit
 DeprecatedTypeProperties -> ScalarType conversion was removed; the kernels are untouched).  Output: oracle/_ref/window_process/
-swin_window_process_ref.so (git-ignored, travels to the GPU box).  Run in the build container: python oracle/build_window_process_ref.py
+swin_window_process_ref.so (git-ignored).  Run where the reference checkout is present: python oracle/build_window_process_ref.py
 """
 import os
 import re
@@ -30,7 +30,7 @@ def build():
         text = re.sub(r"(AT_DISPATCH_[A-Z_]+\(\s*\w+)\.type\(\)", r"\1.scalar_type()", text)
         open(os.path.join(tmp, f), "w").write(text)
     os.makedirs(OUT, exist_ok=True)
-    os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0a"
+    os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"
     load(name="swin_window_process_ref", sources=[os.path.join(tmp, "swin_window_process.cpp"), os.path.join(tmp, "swin_window_process_kernel.cu")],
          build_directory=OUT, extra_cuda_cflags=["-O3"], is_python_module=True, verbose=False)
     return True

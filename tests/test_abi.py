@@ -30,10 +30,11 @@ def test_no_compute_calls_without_gpu_but_metadata_works():
     lib = _lib.load()
     assert lib.b200_abi_version() >= 1
     # pure host-side planners are usable without a device
-    # BN statistics rows: (persistent CTAs / channel blocks) x 4 TMEM quadrants (x2 when the warp pair alternates tiles)
-    assert lib.b200_conv2d_fwd_stats_rows(256, 56, 56, 64, 3, 1) == 148 * 8
-    assert lib.b200_conv2d_fwd_stats_rows(256, 56, 56, 256, 1, 1) == 148 * 4
-    assert lib.b200_conv2d_fwd_stats_rows(256, 7, 7, 2048, 1, 1) == 144 // 8 * 4
+    # BN statistics rows: (persistent CTAs / channel blocks) x 4 row quadrants (x2 when the warp pair alternates tiles);
+    # without a device the planner assumes the 132 SMs of an H100 SXM; channel blocks are 64 or 128 wide
+    assert lib.b200_conv2d_fwd_stats_rows(256, 56, 56, 64, 3, 1) == 132 * 8
+    assert lib.b200_conv2d_fwd_stats_rows(256, 56, 56, 256, 1, 1) == 132 // 2 * 4
+    assert lib.b200_conv2d_fwd_stats_rows(256, 7, 7, 2048, 1, 1) == 128 // 16 * 4
     assert lib.b200_conv2d_fwd_stats_rows(1, 8, 8, 64, 1, 1) == 8
     assert lib.b200_conv2d_wgrad_workspace_bytes(256, 56, 56, 64, 64, 3, 1) > 0
     assert lib.b200_bn_bwd_blocks(256 * 56 * 56, 64) > 0
@@ -65,7 +66,7 @@ def test_missing_library_fails_loudly(monkeypatch):
 def test_wgrad_split_plan_is_one_wave_and_bounded():
     """Split-K plan of the weight-gradient GEMM (abi_conv.cu: plan_wgrad_geom), read back through the workspace size:
     workspace = splits * Cout * taps * Cin * 4 bytes. The cost model must keep (output tiles x splits) within one or two
-    waves of the 148 SMs (no third, mostly empty wave) and never ask for an absurd amount of fp32 partials."""
+    waves of the 132 SMs of an H100 SXM (no third, mostly empty wave) and never ask for an absurd amount of fp32 partials."""
     from deeplearning_b200 import _lib
 
     lib = _lib.load()
@@ -92,6 +93,6 @@ def test_wgrad_split_plan_is_one_wave_and_bounded():
         pixel_blocks = -(-(B * (H // s) * (W // s)) // 64)
         assert 1 <= sp <= max(1, pixel_blocks // 4), (B, H, W, Cin, Cout, k, sp)
         items = tiles(Cin, Cout, k * k, merged) * sp
-        if tiles(Cin, Cout, k * k, merged) <= 148:
-            assert items <= 2 * 148, ("more than two waves", B, H, W, Cin, Cout, k, sp, items)
+        if tiles(Cin, Cout, k * k, merged) <= 132:
+            assert items <= 2 * 132, ("more than two waves", B, H, W, Cin, Cout, k, sp, items)
         assert sp * Cout * k * k * Cin * 4 <= 256 << 20   # at most 256 MB of partials per layer

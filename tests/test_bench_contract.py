@@ -1,5 +1,5 @@
 """bench.py contract on the CPU side: the reference arm prints exactly ONE JSON line on stdout with the keys the driver
-reads, and the B200 arm refuses to run without a GPU instead of falling back to the CPU."""
+reads, and the GPU arm refuses to run without a GPU instead of falling back to the CPU."""
 import json
 import os
 import subprocess

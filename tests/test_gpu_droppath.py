@@ -1,4 +1,4 @@
-"""Stochastic depth (drop_path) and ViT pre_logits on the B200 engines, against the CPU oracle with SHARED per-sample masks
+"""Stochastic depth (drop_path) and ViT pre_logits on the GPU engines, against the CPU oracle with SHARED per-sample masks
 (SURVEY.md 7.3): the reference's default constructors - convnext_tiny() (rate 0.2), SwinTransformer() (0.1),
 vit_base_patch16_224_in21k() (has_logits=True) - train on the drop-in without raising."""
 import pytest

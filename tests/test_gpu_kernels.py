@@ -1,4 +1,4 @@
-"""GPU parity tests of the individual sm_100a kernels against a plain PyTorch fp32 reference of the same op.
+"""GPU parity tests of the individual sm_90a kernels against a plain PyTorch fp32 reference of the same op.
 
 Inputs are rounded to bf16 first so that the only differences are accumulation order and the bf16 rounding of outputs.
 """

@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 ResNet path against the CPU oracle (fp32) on the same weights and inputs."""
+"""End-to-end parity of the GPU ResNet path against the CPU oracle (fp32) on the same weights and inputs."""
 import pytest
 import torch
 import torch.nn.functional as F

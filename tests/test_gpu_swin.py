@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 Swin-T path against the CPU oracle (fp32) on the same weights and inputs, plus the
+"""End-to-end parity of the GPU Swin-T path against the CPU oracle (fp32) on the same weights and inputs, plus the
 kernels/window_process drop-in (SURVEY seam B2) against its torch definition (the reference's own unit_test.py protocol)."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 ViT path against the CPU oracle (fp32) on the same weights and inputs."""
+"""End-to-end parity of the GPU ViT path against the CPU oracle (fp32) on the same weights and inputs."""
 import pytest
 import torch
 import torch.nn.functional as F

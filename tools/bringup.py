@@ -1,4 +1,4 @@
-"""Bring-up diagnostics for the tcgen05 kernels (run on the GPU box): python tools/bringup.py [fwd|wgrad|perf]"""
+"""Bring-up diagnostics for the wgmma kernels (run on an H100): python tools/bringup.py [fwd|wgrad|perf]"""
 import os
 import sys
 import time

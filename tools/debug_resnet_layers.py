@@ -1,4 +1,4 @@
-"""Layer-by-layer error growth of the B200 ResNet-50 forward vs an fp32 PyTorch run, next to torch-autocast(bf16)'s own
+"""Layer-by-layer error growth of the GPU ResNet-50 forward vs an fp32 PyTorch run, next to torch-autocast(bf16)'s own
 error on the same weights/inputs (yardstick for what bf16 storage costs). python tools/debug_resnet_layers.py [B] [train|eval]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -2,7 +2,7 @@
 
 Question: the big (256 / 512-channel) tensors of a bottleneck are written by one kernel and re-read by the next one or two.
 If the chain is run per batch chunk (NHWC batch slices are contiguous) with the intermediate in a chunk-sized buffer that
-is re-used by every chunk, does the 126 MB L2 keep the intermediate on chip (no HBM write, no HBM re-read)?
+is re-used by every chunk, does the 50 MB L2 keep the intermediate on chip (no HBM write, no HBM re-read)?
 
 Chains (layer1: 56x56, 64/256 channels; layer2: 28x28, 128/512):
   tail : bn_bwd_apply(dz, c3 -> dc3)  ->  wgrad(dc3, y2)  ->  dgrad(dc3 -> g2)

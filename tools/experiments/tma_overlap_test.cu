@@ -1,6 +1,6 @@
 // Does cuTensorMapEncodeTiled accept OVERLAPPING rows (stride[1] < dim[0] * elemsize) and does the TMA load them correctly?
 // (Needed for a space-to-depth ResNet stem: 4 x-taps x 16 ch = 64 contiguous elements per pixel, pixel stride 16 elements.)
-// nvcc -gencode arch=compute_100a,code=sm_100a -o tma_overlap_test tma_overlap_test.cu -lcuda
+// nvcc -gencode arch=compute_90a,code=sm_90a -o tma_overlap_test tma_overlap_test.cu -lcuda
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

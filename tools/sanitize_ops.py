@@ -1,4 +1,4 @@
-"""One small launch of every tcgen05 / TMA kernel family, for `compute-sanitizer --tool {memcheck,racecheck,synccheck}`:
+"""One small launch of every wgmma / TMA kernel family, for `compute-sanitizer --tool {memcheck,racecheck,synccheck}`:
 implicit-GEMM conv (forward + statistics, dgrad + residual, affine / mask epilogues, dual-source K), the streaming 1x1 kernel
 (both modes), wgrad, ViT attention forward / backward, window attention forward / backward, BN-algebra kernels.
 usage: compute-sanitizer --tool racecheck python tools/sanitize_ops.py [family ...]"""
@@ -76,8 +76,8 @@ if "wattn" in fam:
     dqkv, dbias = ops.window_attention_bwd(qkv, o, r(B, H, W, C), bias, lse, nH, 0, 32 ** -0.5)
     print("wattn ok", float(o.float().abs().mean()), float(dqkv.float().abs().mean()))
 if "attn2" in fam:
-    # persistent attention forward (attention_fwd2.cuh): 300 (batch, head) items on 148 CTAs, i.e. two or three items per CTA
-    # (buffer reuse, barrier phases, the ping-pong of the two soft-max groups), checked against the per-block kernel's math
+    # persistent attention forward (attention_fwd2.cuh): 300 (batch, head) items on 132 CTAs, i.e. two or three items per CTA
+    # (buffer reuse, barrier phases of the two query-block warpgroups), checked against PyTorch soft-max attention
     qkv = r(100, 197, 3 * 3 * 64, scale=0.5)
     o, lse = ops.attention_fwd(qkv, 3, 0.125)
     q, k, v = qkv[:2].float().view(2, 197, 3, 3, 64).permute(2, 0, 3, 1, 4)

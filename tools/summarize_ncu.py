@@ -1,7 +1,7 @@
-"""Condense `ncu --page raw --csv` exports / launch lists into the small tables committed under profiles/.
+"""Condense `ncu --page raw --csv` exports / launch lists into small markdown tables.
 usage: python tools/summarize_ncu.py raw <in.csv> <out.md> | launches <in.csv> <out.md> | traffic <in.csv> <out.md> <model>
 ("traffic": launch list taken with gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum; also refreshes the
-model's entry of profiles/roofline_traffic.json, which bench.py reads for roofline.traffic)"""
+model's entry of profiles/roofline_traffic.json, which bench.py reads for roofline.traffic when it exists)"""
 import json
 import os
 import collections
@@ -77,7 +77,7 @@ _SCALE = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "ns": 1e-3, "us
 # bench.py span name -> ncu kernel names whose bytes belong to it (a span covers the kernels one C-ABI entry point launches)
 _SPANS = {"wgrad_gemm": ("wgrad_gemm_kernel", "wgrad_reduce_rows_kernel", "wgrad_reduce_flat_kernel"),
           "bn_bwd_reduce": ("bn_bwd_reduce_kernel",), "bn_bwd_apply": ("bn_bwd_apply_kernel",),
-          "bn_apply": ("bn_apply_kernel",), "attention_fwd": ("attn_fwd_kernel", "attn_fwd2_kernel"),
+          "bn_apply": ("bn_apply_kernel",), "attention_fwd": ("attn_fwd2_kernel",),
           "attention_bwd": ("attn_bwd_kernel", "attn_delta_kernel"),
           "window_attention_fwd": ("wattn_fwd_kernel",), "window_attention_bwd": ("wattn_bwd_kernel",),
           "layernorm_fwd": ("layernorm_fwd_kernel",), "layernorm_bwd": ("layernorm_bwd_kernel", "layernorm_bwd2_kernel"),
@@ -142,7 +142,7 @@ def traffic(inp, out, model):
     allm[model] = per
     allm["_note"] = {"what": "DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum, averaged over the launches of "
                              "one training step) for every bench.py kernel span, per model; wgrad_gemm includes its reduce pass",
-                     "source": "tools/summarize_ncu.py traffic on the launch lists under profiles/ (r02_*_launches.md; r01_*_launches_final.md for models not re-profiled)"}
+                     "source": "tools/summarize_ncu.py traffic on an ncu launch list"}
     json.dump(allm, open(tpath, "w"), indent=1)
 
 

@@ -1,5 +1,5 @@
 """Time the ViT attention forward / backward ops alone (CUDA events, qkv of 232 MB per call > L2).
-python tools/time_attention.py [B] [T] [H]      (B200_ATTN_FWD=1|2 selects the forward kernel)"""
+python tools/time_attention.py [B] [T] [H]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -35,5 +35,5 @@ err = (att[:4].float().view(4, T, H, 64).permute(0, 2, 1, 3) - ref).abs().max().
 t_f = timed(lambda: ops.attention_fwd(qkv, H, scale))
 t_b = timed(lambda: ops.attention_bwd(qkv, att, dout, lse, H, scale))
 fl = 4.0 * B * H * T * T * 64
-print(f"attention B={B} T={T} H={H} fwd kernel {os.environ.get('B200_ATTN_FWD', '1')}: fwd {t_f:.1f} us ({fl / t_f / 1e6:.0f} TFLOP/s) "
+print(f"attention B={B} T={T} H={H} : fwd {t_f:.1f} us ({fl / t_f / 1e6:.0f} TFLOP/s) "
       f"bwd(+delta) {t_b:.1f} us ({2.5 * fl / t_b / 1e6:.0f} TFLOP/s)  max|err| vs fp32 {err:.2e}")
