@@ -507,8 +507,8 @@ int b200_conv2d_fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int str
   const int n_tiles = (Cout + BN - 1) / BN;
   const long long tiles = m_tiles * n_tiles;
   const int grid = conv_grid(tiles > (1 << 30) ? (1 << 30) : static_cast<int>(tiles), n_tiles, true);
-  // one partial row per (CTA group, 32-row quadrant); the two warps of a quadrant write separate rows when they alternate
-  // tiles (64-channel tiles) and disjoint column units of one row otherwise
+  // one partial row per (CTA group, 32-row quadrant); with 64-channel tiles two, one per parity of the CTA's tile count
+  // (the layout conv_tap64_kernel shares)
   return grid / n_tiles * (BN == 64 ? 8 : 4);
 }
 

@@ -7,12 +7,13 @@
 //   out-of-image pixels are zero-filled by the TMA unit, which is the convolution's zero padding. Stride-2 convolutions
 //   pass up to four "phase" views (even/odd rows x cols) of the input as separate tensor maps.
 // * B (weights, [Cout][taps*Cin] bf16) is a 2-D TMA box of BLOCK_N rows x 64 k.
-// * Two consumer warpgroups each multiply 64 rows of the 128-row tile with wgmma (m64 x BLOCK_N x k16) into registers; the
-//   TMA producer (warpgroup 0) keeps a ring of k-block stages full, also while the consumers run the epilogue of the previous tile.
-//   The kernel is persistent: grid = min(tiles, #SM).
-// * Epilogue: each warpgroup stores its accumulator into a shared-memory image and its four warps drain it one row per
-//   thread: (+bias, activation, +residual) -> bf16 -> swizzled smem staging -> TMA store, plus optional per-channel sum /
-//   sum-of-squares partials (train-mode BatchNorm statistics).
+// * Two MMA warpgroups each multiply 64 rows of the 128-row tile with wgmma (m64 x BLOCK_N x k16) into registers; the
+//   TMA producer (warpgroup 0) keeps a ring of k-block stages full. The kernel is persistent: grid = min(tiles, #SM).
+// * Epilogue: the MMA warpgroups store their accumulator into a shared-memory image (mbarrier img_full) and go straight on
+//   to the next tile's main loop; a dedicated epilogue warpgroup drains the image one row per thread (mbarrier img_empty
+//   hands it back): (+bias, activation, +residual) -> bf16 -> swizzled smem staging -> TMA store, plus optional
+//   per-channel sum / sum-of-squares partials (train-mode BatchNorm statistics). The tensor cores therefore only wait for
+//   the epilogue when it takes longer than a main loop.
 //
 // Replaces the cuDNN/cuBLAS calls behind nn.Conv2d / nn.Linear on the reference's hot path
 // (classification/resnet/models/networks.py:27-35,104-124; classification/vision_transformer/vit_model.py:95,109,127-133).
@@ -83,16 +84,20 @@ struct ConvGemmCfg {
   static constexpr int BLOCK_K = 64;
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
-  static constexpr int STAGES = BLOCK_N == 128 ? 3 : 5;
+  static constexpr int STAGES = BLOCK_N == 128 ? 4 : 5;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int EPI_WARPS = 8;
+  static constexpr int EPI_WARPS = 4;
   static constexpr int SLAB_BYTES = 32 * 128;                       // one warp's 32 rows x 128 B
   static constexpr int STAGING_BYTES = EPI_WARPS * 2 * SLAB_BYTES;  // double-buffered per warp
   static constexpr int IMG_BYTES = BLOCK_M * BLOCK_N * 4;           // fp32 accumulator image
+  // 64-column tiles have room for a second image: the MMA warpgroups can hand over the next tile while the epilogue
+  // still drains this one (128-column tiles use that room for a fourth k-stage instead)
+  static constexpr int IMGS = BLOCK_N == 128 ? 1 : 2;
   static constexpr int BAR_BYTES = 256;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + IMG_BYTES + BAR_BYTES + 1024;
-  static constexpr int THREADS = 384;   // warpgroup 0: TMA producer, warpgroups 1-2: consumers
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + IMGS * IMG_BYTES + BAR_BYTES + 1024;
+  static constexpr int THREADS = 512;   // warpgroup 0: TMA producer, 1-2: MMA, 3: epilogue
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
+  static_assert(2 * STAGES + 2 * IMGS <= BAR_BYTES / 8, "mbarriers");
 };
 
 // Exact-erf GELU (nn.GELU() of the reference: vit_model.py:121, swin_transformer.py:20, convNext/models/networks.py:84) with
@@ -171,6 +176,20 @@ __device__ __forceinline__ void gelu_erf_val_grad2(float& x0, float& x1, float& 
 #define CPROF_TICK(i)
 #endif
 
+// One step of the warp's column-sum butterfly: px[i] += the partner lane's px[i + S] (or px[i] for the upper half), so that
+// after steps 16 .. 1 px[0] of lane l holds column l summed over the 32 lanes. A template so that the loop is unrolled and
+// px stays in registers (with a run-time step it was placed in local memory).
+template <int S>
+__device__ __forceinline__ void butterfly_step(float (&px)[32], int lane) {
+  const bool up = (lane & S) != 0;
+#pragma unroll
+  for (int i = 0; i < S; ++i) {
+    const float send = up ? px[i] : px[i + S];
+    const float keep = up ? px[i + S] : px[i];
+    px[i] = keep + __shfl_xor_sync(0xffffffffu, send, S);
+  }
+}
+
 // Epilogue specialisation: EPI < 0 keeps every epilogue option a run-time flag (generic fallback); EPI >= 0 is a bit set
 // of compile-time options so that the hot layer types get a branch-free epilogue without the unused operand loads.
 constexpr int kEpiGeneric = -1;
@@ -187,29 +206,28 @@ constexpr int kEpiBias = 1, kEpiColscale = 2, kEpiActShift = 2 /* 2 bits */, kEp
               kEpiAffine = 2048, kEpiMask = 4096, kEpiBnMask = 8192;
 
 template <int BLOCK_N, int EPI = kEpiGeneric>
-__global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
+__global__ void __launch_bounds__(512, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
   pdl_launch_dependents();
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "64- or 128-column tiles");
   using Cfg = ConvGemmCfg<BLOCK_N>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int IMGS = Cfg::IMGS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_base = smem;
   uint8_t* staging = smem + STAGES * Cfg::STAGE_BYTES;
   uint8_t* img = staging + Cfg::STAGING_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(img + Cfg::IMG_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(img + IMGS * Cfg::IMG_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
+  uint64_t* img_full = bars + 2 * STAGES;           // image i holds a finished accumulator (8 MMA warps arrive)
+  uint64_t* img_empty = bars + 2 * STAGES + IMGS;   // image i has been read by the epilogue (4 epilogue warps arrive)
 
   const int warp_idx = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int m_tiles = p.tiles1 * p.tiles2 * p.tiles3;
   const int num_tiles = m_tiles * p.n_tiles;
   const int num_kb = p.var_taps ? p.kb_total : p.num_taps * p.k_blocks_per_tap;
-  // Epilogue work units: 64 bf16 (or 32 fp32) channels x one warp's 32 rows. Two warps share a 32-row quadrant and
-  // take alternate units; with a single unit per tile the second warp of each pair has nothing to do.
-  const int unit_cols = ((EPI < 0) ? (p.out_f32 != 0) : ((EPI & kEpiOutF32) != 0)) ? 32 : 64;
-  const int units = BLOCK_N / unit_cols;
 
   if (warp_idx == 0 && lane == 0) {
     for (int i = 0; i < 4; ++i) tma_prefetch_desc(&p.a_maps[i]);
@@ -217,7 +235,11 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
     tma_prefetch_desc(&p.d_map);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2);   // one arrive per consumer warpgroup
+      mbar_init(&empty_bar[i], 2);   // one arrive per MMA warpgroup
+    }
+    for (int i = 0; i < IMGS; ++i) {
+      mbar_init(&img_full[i], 8);
+      mbar_init(&img_empty[i], Cfg::EPI_WARPS);
     }
     fence_mbar_init();
   }
@@ -269,61 +291,16 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
       }
 #endif
     }
-  } else {
-    // ===================== Two consumer warpgroups: wgmma main loop, then the epilogue of their 64 rows =====================
-    // Warpgroup wg owns tile rows 64 wg .. 64 wg + 63: it multiplies them into registers, hands the accumulator to its own
-    // four warps through the shared-memory image and drains it: warp `ew` owns the 32-row quadrant q (q = 2 wg, 2 wg + 1)
-    // and, with its partner warp of the same quadrant, alternate 64-column units.
-    setmaxnreg_inc<232>();
-    const int ew = warp_idx - 4;
-    const int wg = ew >> 2;
-    const int q = 2 * wg + (ew & 1);   // 32-row quadrant of the tile this warp drains
-    const int pair = (ew >> 1) & 1;    // which of the two warps sharing the quadrant
-    const int row = q * 32 + lane;
-    const uint32_t img_s = smem_u32(img);
+  } else if (warp_idx < 12) {
+    // ===================== Two MMA warpgroups: wgmma main loop, accumulator -> image =====================
+    // Warpgroup wg owns tile rows 64 wg .. 64 wg + 63. It waits for the epilogue only right before it overwrites an image
+    // the epilogue has not finished reading.
+    setmaxnreg_dec<112>();
+    const int wg = (warp_idx - 4) >> 2;
     const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(stage_base) + wg * 8192, p.desc_lbo, p.desc_sbo);
     const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(stage_base) + Cfg::A_BYTES, p.desc_lbo, p.desc_sbo);
     int stage = 0;
     uint32_t phase = 0;
-    const uint32_t stage_s = smem_u32(staging + ew * 2 * Cfg::SLAB_BYTES);
-    const uint32_t row_s = lane * 128;          // this thread's row inside a slab
-    const uint32_t sw = (lane & 7) << 4;        // 128B-swizzle XOR term of that row
-    // statistics read-back: lane owns columns 2*lane, 2*lane+1 -> 4-byte word `lane` of every row
-    uint32_t stat_off[8];
-#pragma unroll
-    for (int m = 0; m < 8; ++m) stat_off[m] = m * 128 + ((((lane >> 2) ^ m) << 4) | ((lane & 3) << 2));
-    // kernel parameters used in the inner loops, hoisted into registers
-    constexpr bool G = EPI < 0;
-    constexpr bool kAffine = !G && (EPI & kEpiAffine) != 0;   // BatchNorm scale / shift, ReLU after the residual add
-    constexpr bool kBnMask = !G && (EPI & kEpiBnMask) != 0;   // ReLU mask recomputed from the raw BN input + sum(dz * x)
-    constexpr bool kMask = !G && (EPI & (kEpiMask | kEpiBnMask)) != 0;   // a second tensor decides which outputs survive
-    const int N = p.N;
-    const float* const bias = (!kAffine && (G || (EPI & kEpiBias))) ? p.bias : nullptr;
-    const float* const colscale = (!kAffine && (G || (EPI & kEpiColscale))) ? p.colscale : nullptr;
-    const int act_bits = G ? p.act : ((EPI >> kEpiActShift) & 3);
-    const int act = kAffine ? 0 : act_bits;                   // (kAffine: the activation is applied after the residual)
-    const bool has_res = G ? (p.residual != nullptr) : ((EPI & (kEpiResBf16 | kEpiResF32)) != 0);
-    const bool res_f32 = G ? (p.res_f32 != 0) : ((EPI & kEpiResF32) != 0);
-    const bool has_aux = G ? (p.has_aux_out != 0) : ((EPI & kEpiAux) != 0);
-    const bool out_f32 = G ? (p.out_f32 != 0) : ((EPI & kEpiOutF32) != 0);
-    float* const out_direct = (G || (EPI & kEpiDirect)) ? p.out_direct : nullptr;
-    float* const stats = (G || (EPI & (kEpiStats | kEpiBnMask))) ? p.stats : nullptr;
-    const float* const rowscale = G ? p.rowscale : nullptr;
-    const bool need_rowmap = has_res || act == 3 || kMask || out_direct != nullptr || rowscale != nullptr || p.dim1 % p.box1 != 0 ||
-                             p.dim2 % p.box2 != 0 || p.dim3 % p.box3 != 0;
-    const bool full_cols = (N % BLOCK_N) == 0;  // no partially valid 32-column group anywhere
-    uint32_t store_counter = 0;
-    const int nsub = out_f32 ? 1 : 2;  // 32-column image loads per unit
-    const bool split_tiles = units < 2;  // single unit: the pair alternates tiles
-    const int u_first = split_tiles ? 0 : pair;
-    // Train-mode BN statistics: every epilogue warp keeps running column sums of the slabs it stored (its 32 rows x
-    // its 64-column units; the launch guarantees grid % n_tiles == 0, so a CTA always sees the same channel block) and
-    // writes ONE partial row at the end of the kernel.
-    constexpr int UN = BLOCK_N >= 128 ? BLOCK_N / 128 : 1;
-    uint64_t run_s[UN], run_q[UN];
-    float run_x[UN][2];   // kBnMask: sum(dz * x) of column (unit k, half h, lane)
-#pragma unroll
-    for (int k = 0; k < UN; ++k) run_s[k] = 0, run_q[k] = 0, run_x[k][0] = run_x[k][1] = 0.f;
     int it = 0;
     CPROF_DECL(3)
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
@@ -353,10 +330,72 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
       wgmma_reg_fence(acc);
       if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
       CPROF_TICK(0)
-      named_bar_sync(1 + wg, 128);   // this warpgroup's epilogue of the previous tile has read the image
-      acc_to_img<BLOCK_N>(acc, img_s, BLOCK_N, 64 * wg, 0);
-      named_bar_sync(1 + wg, 128);
-      if (split_tiles && (it & 1) != pair) continue;
+      const int b = IMGS == 1 ? 0 : it % IMGS;
+      mbar_wait(&img_empty[b], ((it / IMGS) & 1) ^ 1);   // (passes at once on the first use of each image)
+      CPROF_TICK(1)
+      acc_to_img<BLOCK_N>(acc, smem_u32(img + b * Cfg::IMG_BYTES), BLOCK_N, 64 * wg, 0);
+      __syncwarp();   // the warp's image stores happen before lane 0's (release) arrive
+      if (lane == 0) mbar_arrive(&img_full[b]);
+    }
+#ifdef CONV_PROFILE
+    if (blockIdx.x == 0 && lane == 0 && (warp_idx & 3) == 0) {
+      const int nt = (num_tiles - 1) / gridDim.x + 1;
+      printf("conv mma wg %d: main loop %lld wait img_empty %lld acc->img %lld  (cycles/tile)\n", wg, cp_t[0] / nt, cp_t[1] / nt,
+             cp_t[2] / nt);
+    }
+#endif
+  } else {
+    // ===================== Epilogue warpgroup: drains the image one row per thread =====================
+    // Warp q owns the 32-row quadrant q of every tile, over all of its column units.
+    setmaxnreg_inc<248>();
+    const int q = warp_idx - 12;
+    const int row = q * 32 + lane;
+    const uint32_t stage_s = smem_u32(staging + q * 2 * Cfg::SLAB_BYTES);
+    const uint32_t row_s = lane * 128;          // this thread's row inside a slab
+    const uint32_t sw = (lane & 7) << 4;        // 128B-swizzle XOR term of that row
+    // statistics read-back: lane owns columns 2*lane, 2*lane+1 -> 4-byte word `lane` of every row
+    uint32_t stat_off[8];
+#pragma unroll
+    for (int m = 0; m < 8; ++m) stat_off[m] = m * 128 + ((((lane >> 2) ^ m) << 4) | ((lane & 3) << 2));
+    // kernel parameters used in the inner loops, hoisted into registers
+    constexpr bool G = EPI < 0;
+    constexpr bool kAffine = !G && (EPI & kEpiAffine) != 0;   // BatchNorm scale / shift, ReLU after the residual add
+    constexpr bool kBnMask = !G && (EPI & kEpiBnMask) != 0;   // ReLU mask recomputed from the raw BN input + sum(dz * x)
+    constexpr bool kMask = !G && (EPI & (kEpiMask | kEpiBnMask)) != 0;   // a second tensor decides which outputs survive
+    const int N = p.N;
+    const float* const bias = (!kAffine && (G || (EPI & kEpiBias))) ? p.bias : nullptr;
+    const float* const colscale = (!kAffine && (G || (EPI & kEpiColscale))) ? p.colscale : nullptr;
+    const int act_bits = G ? p.act : ((EPI >> kEpiActShift) & 3);
+    const int act = kAffine ? 0 : act_bits;                   // (kAffine: the activation is applied after the residual)
+    const bool has_res = G ? (p.residual != nullptr) : ((EPI & (kEpiResBf16 | kEpiResF32)) != 0);
+    const bool res_f32 = G ? (p.res_f32 != 0) : ((EPI & kEpiResF32) != 0);
+    const bool has_aux = G ? (p.has_aux_out != 0) : ((EPI & kEpiAux) != 0);
+    const bool out_f32 = G ? (p.out_f32 != 0) : ((EPI & kEpiOutF32) != 0);
+    float* const out_direct = (G || (EPI & kEpiDirect)) ? p.out_direct : nullptr;
+    float* const stats = (G || (EPI & (kEpiStats | kEpiBnMask))) ? p.stats : nullptr;
+    const float* const rowscale = G ? p.rowscale : nullptr;
+    const bool need_rowmap = has_res || act == 3 || kMask || out_direct != nullptr || rowscale != nullptr || p.dim1 % p.box1 != 0 ||
+                             p.dim2 % p.box2 != 0 || p.dim3 % p.box3 != 0;
+    const bool full_cols = (N % BLOCK_N) == 0;  // no partially valid 32-column group anywhere
+    uint32_t store_counter = 0;
+    // Work units: 64 bf16 (or 32 fp32) channels x the warp's 32 rows
+    const int unit_cols = out_f32 ? 32 : 64;
+    const int units = BLOCK_N / unit_cols;
+    const int nsub = out_f32 ? 1 : 2;  // 32-column image loads per unit
+    // Train-mode BN statistics: every epilogue warp keeps running column sums of the slabs it stored (the launch guarantees
+    // grid % n_tiles == 0, so a CTA always sees the same channel block) and writes them out at the end of the kernel, in
+    // one of two slots: the 64-column unit of a 128-column tile (both slots share a partial row), or for 64-column tiles
+    // the parity of the CTA's tile count (two partial rows per quadrant, the layout conv_tap64_kernel shares).
+    constexpr int SLOTS = 2;
+    uint64_t run_s[SLOTS], run_q[SLOTS];
+    float run_x[SLOTS][2];   // kBnMask: sum(dz * x) of column (slot k, half h, lane)
+#pragma unroll
+    for (int k = 0; k < SLOTS; ++k) run_s[k] = 0, run_q[k] = 0, run_x[k][0] = run_x[k][1] = 0.f;
+    int it = 0;
+    CPROF_DECL(2)
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+      const int b = IMGS == 1 ? 0 : it % IMGS;
+      const uint32_t img_s = smem_u32(img + b * Cfg::IMG_BYTES);
       const int n_tile = tile % p.n_tiles;
       const int m_tile = tile / p.n_tiles;
       const int t1 = m_tile % p.tiles1;
@@ -410,10 +449,13 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
             if (full_cols || ncp + j * 8 < N) nx_m[j] = __ldg(mp + j);
         }
       };
-      if (has_res || act == 3 || kMask) issue_pre(u_first, 0);
+      if (has_res || act == 3 || kMask) issue_pre(0, 0);   // (they do not depend on the accumulator)
+      CPROF_TICK(1)
+      mbar_wait(&img_full[b], (it / IMGS) & 1);
+      CPROF_TICK(0)
 
 #pragma unroll 1
-      for (int u = u_first; u < units; u += 2) {
+      for (int u = 0; u < units; ++u) {
         const int n0 = n_tile * BLOCK_N + u * unit_cols;
         const bool chunk_live = n0 < N;  // warp-uniform
         const uint32_t buf_s = stage_s + (store_counter & 1) * Cfg::SLAB_BYTES;
@@ -429,6 +471,11 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
         for (int h = 0; h < nsub; ++h) {
           uint32_t v[32];
           img_ld32(img_s, BLOCK_N, row, u * unit_cols + h * 32, v);
+          if (u == units - 1 && h == nsub - 1) {
+            // the last image read of this tile: the MMA warpgroups may overwrite the image (release orders the loads)
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&img_empty[b]);
+          }
           uint4 pre_b[4];
           float4 pre_f[8];
           uint4 pre_m[4];
@@ -443,8 +490,8 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
             }
             if (h + 1 < nsub)
               issue_pre(u, h + 1);
-            else if (u + 2 < units)
-              issue_pre(u + 2, 0);
+            else if (u + 1 < units)
+              issue_pre(u + 1, 0);
           }
           if (!chunk_live) continue;
           const int nc = n0 + h * 32;  // first channel of this 32-column group
@@ -587,20 +634,15 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
 #pragma unroll
               for (int j = 0; j < 32; ++j) px[j] = 0.f;
             }
+            butterfly_step<16>(px, lane);
+            butterfly_step<8>(px, lane);
+            butterfly_step<4>(px, lane);
+            butterfly_step<2>(px, lane);
+            butterfly_step<1>(px, lane);
+            const int slot = units == 1 ? (it & 1) : u;
 #pragma unroll
-            for (int s = 16; s >= 1; s >>= 1) {
-              const bool up = (lane & s) != 0;
-#pragma unroll
-              for (int i = 0; i < s; ++i) {
-                const float send = up ? px[i] : px[i + s];
-                const float keep = up ? px[i + s] : px[i];
-                px[i] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-              }
-            }
-            const int ui = u >> 1;
-#pragma unroll
-            for (int k = 0; k < UN; ++k) {
-              if (k == ui) {
+            for (int k = 0; k < SLOTS; ++k) {
+              if (k == slot) {
                 run_x[k][0] += h == 0 ? px[0] : 0.f;
                 run_x[k][1] += h == 0 ? 0.f : px[0];
               }
@@ -660,10 +702,10 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
             a_s = f2_add(a_s, x2);
             a_q = f2_fma(x2, x2, a_q);
           }
-          const int ui = u >> 1;
+          const int slot = units == 1 ? (it & 1) : u;
 #pragma unroll
-          for (int k = 0; k < UN; ++k) {
-            if (k == ui) {
+          for (int k = 0; k < SLOTS; ++k) {
+            if (k == slot) {
               run_s[k] = f2_add(run_s[k], a_s);
               run_q[k] = f2_add(run_q[k], a_q);
             }
@@ -690,21 +732,20 @@ __global__ void __launch_bounds__(384, 1) conv_gemm_kernel(const __grid_constant
       }
     }
 #ifdef CONV_PROFILE
-    if (blockIdx.x == 0 && lane == 0 && (ew == 0 || ew == 4)) {
+    if (blockIdx.x == 0 && lane == 0 && q == 0) {
       const int nt = (num_tiles - 1) / gridDim.x + 1;
-      printf("conv consumer warp %d: main loop %lld epilogue %lld  (cycles/tile)\n", ew, cp_t[0] / nt, cp_t[2] / nt);
+      printf("conv epilogue: wait img_full %lld drain %lld  (cycles/tile)\n", cp_t[0] / nt, cp_t[1] / nt);
     }
 #endif
     if (stats != nullptr) {
       const int cta = static_cast<int>(blockIdx.x);
       const int n_tile = cta % p.n_tiles;
       const int grp = cta / p.n_tiles;
-      const int srow = split_tiles ? (grp * 4 + q) * 2 + pair : grp * 4 + q;
 #pragma unroll
-      for (int k = 0; k < UN; ++k) {
-        const int u = u_first + 2 * k;
-        const int col = n_tile * BLOCK_N + u * unit_cols + 2 * lane;
-        if (u < units && col < N) {
+      for (int k = 0; k < SLOTS; ++k) {
+        const int srow = units == 1 ? (grp * 4 + q) * 2 + k : grp * 4 + q;
+        const int col = n_tile * BLOCK_N + (units == 1 ? 0 : k * unit_cols) + 2 * lane;
+        if (col < N) {
           float s_lo, s_hi, q_lo, q_hi;
           f2_unpack(run_s[k], s_lo, s_hi);
           f2_unpack(run_q[k], q_lo, q_hi);
