@@ -62,6 +62,11 @@ SIGNATURES = {
     "b200_conv2d_wgrad_set_bias_partial": (_I, [_P]),
     "b200_conv2d_wgrad_set_bias_out": (_I, [_P]),
     "b200_conv2d_wgrad_splits": (_I, [_I, _I, _I, _I, _I, _I, _I]),
+    "b200_conv2d_grouped_fwd": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
+    "b200_conv2d_grouped_fwd_stats_rows": (_I, [_I, _I, _I, _I, _I, _I, _I]),
+    "b200_conv2d_grouped_dgrad": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_conv2d_grouped_wgrad": (_I, [_P, _P, _P, _P, c_size_t, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_conv2d_grouped_wgrad_workspace_bytes": (c_size_t, [_I, _I, _I, _I, _I, _I, _I]),
     "b200_dwconv7_pack": (_I, [_P, _P, _I, _P]),
     "b200_dwconv7": (_I, [_P, _I, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "b200_dwconv7_wgrad_workspace_bytes": (c_size_t, [_I, _I, _I, _I]),

@@ -240,7 +240,7 @@ bool tap64_enabled() {
 }
 bool tap64_ok(const ConvGemmParams& p) {
   const int f = epilogue_flags(p);
-  return tap64_enabled() && p.N == 64 && p.n_tiles == 1 && p.k_per_tap == 64 && p.k_blocks_per_tap == 1 && !p.var_taps &&
+  return tap64_enabled() && p.N == 64 && p.n_tiles == 1 && p.k_per_tap == 64 && p.k_blocks_per_tap == 1 && !p.var_taps && !p.chan_window &&
          p.num_taps >= 2 && p.num_taps <= 9 && (f == 0 || f == kEpiStats) && p.dim1 % p.box1 == 0 && p.dim2 % p.box2 == 0 &&
          p.dim3 % p.box3 == 0;
 }
@@ -359,15 +359,20 @@ int dispatch_conv_gemm(ConvGemmParams& p, int N, cudaStream_t st) {
 }
 int block_n_for(int N) { return N <= 64 ? 64 : 128; }
 
-template <int BLOCK_NG>
+template <int BLOCK_NG, bool kGrouped = false>
 int launch_wgrad(const WgradParams& p, cudaStream_t st) {
   using Cfg = WgradCfg<BLOCK_NG>;
   static bool configured = false;
   if (!configured) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BLOCK_NG, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES));
-    B200_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BLOCK_NG, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES));
+    if constexpr (kGrouped) {
+      B200_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BLOCK_NG, false, true>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    } else {
+      B200_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BLOCK_NG, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           Cfg::SMEM_BYTES));
+      B200_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BLOCK_NG, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           Cfg::SMEM_BYTES));
+    }
     configured = true;
   }
   const int items = p.mg_tiles * p.ng_tiles * p.num_taps * p.splits;
@@ -376,7 +381,9 @@ int launch_wgrad(const WgradParams& p, cudaStream_t st) {
   q.desc_lbo = g_wg_lbo;
   q.desc_sbo = g_wg_sbo;
   q.desc_kstep = g_wg_kstep;
-  if (q.bias_partial != nullptr)   // + four warps that sum the dY tiles' columns (the layer's bias gradient)
+  if constexpr (kGrouped)
+    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, false, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
+  else if (q.bias_partial != nullptr)   // + four warps that sum the dY tiles' columns (the layer's bias gradient)
     B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
   else
     B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, false>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
@@ -414,7 +421,8 @@ struct WgradPlan {
   int Ho, Wo;
 };
 
-WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int Cout, int taps) {
+// grouped: the kGrouped kernel of a 3x3 grouped convolution (Cin = 64: one channel block per row block; items of 3 taps)
+WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int Cout, int taps, bool grouped = false) {
   WgradPlan pl;
   pl.taps = taps;
   pl.Ho = static_cast<int>(d2), pl.Wo = static_cast<int>(d1);
@@ -424,7 +432,10 @@ WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int
   pl.mg_tiles = (Cout + 127) / 128;
   pl.ng_tiles = (Cin + pl.block_ng - 1) / pl.block_ng;
   pl.merge_atoms = 0;
-  if (Cin == 64 && taps > 1 && (taps % 4 == 0 || taps % 3 == 0)) {
+  if (grouped) {
+    pl.block_ng = 384;
+    pl.ng_tiles = 1;
+  } else if (Cin == 64 && taps > 1 && (taps % 4 == 0 || taps % 3 == 0)) {
     pl.merge_atoms = 1;
     pl.block_ng = taps % 4 == 0 ? 256 : 192;
     pl.ng_tiles = taps * 64 / pl.block_ng;
@@ -436,9 +447,9 @@ WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int
   pl.kb_total = pl.tiles1 * pl.tiles2 * pl.tiles3;
   // Split-K factor: minimise (waves x pixel blocks per item x time per block) + the fp32 partial traffic it causes. The
   // per-block times are estimates of the kernel's L2-operand-bound time (us per 64-pixel block, by tile width).
-  const int items_per_split = pl.mg_tiles * pl.ng_tiles * (pl.merge_atoms ? 1 : pl.taps);
+  const int items_per_split = pl.mg_tiles * pl.ng_tiles * (pl.merge_atoms ? 1 : (grouped ? pl.taps / 3 : pl.taps));
   const int sms = device_sm_count();
-  const double t_kb = pl.block_ng == 256 ? 0.45 : (pl.block_ng == 192 ? 0.36 : (pl.block_ng == 128 ? 0.30 : 0.25));
+  const double t_kb = pl.block_ng >= 256 ? 0.45 : (pl.block_ng == 192 ? 0.36 : (pl.block_ng == 128 ? 0.30 : 0.25));
   const double part_us = static_cast<double>(Cout) * Cin * taps * 4.0 * 2.0 / 3.0e6;  // write + read of one split at ~3 TB/s
   const int max_splits = pl.kb_total / 4 > 0 ? pl.kb_total / 4 : 1;
   int splits = 1;
@@ -458,13 +469,52 @@ WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int
   return pl;
 }
 
-WgradPlan plan_wgrad(int B, int H, int W, int Cin, int Cout, int ksize, int stride) {
+WgradPlan plan_wgrad(int B, int H, int W, int Cin, int Cout, int ksize, int stride, bool grouped = false) {
   const int Ho = out_dim(H, ksize, stride), Wo = out_dim(W, ksize, stride);
   const bool flat = (ksize == 1 && stride == 1);
   WgradPlan pl = plan_wgrad_geom(flat ? static_cast<long long>(B) * H * W : Wo, flat ? 1 : Ho, flat ? 1 : B, Cin, Cout,
-                                 ksize * ksize);
+                                 ksize * ksize, grouped);
   pl.Ho = Ho, pl.Wo = Wo;
   return pl;
+}
+
+// Tensor maps of dY and of the activation (tap / phase views) of a weight-gradient launch, and its tap table.
+int setup_wgrad_maps(WgradParams& p, const WgradPlan& pl, const void* dy, const void* x, int B, int H, int W, int Cin,
+                     int Cout, int ksize, int stride) {
+  const bool flat = (ksize == 1 && stride == 1);
+  int rc;
+  View dyv = flat ? make_flat_view(dy, static_cast<long long>(B) * H * W, Cout)
+                  : make_view(dy, B, pl.Ho, pl.Wo, Cout, 1, 0, 0);
+  if ((rc = encode_view(&p.dy_map, dyv, pl.box))) return rc;
+  if (flat) {
+    if ((rc = encode_view(&p.x_maps[0], make_flat_view(x, static_cast<long long>(B) * H * W, Cin), pl.box))) return rc;
+    for (int i = 1; i < 4; ++i) p.x_maps[i] = p.x_maps[0];
+  } else if (stride == 1) {
+    if ((rc = encode_view(&p.x_maps[0], make_view(x, B, H, W, Cin, 1, 0, 0), pl.box))) return rc;
+    for (int i = 1; i < 4; ++i) p.x_maps[i] = p.x_maps[0];
+    for (int kh = 0; kh < ksize; ++kh)
+      for (int kw = 0; kw < ksize; ++kw) {
+        const int t = kh * ksize + kw;
+        p.tap_map[t] = 0;
+        p.tap_o1[t] = static_cast<int8_t>(kw - ksize / 2);
+        p.tap_o2[t] = static_cast<int8_t>(kh - ksize / 2);
+      }
+  } else {
+    for (int ph = 0; ph < 2; ++ph)
+      for (int pw = 0; pw < 2; ++pw)
+        if ((rc = encode_view(&p.x_maps[ph * 2 + pw], make_view(x, B, H, W, Cin, 2, ph, pw), pl.box))) return rc;
+    const int pad = pad_of(ksize);
+    for (int kh = 0; kh < ksize; ++kh)
+      for (int kw = 0; kw < ksize; ++kw) {
+        const int t = kh * ksize + kw;
+        const int dh = kh - pad, dw_ = kw - pad;
+        const int ph = dh & 1, pw = dw_ & 1;
+        p.tap_map[t] = static_cast<int8_t>(ph * 2 + pw);
+        p.tap_o1[t] = static_cast<int8_t>((dw_ - pw) / 2);
+        p.tap_o2[t] = static_cast<int8_t>((dh - ph) / 2);
+      }
+  }
+  return OK;
 }
 
 // Space-to-depth stem (conv 7x7 / stride 2 / pad 3 on 3 channels, classification/resnet/models/networks.py:150,206):
@@ -495,7 +545,8 @@ int b200_debug_set_desc(int which, unsigned lbo, unsigned sbo, unsigned kstep) {
   return OK;
 }
 
-int b200_conv2d_fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int stride) {
+// Statistics rows of a forward launch with BN-column tiles (see b200_conv2d_fwd_stats_rows).
+static int fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int stride, int BN) {
   const int Ho = out_dim(H, ksize, stride), Wo = out_dim(W, ksize, stride);
   const bool flat = (ksize == 1 && stride == 1);
   const long long d1 = flat ? static_cast<long long>(B) * H * W : Wo;
@@ -503,13 +554,16 @@ int b200_conv2d_fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int str
   const long long d3 = flat ? 1 : B;
   const Box3 bx = choose_box(d1, d2, d3, 128);
   const long long m_tiles = ((d1 + bx.b1 - 1) / bx.b1) * ((d2 + bx.b2 - 1) / bx.b2) * ((d3 + bx.b3 - 1) / bx.b3);
-  const int BN = Cout <= 64 ? 64 : 128;
   const int n_tiles = (Cout + BN - 1) / BN;
   const long long tiles = m_tiles * n_tiles;
   const int grid = conv_grid(tiles > (1 << 30) ? (1 << 30) : static_cast<int>(tiles), n_tiles, true);
   // one partial row per (CTA group, 32-row quadrant); with 64-channel tiles two, one per parity of the CTA's tile count
   // (the layout conv_tap64_kernel shares)
   return grid / n_tiles * (BN == 64 ? 8 : 4);
+}
+
+int b200_conv2d_fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int stride) {
+  return fwd_stats_rows(B, H, W, Cout, ksize, stride, block_n_for(Cout));
 }
 
 static thread_local int g_conv_out_f32_tma = 0;
@@ -522,9 +576,10 @@ int b200_conv2d_fwd_f32(const void* x, const void* w, float* y, int B, int H, in
   return rc;
 }
 
-int b200_conv2d_fwd(const void* x, const void* w, void* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride,
+// Cg > 0: grouped convolution of group width Cg (Cin == Cout, validated by the caller) in channel-window mode
+static int conv_fwd(const void* x, const void* w, void* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride,
                     float* stats, const float* bias, int act, const void* residual, float* out_f32, long long ld_out,
-                    void* stream) {
+                    void* stream, int Cg) {
   B200_REQUIRE(ksize == 1 || ksize == 3 || (ksize == 2 && stride == 2), "conv2d_fwd: ksize %d / stride %d unsupported", ksize, stride);
   B200_REQUIRE(stride == 1 || stride == 2, "conv2d_fwd: stride %d unsupported (1 or 2)", stride);
   B200_REQUIRE(Cin % 8 == 0 && Cout % 8 == 0, "conv2d_fwd: Cin=%d / Cout=%d must be multiples of 8", Cin, Cout);
@@ -545,9 +600,11 @@ int b200_conv2d_fwd(const void* x, const void* w, void* y, int B, int H, int W, 
     if ((rc = setup_output(p, dv, Cout, g_conv_out_f32_tma, nullptr))) return rc;
   }
   const Box3 bx = box_of(p);
-  const int BN = block_n_for(Cout);
-  p.k_per_tap = Cin;
-  p.k_blocks_per_tap = (Cin + 63) / 64;
+  const int BN = Cg ? 64 : block_n_for(Cout);
+  p.n_tiles = (Cout + BN - 1) / BN;
+  p.chan_window = Cg ? 1 : 0;
+  p.k_per_tap = Cg ? 64 : Cin;
+  p.k_blocks_per_tap = Cg ? 1 : (Cin + 63) / 64;
   p.num_taps = ksize * ksize;
   if (flat) {
     if ((rc = encode_view(&p.a_maps[0], make_flat_view(x, d1, Cin), bx))) return rc;
@@ -583,8 +640,8 @@ int b200_conv2d_fwd(const void* x, const void* w, void* y, int B, int H, int W, 
       }
   }
   {
-    uint64_t dims[2] = {static_cast<uint64_t>(p.num_taps) * Cin, static_cast<uint64_t>(Cout)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(p.num_taps) * Cin};
+    uint64_t dims[2] = {static_cast<uint64_t>(p.num_taps) * p.k_per_tap, static_cast<uint64_t>(Cout)};
+    uint64_t strides[2] = {1, static_cast<uint64_t>(p.num_taps) * p.k_per_tap};
     uint32_t box[2] = {64, static_cast<uint32_t>(BN)};
     if ((rc = encode_tmap_bf16(&p.b_map, w, 2, dims, strides, box))) return rc;
   }
@@ -609,7 +666,13 @@ int b200_conv2d_fwd(const void* x, const void* w, void* y, int B, int H, int W, 
     p.colscale = sc;
     p.bias = sh;
   }
-  return dispatch_conv_gemm(p, Cout, st);
+  return Cg ? launch_conv_gemm<64>(p, st) : dispatch_conv_gemm(p, Cout, st);
+}
+
+int b200_conv2d_fwd(const void* x, const void* w, void* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride,
+                    float* stats, const float* bias, int act, const void* residual, float* out_f32, long long ld_out,
+                    void* stream) {
+  return conv_fwd(x, w, y, B, H, W, Cin, Cout, ksize, stride, stats, bias, act, residual, out_f32, ld_out, stream, 0);
 }
 
 int b200_dgrad_set_bn_mask(const void* x_raw, const float* scale, const float* shift, float* stats) {
@@ -623,20 +686,22 @@ int b200_conv2d_fwd_set_bn(const float* scale, const float* shift) {
   return OK;
 }
 
-int b200_conv2d_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int Cin, int Cout, int ksize,
-                      int stride, const void* residual, void* stream) {
+// Cg > 0: grouped convolution of group width Cg (Cin == Cout, validated by the caller) in channel-window mode
+static int conv_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int Cin, int Cout, int ksize,
+                      int stride, const void* residual, void* stream, int Cg) {
   B200_REQUIRE(ksize == 1 || ksize == 3 || (ksize == 2 && stride == 2), "conv2d_dgrad: ksize %d / stride %d unsupported", ksize, stride);
   B200_REQUIRE(stride == 1 || stride == 2, "conv2d_dgrad: stride %d unsupported", stride);
   B200_REQUIRE(Cin % 8 == 0 && Cout % 8 == 0, "conv2d_dgrad: Cin=%d / Cout=%d must be multiples of 8", Cin, Cout);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int Ho = out_dim(H, ksize, stride), Wo = out_dim(W, ksize, stride);
   const int taps = ksize * ksize;
-  const int BN = block_n_for(Cin);
+  const int BN = Cg ? 64 : block_n_for(Cin);
+  const int k_per_tap = Cg ? 64 : Cout;
   int rc;
   CUtensorMap b_map;
   {
-    uint64_t dims[2] = {static_cast<uint64_t>(taps) * Cout, static_cast<uint64_t>(Cin)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(taps) * Cout};
+    uint64_t dims[2] = {static_cast<uint64_t>(taps) * k_per_tap, static_cast<uint64_t>(Cin)};
+    uint64_t strides[2] = {1, static_cast<uint64_t>(taps) * k_per_tap};
     uint32_t box[2] = {64, static_cast<uint32_t>(BN)};
     if ((rc = encode_tmap_bf16(&b_map, wd, 2, dims, strides, box))) return rc;
   }
@@ -659,8 +724,10 @@ int b200_conv2d_dgrad(const void* dy, const void* wd, void* dx, int B, int H, in
                      : make_view(dx, B, H, W, Cin, stride, ph, pw);
       if ((rc = setup_output(p, dv, Cin, 0, nullptr))) return rc;
       const Box3 bx = box_of(p);
-      p.k_per_tap = Cout;
-      p.k_blocks_per_tap = (Cout + 63) / 64;
+      p.n_tiles = (Cin + BN - 1) / BN;
+      p.chan_window = Cg ? 1 : 0;
+      p.k_per_tap = k_per_tap;
+      p.k_blocks_per_tap = Cg ? 1 : (Cout + 63) / 64;
       View av = flat ? make_flat_view(dy, static_cast<long long>(B) * H * W, Cout)
                      : make_view(dy, B, Ho, Wo, Cout, 1, 0, 0);
       if ((rc = encode_view(&p.a_maps[0], av, bx))) return rc;
@@ -712,10 +779,15 @@ int b200_conv2d_dgrad(const void* dy, const void* wd, void* dx, int B, int H, in
         p.ms3 = static_cast<long long>(dv.strides[3]);
         p.bn_scale = bnmask_scale, p.bn_shift = bnmask_shift, p.stats = bnmask_stats;
       }
-      if ((rc = dispatch_conv_gemm(p, Cin, st))) return rc;
+      if ((rc = Cg ? launch_conv_gemm<64>(p, st) : dispatch_conv_gemm(p, Cin, st))) return rc;
     }
   }
   return OK;
+}
+
+int b200_conv2d_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int Cin, int Cout, int ksize,
+                      int stride, const void* residual, void* stream) {
+  return conv_dgrad(dy, wd, dx, B, H, W, Cin, Cout, ksize, stride, residual, stream, 0);
 }
 
 int b200_gemm_ex(const b200_view_t* a, const b200_view_t* out, const b200_gemm_args_t* g, void* stream) {
@@ -829,39 +901,8 @@ int b200_conv2d_wgrad(const void* dy, const void* x, float* dw, void* workspace,
   g_wgrad_bias_partial = nullptr;
   float* const bias_out = p.bias_partial != nullptr ? g_wgrad_bias_out : nullptr;
   g_wgrad_bias_out = nullptr;
-  const bool flat = (ksize == 1 && stride == 1);
   int rc;
-  View dyv = flat ? make_flat_view(dy, static_cast<long long>(B) * H * W, Cout)
-                  : make_view(dy, B, pl.Ho, pl.Wo, Cout, 1, 0, 0);
-  if ((rc = encode_view(&p.dy_map, dyv, pl.box))) return rc;
-  if (flat) {
-    if ((rc = encode_view(&p.x_maps[0], make_flat_view(x, static_cast<long long>(B) * H * W, Cin), pl.box))) return rc;
-    for (int i = 1; i < 4; ++i) p.x_maps[i] = p.x_maps[0];
-  } else if (stride == 1) {
-    if ((rc = encode_view(&p.x_maps[0], make_view(x, B, H, W, Cin, 1, 0, 0), pl.box))) return rc;
-    for (int i = 1; i < 4; ++i) p.x_maps[i] = p.x_maps[0];
-    for (int kh = 0; kh < ksize; ++kh)
-      for (int kw = 0; kw < ksize; ++kw) {
-        const int t = kh * ksize + kw;
-        p.tap_map[t] = 0;
-        p.tap_o1[t] = static_cast<int8_t>(kw - ksize / 2);
-        p.tap_o2[t] = static_cast<int8_t>(kh - ksize / 2);
-      }
-  } else {
-    for (int ph = 0; ph < 2; ++ph)
-      for (int pw = 0; pw < 2; ++pw)
-        if ((rc = encode_view(&p.x_maps[ph * 2 + pw], make_view(x, B, H, W, Cin, 2, ph, pw), pl.box))) return rc;
-    const int pad = pad_of(ksize);
-    for (int kh = 0; kh < ksize; ++kh)
-      for (int kw = 0; kw < ksize; ++kw) {
-        const int t = kh * ksize + kw;
-        const int dh = kh - pad, dw_ = kw - pad;
-        const int ph = dh & 1, pw = dw_ & 1;
-        p.tap_map[t] = static_cast<int8_t>(ph * 2 + pw);
-        p.tap_o1[t] = static_cast<int8_t>((dw_ - pw) / 2);
-        p.tap_o2[t] = static_cast<int8_t>((dh - ph) / 2);
-      }
-  }
+  if ((rc = setup_wgrad_maps(p, pl, dy, x, B, H, W, Cin, Cout, ksize, stride))) return rc;
   if (pl.block_ng == 64)
     rc = launch_wgrad<64>(p, st);
   else if (pl.block_ng == 128)
@@ -1071,6 +1112,83 @@ int b200_gemm_dual(const void* a0, int K0, const void* a1, int K1, const void* w
     g_bnmask_x = nullptr;
   }
   return dispatch_conv_gemm(p, N, static_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Grouped 3x3 convolutions (ResNeXt conv2, classification/resnet/models/networks.py:295-321): C input = C output channels,
+// C % 64 == 0, group width Cg = C / groups in {4, 8, 16, 32, 64}, so no group straddles a 64-channel block. Forward and
+// dgrad run conv_gemm_kernel<64> in channel-window mode on the block-diagonal operands of b200_pack_weight modes 3 / 4;
+// the weight gradient runs the kGrouped mode of wgrad_gemm_kernel.
+
+static int grouped_check(const char* fn, int C, int groups, int ksize, int stride) {
+  B200_REQUIRE(ksize == 3, "%s: ksize %d unsupported (3x3 only)", fn, ksize);
+  B200_REQUIRE(stride == 1 || stride == 2, "%s: stride %d unsupported (1 or 2)", fn, stride);
+  B200_REQUIRE(groups > 0 && C > 0 && C % 64 == 0 && C % groups == 0, "%s: C=%d must be a multiple of 64 and of groups=%d",
+               fn, C, groups);
+  const int Cg = C / groups;
+  B200_REQUIRE(Cg >= 4 && 64 % Cg == 0, "%s: group width C / groups = %d unsupported (4, 8, 16, 32 or 64)", fn, Cg);
+  return OK;
+}
+
+int b200_conv2d_grouped_fwd_stats_rows(int B, int H, int W, int C, int groups, int ksize, int stride) {
+  int rc;
+  if ((rc = grouped_check("conv2d_grouped_fwd_stats_rows", C, groups, ksize, stride))) return rc;
+  return fwd_stats_rows(B, H, W, C, ksize, stride, 64);
+}
+
+int b200_conv2d_grouped_fwd(const void* x, const void* w, void* y, int B, int H, int W, int C, int groups, int ksize,
+                            int stride, float* stats, int act, void* stream) {
+  int rc;
+  if ((rc = grouped_check("conv2d_grouped_fwd", C, groups, ksize, stride))) return rc;
+  B200_REQUIRE(act == 0 || act == 1, "conv2d_grouped_fwd: act %d unsupported (none or relu)", act);
+  return conv_fwd(x, w, y, B, H, W, C, C, ksize, stride, stats, nullptr, act, nullptr, nullptr, 0, stream, C / groups);
+}
+
+int b200_conv2d_grouped_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int C, int groups, int ksize,
+                              int stride, void* stream) {
+  int rc;
+  if ((rc = grouped_check("conv2d_grouped_dgrad", C, groups, ksize, stride))) return rc;
+  return conv_dgrad(dy, wd, dx, B, H, W, C, C, ksize, stride, nullptr, stream, C / groups);
+}
+
+static size_t grouped_wgrad_bytes(const WgradPlan& pl, int C) {
+  return static_cast<size_t>(pl.splits) * C * pl.taps * 64 * sizeof(float);
+}
+
+size_t b200_conv2d_grouped_wgrad_workspace_bytes(int B, int H, int W, int C, int groups, int ksize, int stride) {
+  if (grouped_check("conv2d_grouped_wgrad_workspace_bytes", C, groups, ksize, stride)) return 0;
+  return grouped_wgrad_bytes(plan_wgrad(B, H, W, 64, C, ksize, stride, true), C);
+}
+
+int b200_conv2d_grouped_wgrad(const void* dy, const void* x, float* dw, void* workspace, size_t workspace_bytes, int B,
+                              int H, int W, int C, int groups, int ksize, int stride, int accumulate, void* stream) {
+  int rc;
+  if ((rc = grouped_check("conv2d_grouped_wgrad", C, groups, ksize, stride))) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const WgradPlan pl = plan_wgrad(B, H, W, 64, C, ksize, stride, true);
+  const size_t need = grouped_wgrad_bytes(pl, C);
+  B200_REQUIRE(workspace != nullptr && workspace_bytes >= need, "conv2d_grouped_wgrad: workspace too small (%zu < %zu)",
+               workspace_bytes, need);
+  WgradParams p;
+  memset(&p, 0, sizeof(p));
+  p.num_taps = pl.taps / 3;   // work items of three taps each
+  p.n_cols = 3 * 64;
+  p.Cout = C, p.Cin = 3 * 64;
+  p.mg_tiles = pl.mg_tiles, p.ng_tiles = 1;
+  p.tiles1 = pl.tiles1, p.tiles2 = pl.tiles2, p.tiles3 = pl.tiles3;
+  p.box1 = pl.box.b1, p.box2 = pl.box.b2, p.box3 = pl.box.b3;
+  p.splits = pl.splits, p.kb_per_split = pl.kb_per_split, p.kb_total = pl.kb_total;
+  p.ld_partial = static_cast<long long>(pl.taps) * 64;
+  p.partial = static_cast<float*>(workspace);
+  if ((rc = setup_wgrad_maps(p, pl, dy, x, B, H, W, C, C, ksize, stride))) return rc;
+  if ((rc = launch_wgrad<384, true>(p, st))) return rc;
+  const long long total = static_cast<long long>(C) * (C / groups) * pl.taps;
+  int blocks = static_cast<int>((total + 255) / 256);
+  if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
+  B200_CHECK_CUDA(launch_pdl(wgrad_reduce_grouped_kernel, dim3(blocks), dim3(256), 0, st, static_cast<const float*>(p.partial),
+                             dw, pl.splits, C, C / groups, pl.taps, accumulate));
+  B200_LAUNCHED();
+  return OK;
 }
 
 }  // extern "C"

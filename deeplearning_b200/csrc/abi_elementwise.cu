@@ -200,9 +200,11 @@ int b200_colsum_bf16(const void* m, long long rows, long long ld, int cols, floa
 }
 
 int b200_pack_weight(const float* src, void* dst, int O, int I, int taps, int mode, long long ld_dst, void* stream) {
-  B200_REQUIRE(mode == 0 || mode == 1, "pack_weight: mode %d", mode);
-  const long long rows = mode == 0 ? O : I;
-  const long long need = static_cast<long long>(taps) * (mode == 0 ? I : O);
+  B200_REQUIRE(mode == 0 || mode == 1 || mode == 3 || mode == 4, "pack_weight: mode %d", mode);
+  B200_REQUIRE(mode < 3 || (O % 64 == 0 && I > 0 && 64 % I == 0),
+               "pack_weight: grouped modes need C %% 64 == 0 and a group width dividing 64 (C=%d, Cg=%d)", O, I);
+  const long long rows = mode == 1 ? I : O;
+  const long long need = static_cast<long long>(taps) * (mode == 0 ? I : (mode == 1 ? O : 64));
   B200_REQUIRE(ld_dst >= need, "pack_weight: ld_dst %lld < %lld", ld_dst, need);
   B200_CHECK_CUDA(launch_pdl(pack_weight_kernel, dim3(ew_grid(rows * ld_dst)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       src, static_cast<__nv_bfloat16*>(dst), O, I, taps, mode, ld_dst));

@@ -76,6 +76,10 @@ struct alignas(64) ConvGemmParams {
   // alive = x * bn_scale + bn_shift > 0; the statistics rows carry sum(dz) and sum(dz * x) (what bn_bwd_reduce produces)
   const float* bn_scale;
   const float* bn_shift;
+  // --- grouped convolution whose groups never straddle a 64-channel block (BLOCK_N = 64 only): output channel block n
+  // reads only input channel block n, so the activation box of every k-block starts at channel n_tile * 64 (one k-block
+  // per tap) and B is the block-diagonal [C][taps * 64] operand (b200_pack_weight mode 3 / 4)
+  int chan_window;
 };
 
 template <int BLOCK_N>
@@ -275,7 +279,7 @@ __global__ void __launch_bounds__(512, 1) conv_gemm_kernel(const __grid_constant
           uint8_t* a_dst = stage_base + stage * Cfg::STAGE_BYTES;
           uint8_t* b_dst = a_dst + Cfg::A_BYTES;
           mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          tma_load_4d(a_dst, &p.a_maps[p.tap_map[tap]], &full_bar[stage], cb * 64, c1 + p.tap_o1[tap],
+          tma_load_4d(a_dst, &p.a_maps[p.tap_map[tap]], &full_bar[stage], p.chan_window ? n_tile * BLOCK_N : cb * 64, c1 + p.tap_o1[tap],
                       c2 + p.tap_o2[tap], c3);
           tma_load_2d(b_dst, &p.b_map, &full_bar[stage], wk, n_tile * BLOCK_N);
           if (++stage == STAGES) {

@@ -692,18 +692,34 @@ __global__ void colsum_kernel(const __nv_bfloat16* __restrict__ m, long long row
 // Weight packing: fp32 OIHW master parameter -> bf16 GEMM operand.
 //   mode 0 (forward / wgrad layout): dst[o][tap*I + i]      (row pitch ld_dst, zero padded)
 //   mode 1 (dgrad layout):           dst[i][tap*O + o]
+//   modes 3 / 4: grouped convolution, src [C][Cg][taps] (O = C, I = Cg, 64 % Cg == 0) -> block-diagonal [C][taps*64]
+//     mode 3 (forward): dst[o][tap*64 + j] = W[o][c - g*Cg][tap] with input channel c = (o & ~63) + j, if c is in o's group g
+//     mode 4 (dgrad):   dst[c][tap*64 + j] = W[o][c - g*Cg][tap] with output channel o = (c & ~63) + j, if o is in c's group g
+//     (taps unflipped as in mode 1; everything outside the group is zero)
+__device__ __forceinline__ float grouped_pack_value(const float* __restrict__ src, int Cg, int taps, int mode, long long r,
+                                                    long long k) {
+  if (k >= static_cast<long long>(taps) * 64) return 0.f;
+  const int tap = static_cast<int>(k >> 6);
+  const long long other = (r & ~63ll) + (k & 63);   // the channel of the other side in the same 64-channel block
+  if (r / Cg != other / Cg) return 0.f;
+  const long long o = mode == 3 ? r : other, c = mode == 3 ? other : r;
+  return src[(o * Cg + c % Cg) * taps + tap];
+}
+
 __global__ void pack_weight_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int O, int I,
                                    int taps, int mode, long long ld_dst) {
   pdl_launch_dependents();
   pdl_wait();
-  const long long rows = mode == 0 ? O : I;
+  const long long rows = mode == 1 ? I : O;
   const long long total = rows * ld_dst;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long r = idx / ld_dst;
     const long long k = idx % ld_dst;
     float v = 0.f;
-    if (mode == 0) {
+    if (mode >= 3) {
+      v = grouped_pack_value(src, I, taps, mode, r, k);
+    } else if (mode == 0) {
       if (k < static_cast<long long>(taps) * I) {
         const int tap = static_cast<int>(k / I), i = static_cast<int>(k % I);
         v = src[(r * I + i) * taps + tap];
@@ -849,6 +865,15 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const long long
         }
       }
       dst[idx] = __float2bfloat16_rn(v);
+    }
+    return;
+  }
+
+  if (mode >= 3) {
+    // grouped convolution operands (see grouped_pack_value): rows_out = O = C
+    for (long long idx = blk * 256ll + tid; idx < rows_out * ld; idx += nblk * 256ll) {
+      const long long r = idx / ld, k = idx % ld;
+      dst[idx] = __float2bfloat16_rn(r < O ? grouped_pack_value(src, I, taps, mode, r, k) : 0.f);
     }
     return;
   }

@@ -10,6 +10,12 @@
 // atoms of one B tile belong to DIFFERENT taps (same pixels, shifted TMA coordinates), so one dY tile feeds an N = 192 / 256
 // MMA instead of one N = 64 MMA per tap.
 //
+// GROUPED mode (kGrouped, 3x3 grouped convolutions whose groups never straddle a 64-channel block): dW of such a layer only
+// needs the diagonal 64 x 64 blocks of dY^T X_tap. Each consumer warpgroup owns one 64-channel block and multiplies its dY
+// atom with X atoms of the SAME channel block for three taps (BLOCK_NG / 2 = 192 columns per warpgroup); a work item is one
+// (split, 128-channel pair, tap triple). The dense C x C product is never formed; wgrad_reduce_grouped_kernel picks the
+// in-group columns.
+//
 // Two consumer warpgroups multiply with wgmma (64 output channels each: one dY atom) and store their fp32 fragments straight
 // to the partial rows; warp 0 is the TMA producer.
 //
@@ -51,17 +57,19 @@ struct WgradCfg {
   static constexpr int A_BYTES = 2 * 64 * 128;             // two 64-channel atoms of dY
   static constexpr int B_BYTES = (BLOCK_NG / 64) * 64 * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BLOCK_NG == 256) ? 4 : (BLOCK_NG == 192 ? 5 : (BLOCK_NG == 128 ? 6 : 8));
+  static constexpr int STAGES = BLOCK_NG == 384 ? 3 : (BLOCK_NG == 256 ? 4 : (BLOCK_NG == 192 ? 5 : (BLOCK_NG == 128 ? 6 : 8)));
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory of one H100 block");
 };
 constexpr int kWgradThreads = 384;   // warpgroup 0: TMA producer (warp 0), warpgroups 1-2: consumers
 
-template <int BLOCK_NG, bool kBias = false>
+template <int BLOCK_NG, bool kBias = false, bool kGrouped = false>
 __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
   pdl_launch_dependents();
+  static_assert(!kGrouped || (BLOCK_NG == 384 && !kBias), "grouped mode: two warpgroups x three 64-column taps");
   using Cfg = WgradCfg<BLOCK_NG>;
+  constexpr int NW = kGrouped ? BLOCK_NG / 2 : BLOCK_NG;   // columns of one warpgroup's MMA
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -108,7 +116,11 @@ __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __gr
 #pragma unroll
         for (int j = 0; j < BLOCK_NG / 64; ++j) {
           int tp = tap, ca = ng * (BLOCK_NG / 64) + j;
-          if (p.merge_atoms) {
+          if constexpr (kGrouped) {
+            // atom j: tap 3 * tap + j % 3 of channel block 2 mg + j / 3 (the dY atom of consumer warpgroup j / 3)
+            tp = tap * 3 + j % 3;
+            ca = mg * 2 + j / 3;
+          } else if (p.merge_atoms) {
             tp = ca / p.merge_atoms;
             ca -= tp * p.merge_atoms;
           }
@@ -144,7 +156,8 @@ __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __gr
     const bool leader = (threadIdx.x & 127) == 0;
     // A = dY atom wg (64 output channels, MN-major), B = BLOCK_NG / 64 atoms of X (MN-major): 16 pixel rows per K step
     const uint64_t desc_a0 = make_smem_desc_sw128(smem_u32(smem) + wg * 8192, p.desc_lbo, p.desc_sbo);
-    const uint64_t desc_b0 = make_smem_desc_sw128(smem_u32(smem) + Cfg::A_BYTES, p.desc_lbo, p.desc_sbo);
+    const uint64_t desc_b0 =
+        make_smem_desc_sw128(smem_u32(smem) + Cfg::A_BYTES + (kGrouped ? wg * NW * 128 : 0), p.desc_lbo, p.desc_sbo);
     const uint64_t kstep = p.desc_kstep >> 4;
     const int t = threadIdx.x & 127;
     const int frow = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);   // fragment row of d[4j], d[4j+1]; d[4j+2..3]: + 8
@@ -166,9 +179,9 @@ __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __gr
       const bool summed = kBias && ng == 0 && tap == 0;
       const int cc = t & 7, rg = t >> 3;
       float bsum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      float acc[BLOCK_NG / 2];
+      float acc[NW / 2];
 #pragma unroll
-      for (int i = 0; i < BLOCK_NG / 2; ++i) acc[i] = 0.f;
+      for (int i = 0; i < NW / 2; ++i) acc[i] = 0.f;
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -176,7 +189,7 @@ __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __gr
         const uint64_t soff = static_cast<uint64_t>(stage) * (Cfg::STAGE_BYTES >> 4);
         const uint64_t da = desc_a0 + soff, db = desc_b0 + soff;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) Wgmma<BLOCK_NG, 1, 1>::mma(acc, da + k * kstep, db + k * kstep, 1u);
+        for (int k = 0; k < 4; ++k) Wgmma<NW, 1, 1>::mma(acc, da + k * kstep, db + k * kstep, 1u);
         wgmma_commit();
         if (summed) {
           const uint32_t base = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * 8192;
@@ -236,7 +249,7 @@ __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __gr
           float* out_row = p.partial + (static_cast<long long>(split) * p.Cout + cout) * p.ld_partial +
                            static_cast<long long>(tap) * p.Cin + ng * BLOCK_NG;
 #pragma unroll
-          for (int j = 0; j < BLOCK_NG / 8; ++j)
+          for (int j = 0; j < NW / 8; ++j)
             if (8 * j + fcol < ncol)
               *reinterpret_cast<float2*>(out_row + 8 * j + fcol) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
@@ -334,6 +347,27 @@ __global__ void wgrad_reduce_flat_kernel(const float* __restrict__ partial, floa
     if (rowscale != nullptr) s *= __ldg(rowscale + cout);
     const long long o = (static_cast<long long>(cout) * Cin + cin) * taps + tap;
     grad[o] = accumulate ? grad[o] + s : s;
+  }
+}
+
+// Grouped mode: grad[co][ci][tap] (OIHW [C][Cg][taps]) (+)= sum_s partial[s][co][tap * 64 + (co % 64) / Cg * Cg + ci], the
+// in-group columns of the diagonal blocks the kGrouped wgrad kernel wrote. One thread per gradient element, splits summed
+// in order (deterministic).
+__global__ void wgrad_reduce_grouped_kernel(const float* __restrict__ partial, float* __restrict__ grad, int splits, int C,
+                                            int Cg, int taps, int accumulate) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long long total = static_cast<long long>(C) * Cg * taps;
+  const long long slice = static_cast<long long>(C) * taps * 64;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int tap = static_cast<int>(i % taps);
+    const int ci = static_cast<int>((i / taps) % Cg);
+    const int co = static_cast<int>(i / (static_cast<long long>(taps) * Cg));
+    const float* src = partial + static_cast<long long>(co) * taps * 64 + tap * 64 + (co & 63) / Cg * Cg + ci;
+    float s = 0.f;
+    for (int k = 0; k < splits; ++k) s += src[k * slice];
+    grad[i] = accumulate ? grad[i] + s : s;
   }
 }
 

@@ -30,12 +30,25 @@ from .packing import weight_cache
 BF16 = torch.bfloat16
 
 
+_GROUP_WIDTHS = (4, 8, 16, 32, 64)
+
+
 def _check_conv(conv, name):
     k = conv.kernel_size[0]
-    if (conv.groups != 1 or conv.dilation != (1, 1) or conv.kernel_size[0] != conv.kernel_size[1] or conv.bias is not None
+    if (conv.dilation != (1, 1) or conv.kernel_size[0] != conv.kernel_size[1] or conv.bias is not None
             or conv.padding != (k // 2, k // 2) or conv.stride[0] != conv.stride[1] or conv.stride[0] not in (1, 2)):
-        raise NotImplementedError(f"{name}: only dense k x k convolutions with pad=k//2, stride 1/2, no bias run on the "
+        raise NotImplementedError(f"{name}: only undilated k x k convolutions with pad=k//2, stride 1/2, no bias run on the "
                                   f"GPU engine (got {conv})")
+    if conv.groups != 1:
+        C = conv.in_channels
+        if k != 3 or conv.out_channels != C or C % 64 != 0 or C // conv.groups not in _GROUP_WIDTHS:
+            raise NotImplementedError(f"{name}: grouped convolutions run on the GPU engine as 3x3 with in_channels == "
+                                      f"out_channels, a multiple of 64, and a group width in {_GROUP_WIDTHS} (got {conv})")
+
+
+def _pack_modes(conv):
+    """(forward, dgrad) packed-operand modes of a convolution weight (ops.pack_weight)."""
+    return (3, 4) if conv.groups != 1 else (0, 1)
 
 
 def _check_bn(bn, name):
@@ -75,6 +88,10 @@ class _PackSpec:
                 O, I, kh, kw = w.shape
                 if name == "conv1":
                     specs.append((w, 2, 256, O, (O, I, kh * kw)))  # space-to-depth stem operand [64][256]
+                    continue
+                if mod.groups != 1:   # block-diagonal operands of a grouped 3x3 convolution
+                    specs.append((w, 3, kh * kw * 64, O))
+                    specs.append((w, 4, kh * kw * 64, O))
                     continue
                 specs.append((w, 0, kh * kw * I, O))
                 specs.append((w, 1, kh * kw * O, I))
@@ -171,13 +188,13 @@ def _ds_conv_bn_algebra(pack, tape, x_in, conv, bn, name=""):
 def _conv_bn(pack, tape, x, conv, bn, train, relu, residual=None, name=""):
     _check_conv(conv, name)
     _check_bn(bn, name)
-    k, s = conv.kernel_size[0], conv.stride[0]
-    wp = pack.get(conv.weight, 0)
+    k, s, g = conv.kernel_size[0], conv.stride[0], conv.groups
+    wp = pack.get(conv.weight, _pack_modes(conv)[0])
     if not train and tape is None and conv.out_channels % 64 == 0 and _algebra_enabled():
         # eval forward (no tape): running statistics are constants, BatchNorm (+ identity) (+ ReLU) live in the conv epilogue
         co = ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
-        return ops.conv2d_bn_act(x, wp, co, k, s, relu=relu, residual=residual)
-    c, st = ops.conv2d_fwd(x, wp, k, s, want_stats=train)
+        return ops.conv2d_bn_act(x, wp, co, k, s, relu=relu, residual=residual, groups=g)
+    c, st = ops.conv2d_fwd(x, wp, k, s, want_stats=train, groups=g)
     if train:
         rows = c.numel() // c.shape[-1]
         co = ops.bn_finalize(st, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
@@ -414,15 +431,15 @@ def backward(model, tape, dlogits, sink=None):
         dz_prev = dz_prev_stats = None
         for j in range(first, -1, -1):
             u = units[j]
-            k, s = u.conv.kernel_size[0], u.conv.stride[0]
-            grads.put(u.conv.weight, ops.conv2d_wgrad(dc, u.x, k, s, out=grads.dest(u.conv.weight)))
-            wd = pack.get(u.conv.weight, 1)
+            k, s, gr = u.conv.kernel_size[0], u.conv.stride[0], u.conv.groups
+            grads.put(u.conv.weight, ops.conv2d_wgrad(dc, u.x, k, s, out=grads.dest(u.conv.weight), groups=gr))
+            wd = pack.get(u.conv.weight, _pack_modes(u.conv)[1])
             in_hw = tuple(u.x.shape[1:3])
             if j > 0 and s == 1 and _fused_reduce_ok(units[j - 1]):
-                dzj, sumsj = ops.conv2d_dgrad(dc, wd, in_hw, k, s, bn_mask=(units[j - 1].c, units[j - 1].co))
+                dzj, sumsj = ops.conv2d_dgrad(dc, wd, in_hw, k, s, bn_mask=(units[j - 1].c, units[j - 1].co), groups=gr)
                 dc = _unit_backward_from_sums(units[j - 1], dzj, sumsj, grads)
             elif j > 0:
-                g_prev = ops.conv2d_dgrad(dc, wd, in_hw, k, s)
+                g_prev = ops.conv2d_dgrad(dc, wd, in_hw, k, s, groups=gr)
                 dc, _ = _unit_backward(units[j - 1], g_prev, grads)
             else:
                 if has_ds and gxs is not None and ds.conv.stride == (1, 1):

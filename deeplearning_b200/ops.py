@@ -92,7 +92,8 @@ def out_hw(h, ksize, stride):
 
 # --------------------------------------------------------------------------------------------------------- packing
 def pack_weight(w, mode=0, ld=None):
-    """fp32 OIHW (or [out,in]) parameter -> bf16 GEMM operand. mode 0: [O][taps*I]; mode 1 (dgrad): [I][taps*O]."""
+    """fp32 OIHW (or [out,in]) parameter -> bf16 GEMM operand. mode 0: [O][taps*I]; mode 1 (dgrad): [I][taps*O];
+    modes 3 / 4: block-diagonal forward / dgrad operands [C][taps*64] of a grouped convolution weight [C][C/groups][k][k]."""
     lib = _lib.load()
     w = w.detach()
     if w.dtype != F32 or not w.is_contiguous():
@@ -101,8 +102,8 @@ def pack_weight(w, mode=0, ld=None):
     taps = 1
     for d in w.shape[2:]:
         taps *= d
-    rows = O if mode == 0 else I
-    cols = taps * (I if mode == 0 else O)
+    rows = I if mode == 1 else O
+    cols = taps * {0: I, 1: O}.get(mode, 64)
     ld = cols if ld is None else ld
     out = torch.empty(rows, ld, dtype=BF16, device=w.device)
     _lib.check(lib.b200_pack_weight(_p(w), _p(out), O, I, taps, mode, ld, _stream()), "b200_pack_weight")
@@ -139,10 +140,32 @@ def im2col_nchw(x, KH, KW, stride, pad, ldk):
 
 
 # --------------------------------------------------------------------------------------------------------- conv / linear
-def conv2d_fwd(x, w_packed, ksize=1, stride=1, want_stats=False, bias=None, act=0, residual=None, out_f32=False):
-    """y = conv(x) (+bias)(act)(+residual). Returns (y, stats) with stats = [T,2,Cout] partial sums or None."""
+def _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, want_stats, act, groups):
+    B, H, W, C = x.shape
+    Ho, Wo = out_hw(H, ksize, stride), out_hw(W, ksize, stride)
+    stats = None
+    if want_stats:
+        T = lib.b200_conv2d_grouped_fwd_stats_rows(B, H, W, C, groups, ksize, stride)
+        _lib.check(min(T, 0), "b200_conv2d_grouped_fwd_stats_rows")
+        stats = torch.empty(T, 2, C, dtype=F32, device=x.device)
+    y = torch.empty(B, Ho, Wo, C, dtype=BF16, device=x.device)
+    sp = _span("conv_gemm_grouped_fwd", 2.0 * B * Ho * Wo * C * (C // groups) * ksize * ksize, _nb(x, w_packed, y))
+    rc = lib.b200_conv2d_grouped_fwd(_p(x), _p(w_packed), _p(y), B, H, W, C, groups, ksize, stride, _p(stats), act, _stream())
+    _lib.check(rc, "b200_conv2d_grouped_fwd")
+    if sp:
+        sp.end()
+    return y, stats
+
+
+def conv2d_fwd(x, w_packed, ksize=1, stride=1, want_stats=False, bias=None, act=0, residual=None, out_f32=False, groups=1):
+    """y = conv(x) (+bias)(act)(+residual). Returns (y, stats) with stats = [T,2,Cout] partial sums or None.
+    groups > 1: grouped 3x3 convolution (w_packed = pack_weight(w, mode=3)); bias, residual and fp32 output are not offered."""
     lib = _lib.load()
     _chk_act(x, "x")
+    if groups != 1:
+        if bias is not None or residual is not None or out_f32:
+            raise ValueError("conv2d_fwd: a grouped convolution takes no bias, residual or fp32 output")
+        return _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, want_stats, act, groups)
     B, H, W, Cin = x.shape
     Cout = w_packed.shape[0]
     Ho, Wo = out_hw(H, ksize, stride), out_hw(W, ksize, stride)
@@ -166,11 +189,16 @@ def conv2d_fwd(x, w_packed, ksize=1, stride=1, want_stats=False, bias=None, act=
     return y, stats
 
 
-def conv2d_bn_act(x, w_packed, co, ksize=1, stride=1, relu=True, residual=None):
+def conv2d_bn_act(x, w_packed, co, ksize=1, stride=1, relu=True, residual=None, groups=1):
     """Eval-mode conv -> BatchNorm(fixed statistics) (-> + residual) (-> ReLU) as ONE implicit-GEMM launch: the BN scale / shift
-    live in the epilogue, no BatchNorm pass at all."""
+    live in the epilogue, no BatchNorm pass at all.  groups > 1: grouped 3x3 convolution (pack_weight mode 3), no residual."""
     lib = _lib.load()
     _chk_act(x, "x")
+    if groups != 1:
+        if residual is not None:
+            raise ValueError("conv2d_bn_act: a grouped convolution takes no residual")
+        lib.b200_conv2d_fwd_set_bn(_p(co.scale), _p(co.shift))
+        return _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, False, 1 if relu else 0, groups)[0]
     B, H, W, Cin = x.shape
     Cout = w_packed.shape[0]
     Ho, Wo = out_hw(H, ksize, stride), out_hw(W, ksize, stride)
@@ -185,25 +213,45 @@ def conv2d_bn_act(x, w_packed, co, ksize=1, stride=1, relu=True, residual=None):
     return y
 
 
-def _arm_bn_mask(lib, bn_mask, B, H, W, C, ksize):
+def _arm_bn_mask(lib, bn_mask, B, H, W, C, ksize, groups=1):
     """One-shot: the next dgrad / dual GEMM masks its output with relu'(bn(x_raw)) and writes the BN-backward partial sums."""
     x_raw, co = bn_mask
     assert x_raw.dtype == BF16 and x_raw.is_contiguous() and x_raw.shape[-1] == C and C % 64 == 0
-    rows = lib.b200_conv2d_fwd_stats_rows(B, H, W, C, ksize, 1)
+    if groups != 1:   # (the grouped kernel runs 64-channel tiles: its own row count)
+        rows = lib.b200_conv2d_grouped_fwd_stats_rows(B, H, W, C, groups, ksize, 1)
+        _lib.check(min(rows, 0), "b200_conv2d_grouped_fwd_stats_rows")
+    else:
+        rows = lib.b200_conv2d_fwd_stats_rows(B, H, W, C, ksize, 1)
     stats = torch.empty(rows, 2, C, dtype=F32, device=x_raw.device)
     _lib.check(lib.b200_dgrad_set_bn_mask(_p(x_raw), _p(co.scale), _p(co.shift), _p(stats)), "b200_dgrad_set_bn_mask")
     return stats
 
 
-def conv2d_dgrad(dy, wd_packed, in_hw, ksize=1, stride=1, residual=None, out=None, bn_mask=None):
+def conv2d_dgrad(dy, wd_packed, in_hw, ksize=1, stride=1, residual=None, out=None, bn_mask=None, groups=1):
     """dx[B,H,W,Cin] from dy[B,Ho,Wo,Cout]; wd_packed = pack_weight(w, mode=1). `out` lets 1x1/s2 accumulate in place.
     bn_mask = (x_raw, BnCoeffs) (stride 1): dx is the gradient of relu(bn(x_raw)); returns (dz, partial sums) for
-    bn_backward_from_sums instead of dx."""
+    bn_backward_from_sums instead of dx.  groups > 1: grouped 3x3 convolution (wd_packed = pack_weight(w, mode=4)), no
+    residual / out."""
     lib = _lib.load()
     _chk_act(dy, "dy")
     B, Ho, Wo, Cout = dy.shape
     H, W = in_hw
     Cin = wd_packed.shape[0]
+    if groups != 1:
+        if residual is not None or out is not None:
+            raise ValueError("conv2d_dgrad: a grouped convolution takes no residual or out")
+        dx = torch.empty(B, H, W, Cin, dtype=BF16, device=dy.device)
+        stats = None
+        if bn_mask is not None:
+            assert stride == 1, "bn_mask needs a stride-1 convolution"
+            stats = _arm_bn_mask(lib, bn_mask, B, H, W, Cin, ksize, groups)
+        sp = _span("conv_gemm_grouped_dgrad", 2.0 * B * Ho * Wo * Cout * (Cin // groups) * ksize * ksize,
+                   _nb(dy, wd_packed, dx, bn_mask[0] if bn_mask else None))
+        rc = lib.b200_conv2d_grouped_dgrad(_p(dy), _p(wd_packed), _p(dx), B, H, W, Cin, groups, ksize, stride, _stream())
+        _lib.check(rc, "b200_conv2d_grouped_dgrad")
+        if sp:
+            sp.end()
+        return dx if bn_mask is None else (dx, stats)
     if out is not None:
         dx = out
     elif ksize == 1 and stride == 2:
@@ -237,15 +285,32 @@ def _workspace(nbytes, device):
     return ws
 
 
-def conv2d_wgrad(dy, x, ksize=1, stride=1, out=None, accumulate=False, rowscale=None, bias_out=None):
+def conv2d_wgrad(dy, x, ksize=1, stride=1, out=None, accumulate=False, rowscale=None, bias_out=None, groups=1):
     """dw fp32 OIHW [Cout, Cin, k, k] = sum over pixels of dy (x) x  (row `cout` optionally scaled by rowscale[cout]).
     bias_out (fp32 [Cout]): also write the bias gradient (column sums of dy), summed from the dy tiles the kernel already
-    holds in shared memory - no extra pass over dy."""
+    holds in shared memory - no extra pass over dy.  groups > 1: grouped 3x3 convolution, dw [C, C/groups, k, k]."""
     lib = _lib.load()
     _chk_act(dy, "dy")
     _chk_act(x, "x")
     B, H, W, Cin = x.shape
     Cout = dy.shape[-1]
+    if groups != 1:
+        if rowscale is not None or bias_out is not None:
+            raise ValueError("conv2d_wgrad: a grouped convolution takes no rowscale or bias gradient")
+        nbytes = lib.b200_conv2d_grouped_wgrad_workspace_bytes(B, H, W, Cin, groups, ksize, stride)
+        if nbytes == 0:
+            raise RuntimeError(f"b200_conv2d_grouped_wgrad_workspace_bytes failed: {_lib.last_error()}")
+        ws = _workspace(nbytes, x.device)
+        if out is None:
+            out = torch.empty(Cout, Cin // groups, ksize, ksize, dtype=F32, device=x.device)
+            accumulate = False
+        sp = _span("wgrad_gemm_grouped", 2.0 * dy.numel() * (Cin // groups) * ksize * ksize, _nb(dy, x, out))
+        rc = lib.b200_conv2d_grouped_wgrad(_p(dy), _p(x), _p(out), _p(ws), ws.numel(), B, H, W, Cin, groups, ksize, stride,
+                                           1 if accumulate else 0, _stream())
+        _lib.check(rc, "b200_conv2d_grouped_wgrad")
+        if sp:
+            sp.end()
+        return out
     nbytes = lib.b200_conv2d_wgrad_workspace_bytes(B, H, W, Cin, Cout, ksize, stride)
     ws = _workspace(nbytes, x.device)
     if out is None:

@@ -94,6 +94,24 @@ int b200_conv2d_wgrad_set_bias_partial(float* bias_partial);
 int b200_conv2d_wgrad_set_bias_out(float* bias_out);
 int b200_conv2d_wgrad_splits(int B, int H, int W, int Cin, int Cout, int ksize, int stride);
 
+/* ---- grouped 3x3 convolution (ResNeXt conv2: classification/resnet/models/networks.py:295-321, nn.Conv2d(groups=g)) ------
+ * C input = C output channels, C % 64 == 0, group width Cg = C / groups in {4, 8, 16, 32, 64}, ksize 3 (pad 1), stride 1 / 2.
+ * Anything else returns B200_EINVAL with a message and launches nothing.
+ * forward: y[B,Ho,Wo,C] = conv(x[B,H,W,C], w) (act: 0 or B200_ACT_RELU); w bf16 [C][9*64] (b200_pack_weight mode 3);
+ *   stats as for b200_conv2d_fwd, rows = b200_conv2d_grouped_fwd_stats_rows(); honours b200_conv2d_fwd_set_bn. */
+int b200_conv2d_grouped_fwd(const void* x, const void* w, void* y, int B, int H, int W, int C, int groups, int ksize,
+                            int stride, float* stats, int act, void* stream);
+int b200_conv2d_grouped_fwd_stats_rows(int B, int H, int W, int C, int groups, int ksize, int stride);
+/* data gradient dx[B,H,W,C] from dy[B,Ho,Wo,C]; wd bf16 [C][9*64] (b200_pack_weight mode 4). Honours b200_dgrad_set_bn_mask at
+ * stride 1, with rows = b200_conv2d_grouped_fwd_stats_rows(B, H, W, C, groups, 3, 1). */
+int b200_conv2d_grouped_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int C, int groups, int ksize,
+                              int stride, void* stream);
+/* weight gradient dw[C][C/groups][3][3] (fp32, OIHW) (+)= sum_pixels dy (x) x within each group; workspace =
+ * b200_conv2d_grouped_wgrad_workspace_bytes() bytes (0 for an unsupported shape). */
+int b200_conv2d_grouped_wgrad(const void* dy, const void* x, float* dw, void* workspace, size_t workspace_bytes, int B,
+                              int H, int W, int C, int groups, int ksize, int stride, int accumulate, void* stream);
+size_t b200_conv2d_grouped_wgrad_workspace_bytes(int B, int H, int W, int C, int groups, int ksize, int stride);
+
 /* ---- general GEMM with strided pixel views (transformer layers, patch embedding) ----------------------------------------
  * out[pixel, n] = epilogue( sum_k a[pixel, k] * w[n, k] ), pixels = dim[0] x dim[1] x dim[2] (w fastest), channel stride 1.
  * `a` and `out` must have identical pixel extents; strides are in elements and let `out`/`residual` be token-offset or
@@ -275,11 +293,14 @@ int b200_softmax_xent_soft(const float* logits, long long ld, const long long* l
 int b200_mean(const float* v, int n, float* out, void* stream);
 int b200_colsum_bf16(const void* m, long long rows, long long ld, int cols, float* out, int accumulate, void* stream);
 
-/* weight packing fp32 OIHW -> bf16 GEMM operand; mode 0: [O][taps*I] (pitch ld_dst), mode 1: [I][taps*O] */
+/* weight packing fp32 OIHW -> bf16 GEMM operand; mode 0: [O][taps*I] (pitch ld_dst), mode 1: [I][taps*O];
+ * grouped convolution weight [C][Cg][taps] (O = C, I = Cg): mode 3 = block-diagonal forward operand [C][taps*64],
+ * mode 4 = block-diagonal dgrad operand [C][taps*64] (transposed within each group, taps unflipped like mode 1) */
 int b200_pack_weight(const float* src, void* dst, int O, int I, int taps, int mode, long long ld_dst, void* stream);
 /* all weights of a model in one launch: table[n][10] int64 {src, dst, O, I, taps, mode, ld_dst, first_block, rows_out,
  * oscale (optional fp32 [O] multiplier per output channel, 0 = none)}; mode 0 = forward / wgrad operand [O][tap*I+i],
- * 1 = dgrad operand [I][tap*O+o], 2 = space-to-depth stem operand [O][256] of a [O][3][7][7] kernel */
+ * 1 = dgrad operand [I][tap*O+o], 2 = space-to-depth stem operand [O][256] of a [O][3][7][7] kernel, 3 / 4 = grouped
+ * forward / dgrad operands as for b200_pack_weight (rows_out = O = C) */
 int b200_pack_weights_multi(const void* table, int n_entries, int total_blocks, void* stream);
 int b200_cast_f32_to_bf16(const float* src, void* dst, long long n, void* stream);
 int b200_cast_bf16_to_f32(const void* src, float* dst, long long n, void* stream);
