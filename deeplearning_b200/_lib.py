@@ -32,18 +32,22 @@ class GemmArgs(ctypes.Structure):
                 ("aux_in", ctypes.POINTER(View)), ("stats", c_void_p), ("rowscale", c_void_p), ("rows_per_sample", c_int)]
 
 
+class BnMask(ctypes.Structure):
+    """b200_bn_mask_t"""
+    _fields_ = [("x_raw", c_void_p), ("scale", c_void_p), ("shift", c_void_p), ("stats", c_void_p)]
+
+
+
 # name -> (restype, argtypes); must list every symbol of include/b200cls.h (tests/test_abi.py checks this).
 SIGNATURES = {
     "b200_last_error": (c_char_p, []),
     "b200_abi_version": (_I, []),
     "b200_sm_count": (_I, []),
     "b200_launch_count": (ctypes.c_ulonglong, []),
-    "b200_conv2d_fwd": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _L, _P]),
+    "b200_conv2d_fwd": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _P, _L, _P, _P, _P]),
     "b200_conv2d_fwd_stats_rows": (_I, [_I, _I, _I, _I, _I, _I]),
-    "b200_conv2d_fwd_set_bn": (_I, [_P, _P]),
-    "b200_dgrad_set_bn_mask": (_I, [_P, _P, _P, _P]),
-    "b200_conv2d_dgrad": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
-    "b200_conv2d_wgrad": (_I, [_P, _P, _P, _P, c_size_t, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_conv2d_dgrad": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, ctypes.POINTER(BnMask), _P]),
+    "b200_conv2d_wgrad": (_I, [_P, _P, _P, _P, c_size_t, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
     "b200_conv2d_wgrad_workspace_bytes": (c_size_t, [_I, _I, _I, _I, _I, _I, _I]),
     "b200_reduce_scratch_bytes": (c_size_t, [_I, _I]),
     "b200_gemm_ex": (_I, [ctypes.POINTER(View), ctypes.POINTER(View), ctypes.POINTER(GemmArgs), _P]),
@@ -58,13 +62,10 @@ SIGNATURES = {
     "b200_colsum_partial": (_I, [_P, _L, _L, _I, _P, _P]),
     "b200_attention_fwd": (_I, [_P, _P, _P, _I, _I, _I, _F, _P]),
     "b200_attention_bwd": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _P]),
-    "b200_conv2d_wgrad_set_rowscale": (_I, [_P]),
-    "b200_conv2d_wgrad_set_bias_partial": (_I, [_P]),
-    "b200_conv2d_wgrad_set_bias_out": (_I, [_P]),
     "b200_conv2d_wgrad_splits": (_I, [_I, _I, _I, _I, _I, _I, _I]),
-    "b200_conv2d_grouped_fwd": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P]),
+    "b200_conv2d_grouped_fwd": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P, _P, _P]),
     "b200_conv2d_grouped_fwd_stats_rows": (_I, [_I, _I, _I, _I, _I, _I, _I]),
-    "b200_conv2d_grouped_dgrad": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "b200_conv2d_grouped_dgrad": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, ctypes.POINTER(BnMask), _P]),
     "b200_conv2d_grouped_wgrad": (_I, [_P, _P, _P, _P, c_size_t, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "b200_conv2d_grouped_wgrad_workspace_bytes": (c_size_t, [_I, _I, _I, _I, _I, _I, _I]),
     "b200_dwconv7_pack": (_I, [_P, _P, _I, _P]),
@@ -108,7 +109,6 @@ SIGNATURES = {
     "b200_cast_f32_to_bf16": (_I, [_P, _P, _L, _P]),
     "b200_cast_bf16_to_f32": (_I, [_P, _P, _L, _P]),
     "b200_im2col_nchw": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
-    "b200_debug_set_desc": (_I, [_I, ctypes.c_uint, ctypes.c_uint, ctypes.c_uint]),
     "b200_stem_wgrad_relayout": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
     "b200_stem_s2d": (_I, [_P, _P, _I, _I, _I, _P]),
     "b200_stem_s2d_u8": (_I, [_P, _P, _I, _I, _I, ctypes.POINTER(c_float), ctypes.POINTER(c_float), _P]),
@@ -126,7 +126,7 @@ SIGNATURES = {
     "b200_conv1x1_dgrad_masked": (_I, [_P, _P, _P, _L, _I, _I, _P, _P, _P, _P]),
     "b200_bn_conv1x1_bwd_scratch_bytes": (c_size_t, [_I, _I]),
     "b200_bn_conv1x1_bwd": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _D, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P, c_size_t, _P, _P]),
-    "b200_gemm_dual": (_I, [_P, _I, _P, _I, _P, _P, _P, _L, _I, _P]),
+    "b200_gemm_dual": (_I, [_P, _I, _P, _I, _P, _P, _P, _L, _I, ctypes.POINTER(BnMask), _P]),
     "b200_rowscale_bf16": (_I, [_P, _P, _P, _L, _L, _P]),
     "b200_tanh_fwd": (_I, [_P, _P, _P, _L, _P]),
     "b200_tanh_bwd": (_I, [_P, _P, _P, _L, _P]),

@@ -13,21 +13,9 @@ using namespace b200;
 
 namespace {
 
-// Descriptor strides; overridable through b200_debug_set_desc() for bring-up experiments only.
-uint32_t g_fwd_lbo = 16, g_fwd_sbo = 1024;
-uint32_t g_wg_lbo = 8192, g_wg_sbo = 1024, g_wg_kstep = 2048;
-// one-shot per-output-channel multiplier for the next b200_conv2d_wgrad call (see b200_conv2d_wgrad_set_rowscale)
-thread_local const float* g_wgrad_rowscale = nullptr;
-thread_local float* g_wgrad_bias_partial = nullptr;
-thread_local float* g_wgrad_bias_out = nullptr;   // one-shot with bias_partial: the reduce kernel writes the finished bias gradient
-thread_local const float* g_fwd_bn_scale = nullptr;   // one-shot: fold y = conv * scale + shift (eval-mode BN) into the epilogue
-thread_local const float* g_fwd_bn_shift = nullptr;
-// one-shot (b200_dgrad_set_bn_mask): the next stride-1 dgrad / dual GEMM masks its output with relu'(bn(x_raw)) and writes the
-// sum(dz), sum(dz * x_raw) partial rows of that BatchNorm's backward
-thread_local const void* g_bnmask_x = nullptr;
-thread_local const float* g_bnmask_scale = nullptr;
-thread_local const float* g_bnmask_shift = nullptr;
-thread_local float* g_bnmask_stats = nullptr;
+// wgmma shared-memory descriptor strides (bytes): K-major operands of conv_gemm / conv_tap64, MN-major operands of wgrad_gemm
+constexpr uint32_t kFwdDescLbo = 16, kFwdDescSbo = 1024;
+constexpr uint32_t kWgDescLbo = 8192, kWgDescSbo = 1024, kWgDescKstep = 2048;
 
 struct Box3 {
   int b1, b2, b3;
@@ -56,6 +44,15 @@ Box3 choose_box(long long d1, long long d2, long long d3, int P) {
 
 inline int pad_of(int ksize) { return ksize == 2 ? 0 : ksize / 2; }  // 2x2/s2 patch-merging convs are unpadded
 inline int out_dim(int in, int ksize, int stride) { return (in + 2 * pad_of(ksize) - ksize) / stride + 1; }
+
+// Output pixel extents (w, h, n) of a convolution; a 1x1 / stride-1 one is a single flat run of B*H*W pixels.
+struct Dims3 {
+  long long d1, d2, d3;
+};
+Dims3 out_dims(int B, int H, int W, int ksize, int stride) {
+  if (ksize == 1 && stride == 1) return Dims3{static_cast<long long>(B) * H * W, 1, 1};
+  return Dims3{out_dim(W, ksize, stride), out_dim(H, ksize, stride), B};
+}
 
 // 4-D activation view descriptor (channels innermost).
 struct View {
@@ -92,6 +89,10 @@ View make_flat_view(const void* base, long long M, int C) {
   v.strides[3] = static_cast<uint64_t>(M) * C;
   return v;
 }
+// The pixels of a GEMM operand / output, flattened for a 1x1 / stride-1 convolution.
+View act_view(const void* base, int B, int H, int W, int C, bool flat) {
+  return flat ? make_flat_view(base, static_cast<long long>(B) * H * W, C) : make_view(base, B, H, W, C, 1, 0, 0);
+}
 int encode_view(CUtensorMap* m, const View& v, const Box3& bx) {
   uint32_t box[4] = {64, (uint32_t)bx.b1, (uint32_t)bx.b2, (uint32_t)bx.b3};
   if (v.dims[1] == 0 || v.dims[2] == 0 || v.dims[3] == 0) {
@@ -99,6 +100,42 @@ int encode_view(CUtensorMap* m, const View& v, const Box3& bx) {
     return EINVAL_;
   }
   return encode_tmap_bf16(m, v.base, 4, v.dims, v.strides, box);
+}
+
+// Row-major bf16 matrix [rows][cols] (e.g. a GEMM weight [N][K]) loaded in boxes of 64 columns x box_rows rows.
+int encode_matrix(CUtensorMap* m, const void* base, long long cols, long long rows, int box_rows) {
+  uint64_t dims[2] = {static_cast<uint64_t>(cols), static_cast<uint64_t>(rows)};
+  uint64_t strides[2] = {1, static_cast<uint64_t>(cols)};
+  uint32_t box[2] = {64, static_cast<uint32_t>(box_rows)};
+  return encode_tmap_bf16(m, base, 2, dims, strides, box);
+}
+
+// Activation operand x[B][H][W][C] of a ksize x ksize / `stride` convolution whose output pixels are tiled by `bx`: its
+// tensor maps (one; or one per pixel phase at stride 2) and the tap table - tap t = kh * ksize + kw reads map tap_map[t]
+// at offset (tap_o1[t], tap_o2[t]) from the output pixel.
+template <class Params>
+int encode_taps(Params& p, CUtensorMap (&maps)[4], const void* x, int B, int H, int W, int C, int ksize, int stride,
+                const Box3& bx) {
+  int rc;
+  if (stride == 1) {
+    if ((rc = encode_view(&maps[0], act_view(x, B, H, W, C, ksize == 1), bx))) return rc;
+    for (int i = 1; i < 4; ++i) maps[i] = maps[0];
+  } else {
+    for (int ph = 0; ph < 2; ++ph)
+      for (int pw = 0; pw < 2; ++pw)
+        if ((rc = encode_view(&maps[ph * 2 + pw], make_view(x, B, H, W, C, 2, ph, pw), bx))) return rc;
+  }
+  // stride 2: tap (kh,kw) reads input row 2*oh + kh - pad -> phase ((kh-pad)&1), index oh + floor((kh-pad)/2)
+  const int pad = pad_of(ksize);
+  for (int kh = 0; kh < ksize; ++kh)
+    for (int kw = 0; kw < ksize; ++kw) {
+      const int t = kh * ksize + kw, dh = kh - pad, dw = kw - pad;
+      const int ph = stride == 2 ? dh & 1 : 0, pw = stride == 2 ? dw & 1 : 0;
+      p.tap_map[t] = static_cast<int8_t>(ph * 2 + pw);
+      p.tap_o1[t] = static_cast<int8_t>((dw - pw) / stride);
+      p.tap_o2[t] = static_cast<int8_t>((dh - ph) / stride);
+    }
+  return OK;
 }
 
 // The epilogue stores one quadrant (32 consecutive tile rows) per warp: split the 128-pixel box into 4 slabs along
@@ -168,6 +205,17 @@ int setup_output(ConvGemmParams& p, const View& dv, int N, int out_f32, const Vi
   return OK;
 }
 Box3 box_of(const ConvGemmParams& p) { return Box3{p.box1, p.box2, p.box3}; }
+
+bool bn_mask_complete(const b200_bn_mask_t* m) { return m->x_raw && m->scale && m->shift && m->stats; }
+// kEpiBnMask epilogue: mask the output (view dv; x_raw has the same layout) with relu'(bn(x_raw)) and write the sum(dz),
+// sum(dz * x_raw) partial rows of that BatchNorm's backward.
+void set_bn_mask(ConvGemmParams& p, const b200_bn_mask_t* m, const View& dv) {
+  p.mask_in = static_cast<const __nv_bfloat16*>(m->x_raw);
+  p.ms1 = static_cast<long long>(dv.strides[1]);
+  p.ms2 = static_cast<long long>(dv.strides[2]);
+  p.ms3 = static_cast<long long>(dv.strides[3]);
+  p.bn_scale = m->scale, p.bn_shift = m->shift, p.stats = m->stats;
+}
 
 // Persistent grid. With BN statistics every CTA must keep seeing the same channel block (tile % n_tiles), so the grid is
 // rounded down to a multiple of n_tiles.
@@ -262,8 +310,8 @@ int launch_conv_gemm(const ConvGemmParams& p, cudaStream_t st) {
   const int grid = conv_grid(tiles, p.n_tiles, p.stats != nullptr);
   B200_REQUIRE(grid > 0, "conv_gemm: %d channel blocks exceed the SM count (BN statistics need grid %% n_tiles == 0)", p.n_tiles);
   ConvGemmParams q = p;
-  q.desc_lbo = g_fwd_lbo;
-  q.desc_sbo = g_fwd_sbo;
+  q.desc_lbo = kFwdDescLbo;
+  q.desc_sbo = kFwdDescSbo;
   if constexpr (BLOCK_N == 64) {
     if (tap64_ok(p)) return p.stats != nullptr ? launch_tap64<true>(q, grid, st) : launch_tap64<false>(q, grid, st);
   }
@@ -318,26 +366,11 @@ int run_stream(int mode, const void* a, const void* w, void* out, const void* re
   StreamParams q;
   memset(&q, 0, sizeof(q));
   int rc;
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(pixels)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(K)};
-    uint32_t box[2] = {64, 128};
-    if ((rc = encode_tmap_bf16(&q.a_map, a, 2, dims, strides, box))) return rc;
-  }
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(K), static_cast<uint64_t>(N)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(K)};
-    uint32_t box[2] = {64, 256};
-    if ((rc = encode_tmap_bf16(&q.b_map, w, 2, dims, strides, box))) return rc;
-  }
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(N), static_cast<uint64_t>(pixels)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(N)};
-    uint32_t box[2] = {64, 16};
-    if ((rc = encode_tmap_bf16(&q.out_map, out, 2, dims, strides, box))) return rc;
-    if (res != nullptr && (rc = encode_tmap_bf16(&q.res_map, res, 2, dims, strides, box))) return rc;
-    if (mask != nullptr && (rc = encode_tmap_bf16(&q.mask_map, mask, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_matrix(&q.a_map, a, K, pixels, 128))) return rc;
+  if ((rc = encode_matrix(&q.b_map, w, K, N, 256))) return rc;
+  if ((rc = encode_matrix(&q.out_map, out, N, pixels, 16))) return rc;
+  if (res != nullptr && (rc = encode_matrix(&q.res_map, res, N, pixels, 16))) return rc;
+  if (mask != nullptr && (rc = encode_matrix(&q.mask_map, mask, N, pixels, 16))) return rc;
   q.m_tiles = static_cast<int>(pixels / 128);
   q.n_tiles = N / 256;
   q.N = N;
@@ -378,9 +411,9 @@ int launch_wgrad(const WgradParams& p, cudaStream_t st) {
   const int items = p.mg_tiles * p.ng_tiles * p.num_taps * p.splits;
   const int grid = items < device_sm_count() ? items : device_sm_count();
   WgradParams q = p;
-  q.desc_lbo = g_wg_lbo;
-  q.desc_sbo = g_wg_sbo;
-  q.desc_kstep = g_wg_kstep;
+  q.desc_lbo = kWgDescLbo;
+  q.desc_sbo = kWgDescSbo;
+  q.desc_kstep = kWgDescKstep;
   if constexpr (kGrouped)
     B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, false, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
   else if (q.bias_partial != nullptr)   // + four warps that sum the dY tiles' columns (the layer's bias gradient)
@@ -393,7 +426,7 @@ int launch_wgrad(const WgradParams& p, cudaStream_t st) {
 
 // partial[splits][Cout][taps*Cin] -> grad[Cout][Cin][taps] (+)=, see wgrad_gemm.cuh
 int launch_wgrad_reduce(const float* partial, float* dw, int splits, int Cout, int Cin, int taps, int accumulate,
-                         const float* rowscale, cudaStream_t st, const float* bias_partial = nullptr, float* bias_out = nullptr) {
+                        cudaStream_t st, const float* bias_partial = nullptr, float* bias_out = nullptr) {
   const long long total = static_cast<long long>(Cout) * Cin * taps;
   if (Cin % 8 == 0 && (reinterpret_cast<uintptr_t>(partial) & 15) == 0) {
     int chunk = taps == 1 ? 256 : 64;
@@ -403,13 +436,13 @@ int launch_wgrad_reduce(const float* partial, float* dw, int splits, int Cout, i
     const size_t smem = static_cast<size_t>(SL) * taps * chunk * sizeof(float);
     if (smem <= 48 * 1024 && Cout <= 65535 * 32) {
       dim3 grid(Cout, (Cin + chunk - 1) / chunk);
-      B200_CHECK_CUDA(launch_pdl(wgrad_reduce_rows_kernel, dim3(grid), dim3(256), smem, st, partial, dw, splits, Cout, Cin, taps, chunk, SL, accumulate, rowscale, bias_partial, bias_out));
+      B200_CHECK_CUDA(launch_pdl(wgrad_reduce_rows_kernel, dim3(grid), dim3(256), smem, st, partial, dw, splits, Cout, Cin, taps, chunk, SL, accumulate, bias_partial, bias_out));
       return OK;
     }
   }
   int blocks = static_cast<int>((total + 255) / 256);
   if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
-  B200_CHECK_CUDA(launch_pdl(wgrad_reduce_flat_kernel, dim3(blocks), dim3(256), 0, st, partial, dw, splits, Cout, Cin, taps, accumulate, rowscale, bias_partial, bias_out));
+  B200_CHECK_CUDA(launch_pdl(wgrad_reduce_flat_kernel, dim3(blocks), dim3(256), 0, st, partial, dw, splits, Cout, Cin, taps, accumulate, bias_partial, bias_out));
   return OK;
 }
 
@@ -470,51 +503,40 @@ WgradPlan plan_wgrad_geom(long long d1, long long d2, long long d3, int Cin, int
 }
 
 WgradPlan plan_wgrad(int B, int H, int W, int Cin, int Cout, int ksize, int stride, bool grouped = false) {
-  const int Ho = out_dim(H, ksize, stride), Wo = out_dim(W, ksize, stride);
-  const bool flat = (ksize == 1 && stride == 1);
-  WgradPlan pl = plan_wgrad_geom(flat ? static_cast<long long>(B) * H * W : Wo, flat ? 1 : Ho, flat ? 1 : B, Cin, Cout,
-                                 ksize * ksize, grouped);
-  pl.Ho = Ho, pl.Wo = Wo;
+  const Dims3 d = out_dims(B, H, W, ksize, stride);
+  WgradPlan pl = plan_wgrad_geom(d.d1, d.d2, d.d3, Cin, Cout, ksize * ksize, grouped);
+  pl.Ho = out_dim(H, ksize, stride), pl.Wo = out_dim(W, ksize, stride);
   return pl;
 }
 
-// Tensor maps of dY and of the activation (tap / phase views) of a weight-gradient launch, and its tap table.
+// Bytes of the fp32 split-K partials [splits][Cout][taps * Cin] a weight-gradient launch writes to its workspace.
+size_t wgrad_bytes(const WgradPlan& pl, int Cout, int Cin) {
+  return static_cast<size_t>(pl.splits) * Cout * pl.taps * Cin * sizeof(float);
+}
+
+// Tile, split and partial-layout fields of a weight-gradient launch.
+WgradParams wgrad_params(const WgradPlan& pl, int Cout, int Cin, void* workspace) {
+  WgradParams p;
+  memset(&p, 0, sizeof(p));
+  p.num_taps = pl.merge_atoms ? 1 : pl.taps;
+  p.merge_atoms = pl.merge_atoms;
+  p.n_cols = pl.merge_atoms ? pl.taps * Cin : Cin;
+  p.Cout = Cout, p.Cin = Cin;
+  p.mg_tiles = pl.mg_tiles, p.ng_tiles = pl.ng_tiles;
+  p.tiles1 = pl.tiles1, p.tiles2 = pl.tiles2, p.tiles3 = pl.tiles3;
+  p.box1 = pl.box.b1, p.box2 = pl.box.b2, p.box3 = pl.box.b3;
+  p.splits = pl.splits, p.kb_per_split = pl.kb_per_split, p.kb_total = pl.kb_total;
+  p.ld_partial = static_cast<long long>(pl.taps) * Cin;
+  p.partial = static_cast<float*>(workspace);
+  return p;
+}
+
+// Tensor maps of dY and of the activation taps of a weight-gradient launch, and its tap table.
 int setup_wgrad_maps(WgradParams& p, const WgradPlan& pl, const void* dy, const void* x, int B, int H, int W, int Cin,
                      int Cout, int ksize, int stride) {
-  const bool flat = (ksize == 1 && stride == 1);
   int rc;
-  View dyv = flat ? make_flat_view(dy, static_cast<long long>(B) * H * W, Cout)
-                  : make_view(dy, B, pl.Ho, pl.Wo, Cout, 1, 0, 0);
-  if ((rc = encode_view(&p.dy_map, dyv, pl.box))) return rc;
-  if (flat) {
-    if ((rc = encode_view(&p.x_maps[0], make_flat_view(x, static_cast<long long>(B) * H * W, Cin), pl.box))) return rc;
-    for (int i = 1; i < 4; ++i) p.x_maps[i] = p.x_maps[0];
-  } else if (stride == 1) {
-    if ((rc = encode_view(&p.x_maps[0], make_view(x, B, H, W, Cin, 1, 0, 0), pl.box))) return rc;
-    for (int i = 1; i < 4; ++i) p.x_maps[i] = p.x_maps[0];
-    for (int kh = 0; kh < ksize; ++kh)
-      for (int kw = 0; kw < ksize; ++kw) {
-        const int t = kh * ksize + kw;
-        p.tap_map[t] = 0;
-        p.tap_o1[t] = static_cast<int8_t>(kw - ksize / 2);
-        p.tap_o2[t] = static_cast<int8_t>(kh - ksize / 2);
-      }
-  } else {
-    for (int ph = 0; ph < 2; ++ph)
-      for (int pw = 0; pw < 2; ++pw)
-        if ((rc = encode_view(&p.x_maps[ph * 2 + pw], make_view(x, B, H, W, Cin, 2, ph, pw), pl.box))) return rc;
-    const int pad = pad_of(ksize);
-    for (int kh = 0; kh < ksize; ++kh)
-      for (int kw = 0; kw < ksize; ++kw) {
-        const int t = kh * ksize + kw;
-        const int dh = kh - pad, dw_ = kw - pad;
-        const int ph = dh & 1, pw = dw_ & 1;
-        p.tap_map[t] = static_cast<int8_t>(ph * 2 + pw);
-        p.tap_o1[t] = static_cast<int8_t>((dw_ - pw) / 2);
-        p.tap_o2[t] = static_cast<int8_t>((dh - ph) / 2);
-      }
-  }
-  return OK;
+  if ((rc = encode_view(&p.dy_map, act_view(dy, B, pl.Ho, pl.Wo, Cout, ksize == 1 && stride == 1), pl.box))) return rc;
+  return encode_taps(p, p.x_maps, x, B, H, W, Cin, ksize, stride, pl.box);
 }
 
 // Space-to-depth stem (conv 7x7 / stride 2 / pad 3 on 3 channels, classification/resnet/models/networks.py:150,206):
@@ -536,24 +558,11 @@ View stem_s2d_view(const void* z, int B, int Ho, int Wo) {
 
 extern "C" {
 
-int b200_debug_set_desc(int which, unsigned lbo, unsigned sbo, unsigned kstep) {
-  if (which == 0) {
-    g_fwd_lbo = lbo, g_fwd_sbo = sbo;
-  } else {
-    g_wg_lbo = lbo, g_wg_sbo = sbo, g_wg_kstep = kstep;
-  }
-  return OK;
-}
-
 // Statistics rows of a forward launch with BN-column tiles (see b200_conv2d_fwd_stats_rows).
 static int fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int stride, int BN) {
-  const int Ho = out_dim(H, ksize, stride), Wo = out_dim(W, ksize, stride);
-  const bool flat = (ksize == 1 && stride == 1);
-  const long long d1 = flat ? static_cast<long long>(B) * H * W : Wo;
-  const long long d2 = flat ? 1 : Ho;
-  const long long d3 = flat ? 1 : B;
-  const Box3 bx = choose_box(d1, d2, d3, 128);
-  const long long m_tiles = ((d1 + bx.b1 - 1) / bx.b1) * ((d2 + bx.b2 - 1) / bx.b2) * ((d3 + bx.b3 - 1) / bx.b3);
+  const Dims3 d = out_dims(B, H, W, ksize, stride);
+  const Box3 bx = choose_box(d.d1, d.d2, d.d3, 128);
+  const long long m_tiles = ((d.d1 + bx.b1 - 1) / bx.b1) * ((d.d2 + bx.b2 - 1) / bx.b2) * ((d.d3 + bx.b3 - 1) / bx.b3);
   const int n_tiles = (Cout + BN - 1) / BN;
   const long long tiles = m_tiles * n_tiles;
   const int grid = conv_grid(tiles > (1 << 30) ? (1 << 30) : static_cast<int>(tiles), n_tiles, true);
@@ -566,171 +575,101 @@ int b200_conv2d_fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int str
   return fwd_stats_rows(B, H, W, Cout, ksize, stride, block_n_for(Cout));
 }
 
-static thread_local int g_conv_out_f32_tma = 0;
-
-int b200_conv2d_fwd_f32(const void* x, const void* w, float* y, int B, int H, int W, int Cin, int Cout, int ksize,
-                        int stride, const float* bias, void* stream) {
-  g_conv_out_f32_tma = 1;
-  const int rc = b200_conv2d_fwd(x, w, y, B, H, W, Cin, Cout, ksize, stride, nullptr, bias, 0, nullptr, nullptr, 0, stream);
-  g_conv_out_f32_tma = 0;
-  return rc;
-}
-
-// Cg > 0: grouped convolution of group width Cg (Cin == Cout, validated by the caller) in channel-window mode
+// y_f32: y is an fp32 tensor written through TMA (b200_conv2d_fwd_f32).
+// bn_scale / bn_shift: y = act(conv * scale[c] + shift[c] (+ residual)) - BatchNorm with fixed (running) statistics folded
+// into the epilogue; the activation moves AFTER the residual add (conv_gemm.cuh kEpiAffine).
+// Cg > 0: grouped convolution of group width Cg (Cin == Cout, validated by the caller) in channel-window mode.
 static int conv_fwd(const void* x, const void* w, void* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride,
                     float* stats, const float* bias, int act, const void* residual, float* out_f32, long long ld_out,
-                    void* stream, int Cg) {
+                    const float* bn_scale, const float* bn_shift, int y_f32, int Cg, void* stream) {
   B200_REQUIRE(ksize == 1 || ksize == 3 || (ksize == 2 && stride == 2), "conv2d_fwd: ksize %d / stride %d unsupported", ksize, stride);
   B200_REQUIRE(stride == 1 || stride == 2, "conv2d_fwd: stride %d unsupported (1 or 2)", stride);
   B200_REQUIRE(Cin % 8 == 0 && Cout % 8 == 0, "conv2d_fwd: Cin=%d / Cout=%d must be multiples of 8", Cin, Cout);
   B200_REQUIRE(B > 0 && H > 0 && W > 0, "conv2d_fwd: empty input");
+  B200_REQUIRE(stride == 1 || (H >= 2 && W >= 2), "conv2d_fwd: stride-2 needs H,W >= 2");
   B200_REQUIRE(out_f32 == nullptr || (ksize == 1 && stride == 1), "conv2d_fwd: fp32 output only for 1x1/s1");
+  B200_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), "conv2d_fwd: bn_scale and bn_shift go together");
+  B200_REQUIRE(bn_scale == nullptr || (Cout % 64 == 0 && bias == nullptr && stats == nullptr && out_f32 == nullptr && act <= 1 && !y_f32),
+               "conv2d_fwd + folded BN: Cout=%d must be a multiple of 64, no bias / statistics / fp32 output", Cout);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int Ho = out_dim(H, ksize, stride), Wo = out_dim(W, ksize, stride);
-  const bool flat = (ksize == 1 && stride == 1);
   ConvGemmParams p;
   memset(&p, 0, sizeof(p));
-  const long long d1 = flat ? static_cast<long long>(B) * H * W : Wo;
-  const long long d2 = flat ? 1 : Ho;
-  const long long d3 = flat ? 1 : B;
   int rc;
-  {
-    View dv = flat ? make_flat_view(y, d1, Cout) : make_view(y, B, Ho, Wo, Cout, 1, 0, 0);
-    if (out_f32 != nullptr) dv.base = nullptr;  // direct fp32 stores, no TMA map
-    if ((rc = setup_output(p, dv, Cout, g_conv_out_f32_tma, nullptr))) return rc;
-  }
-  const Box3 bx = box_of(p);
+  View dv = act_view(y, B, Ho, Wo, Cout, ksize == 1 && stride == 1);
+  if (out_f32 != nullptr) dv.base = nullptr;  // direct fp32 stores, no TMA map
+  if ((rc = setup_output(p, dv, Cout, y_f32, nullptr))) return rc;
   const int BN = Cg ? 64 : block_n_for(Cout);
   p.n_tiles = (Cout + BN - 1) / BN;
   p.chan_window = Cg ? 1 : 0;
   p.k_per_tap = Cg ? 64 : Cin;
   p.k_blocks_per_tap = Cg ? 1 : (Cin + 63) / 64;
   p.num_taps = ksize * ksize;
-  if (flat) {
-    if ((rc = encode_view(&p.a_maps[0], make_flat_view(x, d1, Cin), bx))) return rc;
-    for (int i = 1; i < 4; ++i) p.a_maps[i] = p.a_maps[0];
-    p.tap_map[0] = 0, p.tap_o1[0] = 0, p.tap_o2[0] = 0, p.tap_w[0] = 0;
-  } else if (stride == 1) {
-    if ((rc = encode_view(&p.a_maps[0], make_view(x, B, H, W, Cin, 1, 0, 0), bx))) return rc;
-    for (int i = 1; i < 4; ++i) p.a_maps[i] = p.a_maps[0];
-    for (int kh = 0; kh < ksize; ++kh)
-      for (int kw = 0; kw < ksize; ++kw) {
-        const int t = kh * ksize + kw;
-        p.tap_map[t] = 0;
-        p.tap_o1[t] = static_cast<int8_t>(kw - ksize / 2);
-        p.tap_o2[t] = static_cast<int8_t>(kh - ksize / 2);
-        p.tap_w[t] = static_cast<int8_t>(t);
-      }
-  } else {
-    // stride 2: tap (kh,kw) reads input row 2*oh + kh - pad -> phase ((kh-pad)&1), index oh + floor((kh-pad)/2)
-    B200_REQUIRE(H >= 2 && W >= 2, "conv2d_fwd: stride-2 needs H,W >= 2");
-    for (int ph = 0; ph < 2; ++ph)
-      for (int pw = 0; pw < 2; ++pw)
-        if ((rc = encode_view(&p.a_maps[ph * 2 + pw], make_view(x, B, H, W, Cin, 2, ph, pw), bx))) return rc;
-    const int pad = pad_of(ksize);
-    for (int kh = 0; kh < ksize; ++kh)
-      for (int kw = 0; kw < ksize; ++kw) {
-        const int t = kh * ksize + kw;
-        const int dh = kh - pad, dw = kw - pad;
-        const int ph = dh & 1, pw = dw & 1;
-        p.tap_map[t] = static_cast<int8_t>(ph * 2 + pw);
-        p.tap_o1[t] = static_cast<int8_t>((dw - pw) / 2);
-        p.tap_o2[t] = static_cast<int8_t>((dh - ph) / 2);
-        p.tap_w[t] = static_cast<int8_t>(t);
-      }
-  }
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(p.num_taps) * p.k_per_tap, static_cast<uint64_t>(Cout)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(p.num_taps) * p.k_per_tap};
-    uint32_t box[2] = {64, static_cast<uint32_t>(BN)};
-    if ((rc = encode_tmap_bf16(&p.b_map, w, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_taps(p, p.a_maps, x, B, H, W, Cin, ksize, stride, box_of(p)))) return rc;
+  for (int t = 0; t < p.num_taps; ++t) p.tap_w[t] = static_cast<int8_t>(t);
+  if ((rc = encode_matrix(&p.b_map, w, static_cast<long long>(p.num_taps) * p.k_per_tap, Cout, BN))) return rc;
   p.stats = stats;
   p.bias = bias;
   p.act = act;
   p.residual = residual;
-  p.rs1 = Cout;
-  p.rs2 = static_cast<long long>(d1) * Cout;
-  p.rs3 = static_cast<long long>(d1) * d2 * Cout;
+  p.rs1 = static_cast<long long>(dv.strides[1]);
+  p.rs2 = static_cast<long long>(dv.strides[2]);
+  p.rs3 = static_cast<long long>(dv.strides[3]);
   p.out_direct = out_f32;
   p.ld_out = ld_out;
-  if (g_fwd_bn_scale != nullptr) {
-    // b200_conv2d_fwd_set_bn: y = act(conv * scale[c] + shift[c] (+ residual)) - BatchNorm with fixed (running) statistics
-    // folded into the epilogue; the activation moves AFTER the residual add (conv_gemm.cuh kEpiAffine)
-    const float* sc = g_fwd_bn_scale;
-    const float* sh = g_fwd_bn_shift;
-    g_fwd_bn_scale = g_fwd_bn_shift = nullptr;
-    B200_REQUIRE(Cout % 64 == 0 && bias == nullptr && stats == nullptr && out_f32 == nullptr && act <= 1 && !g_conv_out_f32_tma,
-                 "conv2d_fwd + folded BN: Cout=%d must be a multiple of 64, no bias / statistics / fp32 output", Cout);
+  if (bn_scale != nullptr) {
     p.affine = 1;
-    p.colscale = sc;
-    p.bias = sh;
+    p.colscale = bn_scale;
+    p.bias = bn_shift;
   }
   return Cg ? launch_conv_gemm<64>(p, st) : dispatch_conv_gemm(p, Cout, st);
 }
 
 int b200_conv2d_fwd(const void* x, const void* w, void* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride,
                     float* stats, const float* bias, int act, const void* residual, float* out_f32, long long ld_out,
-                    void* stream) {
-  return conv_fwd(x, w, y, B, H, W, Cin, Cout, ksize, stride, stats, bias, act, residual, out_f32, ld_out, stream, 0);
+                    const float* bn_scale, const float* bn_shift, void* stream) {
+  return conv_fwd(x, w, y, B, H, W, Cin, Cout, ksize, stride, stats, bias, act, residual, out_f32, ld_out, bn_scale, bn_shift,
+                  0, 0, stream);
 }
 
-int b200_dgrad_set_bn_mask(const void* x_raw, const float* scale, const float* shift, float* stats) {
-  g_bnmask_x = x_raw, g_bnmask_scale = scale, g_bnmask_shift = shift, g_bnmask_stats = stats;
-  return OK;
-}
-
-int b200_conv2d_fwd_set_bn(const float* scale, const float* shift) {
-  g_fwd_bn_scale = scale;
-  g_fwd_bn_shift = shift;
-  return OK;
+int b200_conv2d_fwd_f32(const void* x, const void* w, float* y, int B, int H, int W, int Cin, int Cout, int ksize,
+                        int stride, const float* bias, void* stream) {
+  return conv_fwd(x, w, y, B, H, W, Cin, Cout, ksize, stride, nullptr, bias, 0, nullptr, nullptr, 0, nullptr, nullptr, 1, 0,
+                  stream);
 }
 
 // Cg > 0: grouped convolution of group width Cg (Cin == Cout, validated by the caller) in channel-window mode
 static int conv_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int Cin, int Cout, int ksize,
-                      int stride, const void* residual, void* stream, int Cg) {
+                      int stride, const void* residual, const b200_bn_mask_t* bn_mask, int Cg, void* stream) {
   B200_REQUIRE(ksize == 1 || ksize == 3 || (ksize == 2 && stride == 2), "conv2d_dgrad: ksize %d / stride %d unsupported", ksize, stride);
   B200_REQUIRE(stride == 1 || stride == 2, "conv2d_dgrad: stride %d unsupported", stride);
   B200_REQUIRE(Cin % 8 == 0 && Cout % 8 == 0, "conv2d_dgrad: Cin=%d / Cout=%d must be multiples of 8", Cin, Cout);
+  B200_REQUIRE(bn_mask == nullptr || (stride == 1 && Cin % 64 == 0 && bn_mask_complete(bn_mask)),
+               "conv2d_dgrad: the fused BatchNorm-backward reduce needs stride 1, Cin %% 64 == 0 and every bn_mask field "
+               "(Cin=%d, stride=%d)", Cin, stride);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int Ho = out_dim(H, ksize, stride), Wo = out_dim(W, ksize, stride);
-  const int taps = ksize * ksize;
+  const bool flat = (ksize == 1 && stride == 1);
   const int BN = Cg ? 64 : block_n_for(Cin);
   const int k_per_tap = Cg ? 64 : Cout;
   int rc;
   CUtensorMap b_map;
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(taps) * k_per_tap, static_cast<uint64_t>(Cin)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(taps) * k_per_tap};
-    uint32_t box[2] = {64, static_cast<uint32_t>(BN)};
-    if ((rc = encode_tmap_bf16(&b_map, wd, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_matrix(&b_map, wd, static_cast<long long>(ksize * ksize) * k_per_tap, Cin, BN))) return rc;
   const int nphase = (stride == 2 && ksize >= 2) ? 2 : 1;  // phases per spatial dim that need their own launch
-  const void* const bnmask_x = g_bnmask_x;
-  const float* const bnmask_scale = g_bnmask_scale;
-  const float* const bnmask_shift = g_bnmask_shift;
-  float* const bnmask_stats = g_bnmask_stats;
-  g_bnmask_x = nullptr;
-  B200_REQUIRE(bnmask_x == nullptr || (stride == 1 && Cin % 64 == 0 && bnmask_scale && bnmask_shift && bnmask_stats),
-               "conv2d_dgrad: the fused BatchNorm-backward reduce needs stride 1 and Cin %% 64 == 0 (Cin=%d, stride=%d)", Cin, stride);
   for (int ph = 0; ph < nphase; ++ph) {
     for (int pw = 0; pw < nphase; ++pw) {
       ConvGemmParams p;
       memset(&p, 0, sizeof(p));
       p.b_map = b_map;
-      const bool flat = (ksize == 1 && stride == 1);
       // output (dx) view for this launch
       View dv = flat ? make_flat_view(dx, static_cast<long long>(B) * H * W, Cin)
                      : make_view(dx, B, H, W, Cin, stride, ph, pw);
       if ((rc = setup_output(p, dv, Cin, 0, nullptr))) return rc;
-      const Box3 bx = box_of(p);
       p.n_tiles = (Cin + BN - 1) / BN;
       p.chan_window = Cg ? 1 : 0;
       p.k_per_tap = k_per_tap;
       p.k_blocks_per_tap = Cg ? 1 : (Cout + 63) / 64;
-      View av = flat ? make_flat_view(dy, static_cast<long long>(B) * H * W, Cout)
-                     : make_view(dy, B, Ho, Wo, Cout, 1, 0, 0);
-      if ((rc = encode_view(&p.a_maps[0], av, bx))) return rc;
+      if ((rc = encode_view(&p.a_maps[0], act_view(dy, B, Ho, Wo, Cout, flat), box_of(p)))) return rc;
       for (int i = 1; i < 4; ++i) p.a_maps[i] = p.a_maps[0];
       int nt = 0;
       if (ksize == 1) {
@@ -772,13 +711,7 @@ static int conv_dgrad(const void* dy, const void* wd, void* dx, int B, int H, in
         p.rs2 = static_cast<long long>(dv.strides[2]);
         p.rs3 = static_cast<long long>(dv.strides[3]);
       }
-      if (bnmask_x != nullptr) {
-        p.mask_in = static_cast<const __nv_bfloat16*>(bnmask_x);
-        p.ms1 = static_cast<long long>(dv.strides[1]);
-        p.ms2 = static_cast<long long>(dv.strides[2]);
-        p.ms3 = static_cast<long long>(dv.strides[3]);
-        p.bn_scale = bnmask_scale, p.bn_shift = bnmask_shift, p.stats = bnmask_stats;
-      }
+      if (bn_mask != nullptr) set_bn_mask(p, bn_mask, dv);
       if ((rc = Cg ? launch_conv_gemm<64>(p, st) : dispatch_conv_gemm(p, Cin, st))) return rc;
     }
   }
@@ -786,8 +719,8 @@ static int conv_dgrad(const void* dy, const void* wd, void* dx, int B, int H, in
 }
 
 int b200_conv2d_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int Cin, int Cout, int ksize,
-                      int stride, const void* residual, void* stream) {
-  return conv_dgrad(dy, wd, dx, B, H, W, Cin, Cout, ksize, stride, residual, stream, 0);
+                      int stride, const void* residual, const b200_bn_mask_t* bn_mask, void* stream) {
+  return conv_dgrad(dy, wd, dx, B, H, W, Cin, Cout, ksize, stride, residual, bn_mask, 0, stream);
 }
 
 int b200_gemm_ex(const b200_view_t* a, const b200_view_t* out, const b200_gemm_args_t* g, void* stream) {
@@ -822,13 +755,7 @@ int b200_gemm_ex(const b200_view_t* a, const b200_view_t* out, const b200_gemm_a
   p.num_taps = 1;
   p.k_per_tap = g->K;
   p.k_blocks_per_tap = (g->K + 63) / 64;
-  const int BN = block_n_for(g->N);
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(g->K), static_cast<uint64_t>(g->N)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(g->K)};
-    uint32_t box[2] = {64, static_cast<uint32_t>(BN)};
-    if ((rc = encode_tmap_bf16(&p.b_map, g->w, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_matrix(&p.b_map, g->w, g->K, g->N, block_n_for(g->N)))) return rc;
   p.stats = g->stats;
   p.bias = g->bias;
   p.colscale = g->colscale;
@@ -851,56 +778,28 @@ int b200_gemm_ex(const b200_view_t* a, const b200_view_t* out, const b200_gemm_a
   return dispatch_conv_gemm(p, g->N, static_cast<cudaStream_t>(stream));
 }
 
-int b200_conv2d_wgrad_set_rowscale(const float* rowscale) {
-  g_wgrad_rowscale = rowscale;
-  return OK;
-}
-
-int b200_conv2d_wgrad_set_bias_partial(float* bias_partial) {
-  g_wgrad_bias_partial = bias_partial;
-  return OK;
-}
-
-int b200_conv2d_wgrad_set_bias_out(float* bias_out) {
-  g_wgrad_bias_out = bias_out;
-  return OK;
-}
-
 int b200_conv2d_wgrad_splits(int B, int H, int W, int Cin, int Cout, int ksize, int stride) {
   return plan_wgrad(B, H, W, Cin, Cout, ksize, stride).splits;
 }
 
 size_t b200_conv2d_wgrad_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int stride) {
-  const WgradPlan pl = plan_wgrad(B, H, W, Cin, Cout, ksize, stride);
-  return static_cast<size_t>(pl.splits) * Cout * pl.taps * Cin * sizeof(float);
+  return wgrad_bytes(plan_wgrad(B, H, W, Cin, Cout, ksize, stride), Cout, Cin);
 }
 
 int b200_conv2d_wgrad(const void* dy, const void* x, float* dw, void* workspace, size_t workspace_bytes, int B, int H,
-                      int W, int Cin, int Cout, int ksize, int stride, int accumulate, void* stream) {
+                      int W, int Cin, int Cout, int ksize, int stride, int accumulate, float* bias_partial, float* bias_out,
+                      void* stream) {
   B200_REQUIRE(ksize == 1 || ksize == 3 || (ksize == 2 && stride == 2), "conv2d_wgrad: ksize %d / stride %d unsupported", ksize, stride);
   B200_REQUIRE(stride == 1 || stride == 2, "conv2d_wgrad: stride %d unsupported", stride);
   B200_REQUIRE(Cin % 8 == 0 && Cout % 8 == 0, "conv2d_wgrad: Cin=%d / Cout=%d must be multiples of 8", Cin, Cout);
+  B200_REQUIRE(bias_out == nullptr || bias_partial != nullptr, "conv2d_wgrad: bias_out needs bias_partial");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const WgradPlan pl = plan_wgrad(B, H, W, Cin, Cout, ksize, stride);
-  const size_t need = static_cast<size_t>(pl.splits) * Cout * pl.taps * Cin * sizeof(float);
+  const size_t need = wgrad_bytes(pl, Cout, Cin);
   B200_REQUIRE(workspace != nullptr && workspace_bytes >= need, "conv2d_wgrad: workspace too small (%zu < %zu)",
                workspace_bytes, need);
-  WgradParams p;
-  memset(&p, 0, sizeof(p));
-  p.num_taps = pl.merge_atoms ? 1 : pl.taps;
-  p.merge_atoms = pl.merge_atoms;
-  p.n_cols = pl.merge_atoms ? pl.taps * Cin : Cin;
-  p.Cout = Cout, p.Cin = Cin;
-  p.mg_tiles = pl.mg_tiles, p.ng_tiles = pl.ng_tiles;
-  p.tiles1 = pl.tiles1, p.tiles2 = pl.tiles2, p.tiles3 = pl.tiles3;
-  p.box1 = pl.box.b1, p.box2 = pl.box.b2, p.box3 = pl.box.b3;
-  p.splits = pl.splits, p.kb_per_split = pl.kb_per_split, p.kb_total = pl.kb_total;
-  p.ld_partial = static_cast<long long>(pl.taps) * Cin;
-  p.partial = static_cast<float*>(workspace);
-  p.bias_partial = g_wgrad_bias_partial;   // one-shot (b200_conv2d_wgrad_set_bias_partial)
-  g_wgrad_bias_partial = nullptr;
-  float* const bias_out = p.bias_partial != nullptr ? g_wgrad_bias_out : nullptr;
-  g_wgrad_bias_out = nullptr;
+  WgradParams p = wgrad_params(pl, Cout, Cin, workspace);
+  p.bias_partial = bias_partial;
   int rc;
   if ((rc = setup_wgrad_maps(p, pl, dy, x, B, H, W, Cin, Cout, ksize, stride))) return rc;
   if (pl.block_ng == 64)
@@ -912,10 +811,7 @@ int b200_conv2d_wgrad(const void* dy, const void* x, float* dw, void* workspace,
   else
     rc = launch_wgrad<256>(p, st);
   if (rc) return rc;
-  if ((rc = launch_wgrad_reduce(p.partial, dw, pl.splits, Cout, Cin, pl.taps, accumulate, g_wgrad_rowscale, st, p.bias_partial,
-                                bias_out)))
-    return rc;
-  g_wgrad_rowscale = nullptr;
+  if ((rc = launch_wgrad_reduce(p.partial, dw, pl.splits, Cout, Cin, pl.taps, accumulate, st, bias_partial, bias_out))) return rc;
   B200_LAUNCHED();
   return OK;
 }
@@ -937,19 +833,13 @@ int b200_stem_s2d_conv_fwd(const void* z, const void* w, void* y, float* stats, 
   for (int ky = 0; ky < 4; ++ky) {
     p.tap_map[ky] = 0, p.tap_o1[ky] = 0, p.tap_o2[ky] = static_cast<int8_t>(ky), p.tap_w[ky] = static_cast<int8_t>(ky);
   }
-  {
-    uint64_t dims[2] = {256, static_cast<uint64_t>(Cout)};
-    uint64_t strides[2] = {1, 256};
-    uint32_t box[2] = {64, 64};
-    if ((rc = encode_tmap_bf16(&p.b_map, w, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_matrix(&p.b_map, w, 256, Cout, 64))) return rc;
   p.stats = stats;
   return dispatch_conv_gemm(p, Cout, st);
 }
 
 size_t b200_stem_s2d_conv_wgrad_workspace_bytes(int B, int Ho, int Wo) {
-  const WgradPlan pl = plan_wgrad_geom(Wo, Ho, B, 64, 64, 4);
-  return static_cast<size_t>(pl.splits) * 64 * 4 * 64 * sizeof(float);
+  return wgrad_bytes(plan_wgrad_geom(Wo, Ho, B, 64, 64, 4), 64, 64);
 }
 
 int b200_stem_s2d_conv_wgrad(const void* dy, const void* z, float* g, void* workspace, size_t workspace_bytes, int B, int Ho,
@@ -957,21 +847,10 @@ int b200_stem_s2d_conv_wgrad(const void* dy, const void* z, float* g, void* work
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int Cout = 64, Cin = 64, taps = 4;
   const WgradPlan pl = plan_wgrad_geom(Wo, Ho, B, Cin, Cout, taps);
-  const size_t need = static_cast<size_t>(pl.splits) * Cout * taps * Cin * sizeof(float);
+  const size_t need = wgrad_bytes(pl, Cout, Cin);
   B200_REQUIRE(workspace != nullptr && workspace_bytes >= need, "stem_s2d_conv_wgrad: workspace too small (%zu < %zu)",
                workspace_bytes, need);
-  WgradParams p;
-  memset(&p, 0, sizeof(p));
-  p.num_taps = pl.merge_atoms ? 1 : taps;
-  p.merge_atoms = pl.merge_atoms;
-  p.n_cols = pl.merge_atoms ? taps * Cin : Cin;
-  p.Cout = Cout, p.Cin = Cin;
-  p.mg_tiles = pl.mg_tiles, p.ng_tiles = pl.ng_tiles;
-  p.tiles1 = pl.tiles1, p.tiles2 = pl.tiles2, p.tiles3 = pl.tiles3;
-  p.box1 = pl.box.b1, p.box2 = pl.box.b2, p.box3 = pl.box.b3;
-  p.splits = pl.splits, p.kb_per_split = pl.kb_per_split, p.kb_total = pl.kb_total;
-  p.ld_partial = static_cast<long long>(taps) * Cin;
-  p.partial = static_cast<float*>(workspace);
+  WgradParams p = wgrad_params(pl, Cout, Cin, workspace);
   int rc;
   if ((rc = encode_view(&p.dy_map, make_view(dy, B, Ho, Wo, Cout, 1, 0, 0), pl.box))) return rc;
   if ((rc = encode_view(&p.x_maps[0], stem_s2d_view(z, B, Ho, Wo), pl.box))) return rc;
@@ -979,7 +858,7 @@ int b200_stem_s2d_conv_wgrad(const void* dy, const void* z, float* g, void* work
   for (int ky = 0; ky < 4; ++ky) p.tap_map[ky] = 0, p.tap_o1[ky] = 0, p.tap_o2[ky] = static_cast<int8_t>(ky);
   if ((rc = launch_wgrad<256>(p, st))) return rc;  // merged-tap mode: the four y-taps are the four 64-column atoms
   // g[cout][k64][ky] (the generic "OIHW" layout of a 64-channel, 4-tap conv); b200_stem_s2d_wgrad_relayout maps it to [64,3,7,7]
-  if ((rc = launch_wgrad_reduce(p.partial, g, pl.splits, Cout, Cin, taps, 0, nullptr, st))) return rc;
+  if ((rc = launch_wgrad_reduce(p.partial, g, pl.splits, Cout, Cin, taps, 0, st))) return rc;
   B200_LAUNCHED();
   return OK;
 }
@@ -1006,12 +885,7 @@ int b200_conv1x1_bn_act_fwd(const void* x, const void* w, const float* scale, co
   p.num_taps = 1;
   if ((rc = encode_view(&p.a_maps[0], make_flat_view(x, pixels, Cin), bx))) return rc;
   for (int i = 1; i < 4; ++i) p.a_maps[i] = p.a_maps[0];
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(Cin), static_cast<uint64_t>(Cout)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(Cin)};
-    uint32_t box[2] = {64, static_cast<uint32_t>(block_n_for(Cout))};
-    if ((rc = encode_tmap_bf16(&p.b_map, w, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_matrix(&p.b_map, w, Cin, Cout, block_n_for(Cout)))) return rc;
   p.affine = 1;
   p.colscale = scale;
   p.bias = shift;
@@ -1030,8 +904,8 @@ int b200_conv1x1_bn_fwd(const void* x, const void* w, const float* scale, const 
   if (stream_ok(pixels, Cin, Cout))
     return run_stream(kStreamAffine, x, w, y, nullptr, nullptr, scale, shift, nullptr, pixels, Cin, Cout,
                       static_cast<cudaStream_t>(stream));
-  b200_conv2d_fwd_set_bn(scale, shift);
-  return b200_conv2d_fwd(x, w, y, 1, 1, static_cast<int>(pixels), Cin, Cout, 1, 1, nullptr, nullptr, 0, nullptr, nullptr, 0, stream);
+  return conv_fwd(x, w, y, 1, 1, static_cast<int>(pixels), Cin, Cout, 1, 1, nullptr, nullptr, 0, nullptr, nullptr, 0, scale,
+                  shift, 0, 0, stream);
 }
 
 int b200_conv1x1_dgrad_masked_stats_rows(long long pixels, int Cin, int Cout) {
@@ -1059,12 +933,7 @@ int b200_conv1x1_dgrad_masked(const void* dy, const void* wd, void* dx, long lon
   p.num_taps = 1;
   if ((rc = encode_view(&p.a_maps[0], make_flat_view(dy, pixels, Cout), bx))) return rc;
   for (int i = 1; i < 4; ++i) p.a_maps[i] = p.a_maps[0];
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(Cout), static_cast<uint64_t>(Cin)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(Cout)};
-    uint32_t box[2] = {64, static_cast<uint32_t>(block_n_for(Cin))};
-    if ((rc = encode_tmap_bf16(&p.b_map, wd, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_matrix(&p.b_map, wd, Cout, Cin, block_n_for(Cin)))) return rc;
   p.residual = residual;
   p.rs1 = static_cast<long long>(dv.strides[1]);
   p.rs2 = static_cast<long long>(dv.strides[2]);
@@ -1076,8 +945,10 @@ int b200_conv1x1_dgrad_masked(const void* dy, const void* wd, void* dx, long lon
 }
 
 int b200_gemm_dual(const void* a0, int K0, const void* a1, int K1, const void* wcat, const float* bias, void* out,
-                   long long pixels, int N, void* stream) {
+                   long long pixels, int N, const b200_bn_mask_t* bn_mask, void* stream) {
   B200_REQUIRE(pixels > 0 && K0 % 64 == 0 && K1 % 64 == 0 && N % 8 == 0, "gemm_dual: K0=%d / K1=%d must be multiples of 64", K0, K1);
+  B200_REQUIRE(bn_mask == nullptr || (N % 64 == 0 && bn_mask_complete(bn_mask)),
+               "gemm_dual: fused BN-backward reduce needs N %% 64 == 0 and every bn_mask field (N=%d)", N);
   ConvGemmParams p;
   memset(&p, 0, sizeof(p));
   int rc;
@@ -1095,22 +966,9 @@ int b200_gemm_dual(const void* a0, int K0, const void* a1, int K1, const void* w
   p.tap_kb[0] = static_cast<int16_t>(K0 / 64), p.tap_kb[1] = static_cast<int16_t>(K1 / 64);
   p.tap_k0[0] = 0, p.tap_k0[1] = K0;
   p.kb_total = (K0 + K1) / 64;
-  {
-    uint64_t dims[2] = {static_cast<uint64_t>(K0 + K1), static_cast<uint64_t>(N)};
-    uint64_t strides[2] = {1, static_cast<uint64_t>(K0 + K1)};
-    uint32_t box[2] = {64, static_cast<uint32_t>(block_n_for(N))};
-    if ((rc = encode_tmap_bf16(&p.b_map, wcat, 2, dims, strides, box))) return rc;
-  }
+  if ((rc = encode_matrix(&p.b_map, wcat, K0 + K1, N, block_n_for(N)))) return rc;
   p.bias = bias;
-  if (g_bnmask_x != nullptr) {
-    B200_REQUIRE(N % 64 == 0 && g_bnmask_scale && g_bnmask_shift && g_bnmask_stats, "gemm_dual: fused BN-backward reduce needs N %% 64 == 0 (N=%d)", N);
-    p.mask_in = static_cast<const __nv_bfloat16*>(g_bnmask_x);
-    p.ms1 = static_cast<long long>(dv.strides[1]);
-    p.ms2 = static_cast<long long>(dv.strides[2]);
-    p.ms3 = static_cast<long long>(dv.strides[3]);
-    p.bn_scale = g_bnmask_scale, p.bn_shift = g_bnmask_shift, p.stats = g_bnmask_stats;
-    g_bnmask_x = nullptr;
-  }
+  if (bn_mask != nullptr) set_bn_mask(p, bn_mask, dv);
   return dispatch_conv_gemm(p, N, static_cast<cudaStream_t>(stream));
 }
 
@@ -1137,27 +995,24 @@ int b200_conv2d_grouped_fwd_stats_rows(int B, int H, int W, int C, int groups, i
 }
 
 int b200_conv2d_grouped_fwd(const void* x, const void* w, void* y, int B, int H, int W, int C, int groups, int ksize,
-                            int stride, float* stats, int act, void* stream) {
+                            int stride, float* stats, int act, const float* bn_scale, const float* bn_shift, void* stream) {
   int rc;
   if ((rc = grouped_check("conv2d_grouped_fwd", C, groups, ksize, stride))) return rc;
   B200_REQUIRE(act == 0 || act == 1, "conv2d_grouped_fwd: act %d unsupported (none or relu)", act);
-  return conv_fwd(x, w, y, B, H, W, C, C, ksize, stride, stats, nullptr, act, nullptr, nullptr, 0, stream, C / groups);
+  return conv_fwd(x, w, y, B, H, W, C, C, ksize, stride, stats, nullptr, act, nullptr, nullptr, 0, bn_scale, bn_shift, 0,
+                  C / groups, stream);
 }
 
 int b200_conv2d_grouped_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int C, int groups, int ksize,
-                              int stride, void* stream) {
+                              int stride, const b200_bn_mask_t* bn_mask, void* stream) {
   int rc;
   if ((rc = grouped_check("conv2d_grouped_dgrad", C, groups, ksize, stride))) return rc;
-  return conv_dgrad(dy, wd, dx, B, H, W, C, C, ksize, stride, nullptr, stream, C / groups);
-}
-
-static size_t grouped_wgrad_bytes(const WgradPlan& pl, int C) {
-  return static_cast<size_t>(pl.splits) * C * pl.taps * 64 * sizeof(float);
+  return conv_dgrad(dy, wd, dx, B, H, W, C, C, ksize, stride, nullptr, bn_mask, C / groups, stream);
 }
 
 size_t b200_conv2d_grouped_wgrad_workspace_bytes(int B, int H, int W, int C, int groups, int ksize, int stride) {
   if (grouped_check("conv2d_grouped_wgrad_workspace_bytes", C, groups, ksize, stride)) return 0;
-  return grouped_wgrad_bytes(plan_wgrad(B, H, W, 64, C, ksize, stride, true), C);
+  return wgrad_bytes(plan_wgrad(B, H, W, 64, C, ksize, stride, true), C, 64);
 }
 
 int b200_conv2d_grouped_wgrad(const void* dy, const void* x, float* dw, void* workspace, size_t workspace_bytes, int B,
@@ -1166,20 +1021,12 @@ int b200_conv2d_grouped_wgrad(const void* dy, const void* x, float* dw, void* wo
   if ((rc = grouped_check("conv2d_grouped_wgrad", C, groups, ksize, stride))) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const WgradPlan pl = plan_wgrad(B, H, W, 64, C, ksize, stride, true);
-  const size_t need = grouped_wgrad_bytes(pl, C);
+  const size_t need = wgrad_bytes(pl, C, 64);
   B200_REQUIRE(workspace != nullptr && workspace_bytes >= need, "conv2d_grouped_wgrad: workspace too small (%zu < %zu)",
                workspace_bytes, need);
-  WgradParams p;
-  memset(&p, 0, sizeof(p));
+  WgradParams p = wgrad_params(pl, C, 64, workspace);
   p.num_taps = pl.taps / 3;   // work items of three taps each
-  p.n_cols = 3 * 64;
-  p.Cout = C, p.Cin = 3 * 64;
-  p.mg_tiles = pl.mg_tiles, p.ng_tiles = 1;
-  p.tiles1 = pl.tiles1, p.tiles2 = pl.tiles2, p.tiles3 = pl.tiles3;
-  p.box1 = pl.box.b1, p.box2 = pl.box.b2, p.box3 = pl.box.b3;
-  p.splits = pl.splits, p.kb_per_split = pl.kb_per_split, p.kb_total = pl.kb_total;
-  p.ld_partial = static_cast<long long>(pl.taps) * 64;
-  p.partial = static_cast<float*>(workspace);
+  p.n_cols = p.Cin = 3 * 64;
   if ((rc = setup_wgrad_maps(p, pl, dy, x, B, H, W, C, C, ksize, stride))) return rc;
   if ((rc = launch_wgrad<384, true>(p, st))) return rc;
   const long long total = static_cast<long long>(C) * (C / groups) * pl.taps;

@@ -42,7 +42,7 @@ BnBwdPlan plan_bn_bwd(long long rows, int C) {
 extern "C" {
 
 const char* b200_last_error(void) { return get_error(); }
-int b200_abi_version(void) { return 1; }
+int b200_abi_version(void) { return 2; }
 int b200_sm_count(void) { return device_sm_count(); }
 unsigned long long b200_launch_count(void) { return g_launch_count; }
 

@@ -265,8 +265,7 @@ __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __gr
 // out tap-innermost, so that both the partial reads and the OIHW gradient writes are fully coalesced. Fixed summation order.
 __global__ void __launch_bounds__(256) wgrad_reduce_rows_kernel(const float* __restrict__ partial, float* __restrict__ grad,
                                                                 int splits, int Cout, int Cin, int taps, int chunk, int SL,
-                                                                int accumulate, const float* __restrict__ rowscale,
-                                                                const float* __restrict__ bias_partial,
+                                                                int accumulate, const float* __restrict__ bias_partial,
                                                                 float* __restrict__ bias_out) {
   pdl_launch_dependents();
   pdl_wait();
@@ -308,22 +307,20 @@ __global__ void __launch_bounds__(256) wgrad_reduce_rows_kernel(const float* __r
   }
   __syncthreads();
   const float* sm = reinterpret_cast<const float*>(rows_sm4);
-  const float rs = rowscale != nullptr ? __ldg(rowscale + cout) : 1.f;
   float* out = grad + (static_cast<long long>(cout) * Cin + c0) * taps;
   for (int e = threadIdx.x; e < cw * taps; e += blockDim.x) {
     const int cin = e / taps;
     const int tap = e - cin * taps;
     float s = 0.f;
     for (int sl = 0; sl < SL; ++sl) s += sm[(sl * nvec) * 4 + tap * cw + cin];
-    s *= rs;
     out[e] = accumulate ? out[e] + s : s;
   }
 }
 
 // Same reduction, one thread per element walking the splits: fallback for shapes the row kernel does not take.
 __global__ void wgrad_reduce_flat_kernel(const float* __restrict__ partial, float* __restrict__ grad, int splits, int Cout,
-                                    int Cin, int taps, int accumulate, const float* __restrict__ rowscale,
-                                    const float* __restrict__ bias_partial, float* __restrict__ bias_out) {
+                                    int Cin, int taps, int accumulate, const float* __restrict__ bias_partial,
+                                    float* __restrict__ bias_out) {
   pdl_launch_dependents();
   pdl_wait();
   const long long total = static_cast<long long>(Cout) * Cin * taps;
@@ -344,7 +341,6 @@ __global__ void wgrad_reduce_flat_kernel(const float* __restrict__ partial, floa
     const int cout = static_cast<int>(t / taps);
     float s = 0.f;
     for (int k = 0; k < splits; ++k) s += partial[k * slice + i];
-    if (rowscale != nullptr) s *= __ldg(rowscale + cout);
     const long long o = (static_cast<long long>(cout) * Cin + cin) * taps + tap;
     grad[o] = accumulate ? grad[o] + s : s;
   }

@@ -140,7 +140,7 @@ def im2col_nchw(x, KH, KW, stride, pad, ldk):
 
 
 # --------------------------------------------------------------------------------------------------------- conv / linear
-def _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, want_stats, act, groups):
+def _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, want_stats, act, groups, bn_scale=None, bn_shift=None):
     B, H, W, C = x.shape
     Ho, Wo = out_hw(H, ksize, stride), out_hw(W, ksize, stride)
     stats = None
@@ -150,7 +150,8 @@ def _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, want_stats, act, groups
         stats = torch.empty(T, 2, C, dtype=F32, device=x.device)
     y = torch.empty(B, Ho, Wo, C, dtype=BF16, device=x.device)
     sp = _span("conv_gemm_grouped_fwd", 2.0 * B * Ho * Wo * C * (C // groups) * ksize * ksize, _nb(x, w_packed, y))
-    rc = lib.b200_conv2d_grouped_fwd(_p(x), _p(w_packed), _p(y), B, H, W, C, groups, ksize, stride, _p(stats), act, _stream())
+    rc = lib.b200_conv2d_grouped_fwd(_p(x), _p(w_packed), _p(y), B, H, W, C, groups, ksize, stride, _p(stats), act,
+                                     _p(bn_scale), _p(bn_shift), _stream())
     _lib.check(rc, "b200_conv2d_grouped_fwd")
     if sp:
         sp.end()
@@ -177,11 +178,11 @@ def conv2d_fwd(x, w_packed, ksize=1, stride=1, want_stats=False, bias=None, act=
     if out_f32:
         y = torch.empty(B, Ho, Wo, Cout, dtype=F32, device=x.device)
         rc = lib.b200_conv2d_fwd(_p(x), _p(w_packed), None, B, H, W, Cin, Cout, ksize, stride, _p(stats), _p(bias), act,
-                                 _p(residual), _p(y), Cout, _stream())
+                                 _p(residual), _p(y), Cout, None, None, _stream())
     else:
         y = torch.empty(B, Ho, Wo, Cout, dtype=BF16, device=x.device)
         rc = lib.b200_conv2d_fwd(_p(x), _p(w_packed), _p(y), B, H, W, Cin, Cout, ksize, stride, _p(stats), _p(bias), act,
-                                 _p(residual), None, 0, _stream())
+                                 _p(residual), None, 0, None, None, _stream())
     _lib.check(rc, "b200_conv2d_fwd")
     if sp:
         sp.nbytes = _nb(x, w_packed, y, residual)
@@ -197,24 +198,25 @@ def conv2d_bn_act(x, w_packed, co, ksize=1, stride=1, relu=True, residual=None, 
     if groups != 1:
         if residual is not None:
             raise ValueError("conv2d_bn_act: a grouped convolution takes no residual")
-        lib.b200_conv2d_fwd_set_bn(_p(co.scale), _p(co.shift))
-        return _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, False, 1 if relu else 0, groups)[0]
+        return _conv2d_grouped_fwd(lib, x, w_packed, ksize, stride, False, 1 if relu else 0, groups, co.scale, co.shift)[0]
     B, H, W, Cin = x.shape
     Cout = w_packed.shape[0]
     Ho, Wo = out_hw(H, ksize, stride), out_hw(W, ksize, stride)
     y = torch.empty(B, Ho, Wo, Cout, dtype=BF16, device=x.device)
     sp = _span("conv_gemm_fwd", 2.0 * B * Ho * Wo * Cout * Cin * ksize * ksize, _nb(x, w_packed, y, residual))
-    lib.b200_conv2d_fwd_set_bn(_p(co.scale), _p(co.shift))
     rc = lib.b200_conv2d_fwd(_p(x), _p(w_packed), _p(y), B, H, W, Cin, Cout, ksize, stride, None, None, 1 if relu else 0,
-                             _p(residual), None, 0, _stream())
+                             _p(residual), None, 0, _p(co.scale), _p(co.shift), _stream())
     _lib.check(rc, "b200_conv2d_fwd")
     if sp:
         sp.end()
     return y
 
 
-def _arm_bn_mask(lib, bn_mask, B, H, W, C, ksize, groups=1):
-    """One-shot: the next dgrad / dual GEMM masks its output with relu'(bn(x_raw)) and writes the BN-backward partial sums."""
+def _bn_mask_arg(lib, bn_mask, B, H, W, C, ksize, groups=1):
+    """(BnMask, stats) for a dgrad / dual GEMM that masks its output with relu'(bn(x_raw)) and writes the BN-backward partial
+    sums into stats; (None, None) without bn_mask."""
+    if bn_mask is None:
+        return None, None
     x_raw, co = bn_mask
     assert x_raw.dtype == BF16 and x_raw.is_contiguous() and x_raw.shape[-1] == C and C % 64 == 0
     if groups != 1:   # (the grouped kernel runs 64-channel tiles: its own row count)
@@ -223,8 +225,7 @@ def _arm_bn_mask(lib, bn_mask, B, H, W, C, ksize, groups=1):
     else:
         rows = lib.b200_conv2d_fwd_stats_rows(B, H, W, C, ksize, 1)
     stats = torch.empty(rows, 2, C, dtype=F32, device=x_raw.device)
-    _lib.check(lib.b200_dgrad_set_bn_mask(_p(x_raw), _p(co.scale), _p(co.shift), _p(stats)), "b200_dgrad_set_bn_mask")
-    return stats
+    return _lib.BnMask(_p(x_raw), _p(co.scale), _p(co.shift), _p(stats)), stats
 
 
 def conv2d_dgrad(dy, wd_packed, in_hw, ksize=1, stride=1, residual=None, out=None, bn_mask=None, groups=1):
@@ -241,13 +242,11 @@ def conv2d_dgrad(dy, wd_packed, in_hw, ksize=1, stride=1, residual=None, out=Non
         if residual is not None or out is not None:
             raise ValueError("conv2d_dgrad: a grouped convolution takes no residual or out")
         dx = torch.empty(B, H, W, Cin, dtype=BF16, device=dy.device)
-        stats = None
-        if bn_mask is not None:
-            assert stride == 1, "bn_mask needs a stride-1 convolution"
-            stats = _arm_bn_mask(lib, bn_mask, B, H, W, Cin, ksize, groups)
+        assert bn_mask is None or stride == 1, "bn_mask needs a stride-1 convolution"
+        mask, stats = _bn_mask_arg(lib, bn_mask, B, H, W, Cin, ksize, groups)
         sp = _span("conv_gemm_grouped_dgrad", 2.0 * B * Ho * Wo * Cout * (Cin // groups) * ksize * ksize,
                    _nb(dy, wd_packed, dx, bn_mask[0] if bn_mask else None))
-        rc = lib.b200_conv2d_grouped_dgrad(_p(dy), _p(wd_packed), _p(dx), B, H, W, Cin, groups, ksize, stride, _stream())
+        rc = lib.b200_conv2d_grouped_dgrad(_p(dy), _p(wd_packed), _p(dx), B, H, W, Cin, groups, ksize, stride, mask, _stream())
         _lib.check(rc, "b200_conv2d_grouped_dgrad")
         if sp:
             sp.end()
@@ -260,13 +259,12 @@ def conv2d_dgrad(dy, wd_packed, in_hw, ksize=1, stride=1, residual=None, out=Non
         dx = torch.zeros(B, H, W, Cin, dtype=BF16, device=dy.device)
     else:
         dx = torch.empty(B, H, W, Cin, dtype=BF16, device=dy.device)
-    stats = None
-    if bn_mask is not None:
-        assert stride == 1, "bn_mask needs a stride-1 convolution"
-        stats = _arm_bn_mask(lib, bn_mask, B, H, W, Cin, ksize)
+    assert bn_mask is None or stride == 1, "bn_mask needs a stride-1 convolution"
+    mask, stats = _bn_mask_arg(lib, bn_mask, B, H, W, Cin, ksize)
     sp = _span("conv_gemm_dgrad", 2.0 * B * Ho * Wo * Cout * Cin * ksize * ksize,
                _nb(dy, wd_packed, dx, residual, bn_mask[0] if bn_mask else None))
-    rc = lib.b200_conv2d_dgrad(_p(dy), _p(wd_packed), _p(dx), B, H, W, Cin, Cout, ksize, stride, _p(residual), _stream())
+    rc = lib.b200_conv2d_dgrad(_p(dy), _p(wd_packed), _p(dx), B, H, W, Cin, Cout, ksize, stride, _p(residual), mask,
+                               _stream())
     _lib.check(rc, "b200_conv2d_dgrad")
     if sp:
         sp.end()
@@ -285,8 +283,8 @@ def _workspace(nbytes, device):
     return ws
 
 
-def conv2d_wgrad(dy, x, ksize=1, stride=1, out=None, accumulate=False, rowscale=None, bias_out=None, groups=1):
-    """dw fp32 OIHW [Cout, Cin, k, k] = sum over pixels of dy (x) x  (row `cout` optionally scaled by rowscale[cout]).
+def conv2d_wgrad(dy, x, ksize=1, stride=1, out=None, accumulate=False, bias_out=None, groups=1):
+    """dw fp32 OIHW [Cout, Cin, k, k] = sum over pixels of dy (x) x.
     bias_out (fp32 [Cout]): also write the bias gradient (column sums of dy), summed from the dy tiles the kernel already
     holds in shared memory - no extra pass over dy.  groups > 1: grouped 3x3 convolution, dw [C, C/groups, k, k]."""
     lib = _lib.load()
@@ -295,8 +293,8 @@ def conv2d_wgrad(dy, x, ksize=1, stride=1, out=None, accumulate=False, rowscale=
     B, H, W, Cin = x.shape
     Cout = dy.shape[-1]
     if groups != 1:
-        if rowscale is not None or bias_out is not None:
-            raise ValueError("conv2d_wgrad: a grouped convolution takes no rowscale or bias gradient")
+        if bias_out is not None:
+            raise ValueError("conv2d_wgrad: a grouped convolution takes no bias gradient")
         nbytes = lib.b200_conv2d_grouped_wgrad_workspace_bytes(B, H, W, Cin, groups, ksize, stride)
         if nbytes == 0:
             raise RuntimeError(f"b200_conv2d_grouped_wgrad_workspace_bytes failed: {_lib.last_error()}")
@@ -317,16 +315,12 @@ def conv2d_wgrad(dy, x, ksize=1, stride=1, out=None, accumulate=False, rowscale=
         out = torch.empty(Cout, Cin, ksize, ksize, dtype=F32, device=x.device)
         accumulate = False
     sp = _span("wgrad_gemm", 2.0 * dy.numel() * Cin * ksize * ksize, _nb(dy, x, out))
-    if rowscale is not None:
-        lib.b200_conv2d_wgrad_set_rowscale(_p(rowscale))
     bias_partial = None
-    if bias_out is not None:
+    if bias_out is not None:   # finished by the split-reduction kernel of the same call
         splits = lib.b200_conv2d_wgrad_splits(B, H, W, Cin, Cout, ksize, stride)
         bias_partial = torch.empty(splits, 2, Cout, dtype=F32, device=x.device)
-        lib.b200_conv2d_wgrad_set_bias_partial(_p(bias_partial))
-        lib.b200_conv2d_wgrad_set_bias_out(_p(bias_out))   # finished by the split-reduction kernel of the same call
     rc = lib.b200_conv2d_wgrad(_p(dy), _p(x), _p(out), _p(ws), ws.numel(), B, H, W, Cin, Cout, ksize, stride,
-                               1 if accumulate else 0, _stream())
+                               1 if accumulate else 0, _p(bias_partial), _p(bias_out), _stream())
     _lib.check(rc, "b200_conv2d_wgrad")
     if sp:
         sp.end()
@@ -643,9 +637,9 @@ def gemm_dual(a0, a1, wcat, bias, bn_mask=None):
     N = wcat.shape[0]
     pixels = a0.numel() // K0
     out = torch.empty(*a0.shape[:-1], N, dtype=BF16, device=a0.device)
-    stats = _arm_bn_mask(lib, bn_mask, 1, 1, pixels, N, 1) if bn_mask is not None else None
+    mask, stats = _bn_mask_arg(lib, bn_mask, 1, 1, pixels, N, 1)
     sp = _span("conv_gemm_dgrad", 2.0 * pixels * N * (K0 + K1), _nb(a0, a1, wcat, out, bn_mask[0] if bn_mask else None))
-    rc = lib.b200_gemm_dual(_p(a0), K0, _p(a1), K1, _p(wcat), _p(bias), _p(out), pixels, N, _stream())
+    rc = lib.b200_gemm_dual(_p(a0), K0, _p(a1), K1, _p(wcat), _p(bias), _p(out), pixels, N, mask, _stream())
     _lib.check(rc, "b200_gemm_dual")
     if sp:
         sp.end()

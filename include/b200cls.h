@@ -48,23 +48,30 @@ unsigned long long b200_launch_count(void);
  *            per (persistent CTA group, 32-row quadrant) - a few hundred rows; feed them to b200_bn_finalize
  *   residual optional bf16, same shape as y, added after bias/act
  *   out_f32  optional fp32 [B*Ho*Wo][ld_out] - when given the result is written there instead of y (ksize 1 only)
+ *   bn_scale, bn_shift  both NULL, or both set: fold BatchNorm with FIXED statistics into the epilogue,
+ *            y = act(conv(x) * scale[c] + shift[c] (+ residual)) with act (0 / B200_ACT_RELU) applied after the residual
+ *            add - the eval-mode forward of conv -> bn -> (+identity) -> relu (classification/resnet/models/networks.py:104-124,
+ *            utils.py:61-83 `evaluate`) without any BatchNorm pass. scale / shift from b200_bn_eval_coeffs; Cout % 64 == 0,
+ *            no bias, stats or out_f32.
  * replaces nn.Conv2d.forward / nn.Linear.forward: classification/resnet/models/networks.py:107,111,115,119,218;
  * classification/vision_transformer/vit_model.py:66,95,109,129,132. A linear layer is the case H=W=1, B=rows. */
 int b200_conv2d_fwd(const void* x, const void* w, void* y, int B, int H, int W, int Cin, int Cout, int ksize, int stride,
                     float* stats, const float* bias, int act, const void* residual, float* out_f32, long long ld_out,
-                    void* stream);
+                    const float* bn_scale, const float* bn_shift, void* stream);
 int b200_conv2d_fwd_stats_rows(int B, int H, int W, int Cout, int ksize, int stride);
-/* one-shot (this thread, next b200_conv2d_fwd call): fold BatchNorm with FIXED statistics into the epilogue,
- * y = act(conv(x) * scale[c] + shift[c] (+ residual)) with act (0 / B200_ACT_RELU) applied after the residual add - the
- * eval-mode forward of conv -> bn -> (+identity) -> relu (classification/resnet/models/networks.py:104-124, utils.py:61-83
- * `evaluate`) without any BatchNorm pass.  scale / shift from b200_bn_eval_coeffs; Cout % 64 == 0. */
-int b200_conv2d_fwd_set_bn(const float* scale, const float* shift);
-/* one-shot (this thread, next b200_conv2d_dgrad with stride 1 or b200_gemm_dual): the output is the gradient of
- * relu(bn(x_raw)) - the kernel zeroes it where x_raw * scale + shift <= 0 (dz) and writes the per-CTA partial rows
- * stats[rows][2][C] = sum(dz), sum(dz * x_raw), rows = b200_conv2d_fwd_stats_rows(B, H, W, C, ksize, 1) of the dx geometry:
- * the reduce half of F.batch_norm's backward (classification/resnet/models/networks.py:108,112 bn1 / bn2 under loss.backward(),
- * utils.py:33) without a pass over the gradient.  Feed the rows to b200_bn_bwd_finalize, then b200_bn_bwd_apply(src_is_dz=1). */
-int b200_dgrad_set_bn_mask(const void* x_raw, const float* scale, const float* shift, float* stats);
+/* Fused BatchNorm-backward mask of a dgrad GEMM (b200_conv2d_dgrad at stride 1, b200_conv2d_grouped_dgrad at stride 1,
+ * b200_gemm_dual; NULL = off): the output is the gradient of relu(bn(x_raw)) - the kernel zeroes it where
+ * x_raw * scale + shift <= 0 (dz) and writes the per-CTA partial rows stats[rows][2][C] = sum(dz), sum(dz * x_raw),
+ * rows = b200_conv2d_fwd_stats_rows(B, H, W, C, ksize, 1) of the dx geometry: the reduce half of F.batch_norm's backward
+ * (classification/resnet/models/networks.py:108,112 bn1 / bn2 under loss.backward(), utils.py:33) without a pass over the
+ * gradient. Feed the rows to b200_bn_bwd_finalize, then b200_bn_bwd_apply(src_is_dz=1). The output channel count must be a
+ * multiple of 64 and every field set. */
+typedef struct {
+  const void* x_raw;   /* bf16 raw output of the BatchNorm being differentiated, same geometry as the GEMM output */
+  const float* scale;  /* b200_bn_finalize coefficients */
+  const float* shift;
+  float* stats;        /* [rows][2][C]: sum(dz), sum(dz * x_raw) */
+} b200_bn_mask_t;
 /* same convolution writing an fp32 NHWC output (+bias) through TMA - ConvNeXt downsample conv feeding the fp32 stream */
 int b200_conv2d_fwd_f32(const void* x, const void* w, float* y, int B, int H, int W, int Cin, int Cout, int ksize,
                         int stride, const float* bias, void* stream);
@@ -74,38 +81,35 @@ int b200_conv2d_fwd_f32(const void* x, const void* w, float* y, int B, int H, in
  *   ksize 1 & stride 2 writes only the even (h,w) pixels of dx; the others keep their previous contents.
  * replaces the cuDNN backward-data / cuBLAS dgrad autograd runs inside loss.backward() (classification/resnet/utils.py:43). */
 int b200_conv2d_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int Cin, int Cout, int ksize,
-                      int stride, const void* residual, void* stream);
+                      int stride, const void* residual, const b200_bn_mask_t* bn_mask, void* stream);
 
 /* weight gradient: dw[Cout][Cin][ksize][ksize] (fp32, OIHW) (+)= sum_pixels dy (x) x
  *   workspace: b200_conv2d_wgrad_workspace_bytes() bytes of scratch for the split-K partial tiles.
+ *   bias_partial  optional: also produce the BIAS gradient = column sums of dy, as per-split partial sums
+ *            fp32 [b200_conv2d_wgrad_splits()][2][Cout] (plane 0; fold with b200_bn_bwd_finalize). The dy tiles are summed
+ *            from shared memory by four extra warps of the wgrad kernel: no separate pass over dy
+ *            (replaces the bias part of loss.backward() for nn.Linear / nn.Conv2d(bias=True): vit_model.py:95,109,127-133).
+ *   bias_out optional, requires bias_partial: the split reduction that follows the wgrad GEMM also folds bias_partial into
+ *            the finished bias gradient bias_out[Cout] - no launch of its own.
  * replaces the cuDNN backward-filter / cuBLAS wgrad inside loss.backward(). */
 int b200_conv2d_wgrad(const void* dy, const void* x, float* dw, void* workspace, size_t workspace_bytes, int B, int H,
-                      int W, int Cin, int Cout, int ksize, int stride, int accumulate, void* stream);
+                      int W, int Cin, int Cout, int ksize, int stride, int accumulate, float* bias_partial, float* bias_out,
+                      void* stream);
 size_t b200_conv2d_wgrad_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int stride);
-/* one-shot (this thread, next b200_conv2d_wgrad call): multiply gradient row `cout` by rowscale[cout] (layer scale) */
-int b200_conv2d_wgrad_set_rowscale(const float* rowscale);
-/* one-shot (this thread, next b200_conv2d_wgrad call): also produce the BIAS gradient = column sums of dy, as per-split
- * partial sums bias_partial fp32 [b200_conv2d_wgrad_splits()][2][Cout] (plane 0; fold with b200_bn_bwd_finalize).  The dy tiles
- * are summed from shared memory by four extra warps of the wgrad kernel: no separate pass over dy
- * (replaces the bias part of loss.backward() for nn.Linear / nn.Conv2d(bias=True): vit_model.py:95,109,127-133). */
-int b200_conv2d_wgrad_set_bias_partial(float* bias_partial);
-/* one-shot, together with set_bias_partial: the split reduction that follows the wgrad GEMM also folds bias_partial into the
- * finished bias gradient bias_out[Cout] (nn.Linear / nn.Conv2d bias under loss.backward()) - no launch of its own */
-int b200_conv2d_wgrad_set_bias_out(float* bias_out);
 int b200_conv2d_wgrad_splits(int B, int H, int W, int Cin, int Cout, int ksize, int stride);
 
 /* ---- grouped 3x3 convolution (ResNeXt conv2: classification/resnet/models/networks.py:295-321, nn.Conv2d(groups=g)) ------
  * C input = C output channels, C % 64 == 0, group width Cg = C / groups in {4, 8, 16, 32, 64}, ksize 3 (pad 1), stride 1 / 2.
  * Anything else returns B200_EINVAL with a message and launches nothing.
  * forward: y[B,Ho,Wo,C] = conv(x[B,H,W,C], w) (act: 0 or B200_ACT_RELU); w bf16 [C][9*64] (b200_pack_weight mode 3);
- *   stats as for b200_conv2d_fwd, rows = b200_conv2d_grouped_fwd_stats_rows(); honours b200_conv2d_fwd_set_bn. */
+ *   stats as for b200_conv2d_fwd, rows = b200_conv2d_grouped_fwd_stats_rows(); bn_scale / bn_shift as for b200_conv2d_fwd. */
 int b200_conv2d_grouped_fwd(const void* x, const void* w, void* y, int B, int H, int W, int C, int groups, int ksize,
-                            int stride, float* stats, int act, void* stream);
+                            int stride, float* stats, int act, const float* bn_scale, const float* bn_shift, void* stream);
 int b200_conv2d_grouped_fwd_stats_rows(int B, int H, int W, int C, int groups, int ksize, int stride);
-/* data gradient dx[B,H,W,C] from dy[B,Ho,Wo,C]; wd bf16 [C][9*64] (b200_pack_weight mode 4). Honours b200_dgrad_set_bn_mask at
- * stride 1, with rows = b200_conv2d_grouped_fwd_stats_rows(B, H, W, C, groups, 3, 1). */
+/* data gradient dx[B,H,W,C] from dy[B,Ho,Wo,C]; wd bf16 [C][9*64] (b200_pack_weight mode 4). bn_mask as for
+ * b200_conv2d_dgrad (stride 1), with rows = b200_conv2d_grouped_fwd_stats_rows(B, H, W, C, groups, 3, 1). */
 int b200_conv2d_grouped_dgrad(const void* dy, const void* wd, void* dx, int B, int H, int W, int C, int groups, int ksize,
-                              int stride, void* stream);
+                              int stride, const b200_bn_mask_t* bn_mask, void* stream);
 /* weight gradient dw[C][C/groups][3][3] (fp32, OIHW) (+)= sum_pixels dy (x) x within each group; workspace =
  * b200_conv2d_grouped_wgrad_workspace_bytes() bytes (0 for an unsupported shape). */
 int b200_conv2d_grouped_wgrad(const void* dy, const void* x, float* dw, void* workspace, size_t workspace_bytes, int B,
@@ -367,9 +371,9 @@ int b200_bn_conv1x1_bwd(const float* dz_partial, int T, const float* D, const fl
                         const float* w_f32, int N, int K, double count, const float* gamma, const float* mean,
                         const float* invstd, float* dgamma, float* dbeta, float* dW, int accumulate, void* wcat, float* bias,
                         void* scratch, size_t scratch_bytes, void* tickets, void* stream);
-/* out[pixels][N] (bf16) = [a0[pixels][K0] | a1[pixels][K1]] * wcat[N][K0 + K1]^T + bias[N] */
+/* out[pixels][N] (bf16) = [a0[pixels][K0] | a1[pixels][K1]] * wcat[N][K0 + K1]^T + bias[N]; bn_mask as for b200_conv2d_dgrad */
 int b200_gemm_dual(const void* a0, int K0, const void* a1, int K1, const void* wcat, const float* bias, void* out,
-                   long long pixels, int N, void* stream);
+                   long long pixels, int N, const b200_bn_mask_t* bn_mask, void* stream);
 
 /* ---- stochastic depth / pre_logits helpers -------------------------------------------------------------------------------
  * y[b, :] = x[b, :] * scale[b] over bf16 samples of elems_per_sample elements: the gradient entering a residual branch whose
@@ -381,9 +385,6 @@ int b200_rowscale_bf16(const void* x, const float* scale, void* y, long long n_s
  * its bf16 copy (operand of the classifier GEMM); backward du = dt * (1 - t^2), bf16 in / out. */
 int b200_tanh_fwd(const float* u, float* t, void* t_bf16, long long n, void* stream);
 int b200_tanh_bwd(const void* dt_bf16, const float* t, void* du_bf16, long long n, void* stream);
-
-/* bring-up only: override the wgmma shared-memory descriptor strides (which: 0 = forward K-major, 1 = wgrad MN-major) */
-int b200_debug_set_desc(int which, unsigned lbo, unsigned sbo, unsigned kstep);
 
 #ifdef __cplusplus
 }

@@ -28,7 +28,7 @@ def test_no_compute_calls_without_gpu_but_metadata_works():
     from deeplearning_b200 import _lib
 
     lib = _lib.load()
-    assert lib.b200_abi_version() >= 1
+    assert lib.b200_abi_version() == 2
     # pure host-side planners are usable without a device
     # BN statistics rows: (persistent CTAs / channel blocks) x 4 row quadrants (x2 when the warp pair alternates tiles);
     # without a device the planner assumes the 132 SMs of an H100 SXM; channel blocks are 64 or 128 wide
@@ -41,13 +41,37 @@ def test_no_compute_calls_without_gpu_but_metadata_works():
     assert lib.b200_bn_bwd_blocks(100, 96) == -1  # unsupported channel count is reported, not guessed
 
 
-def test_error_convention():
+def test_rejected_call_returns_einval_with_message():
     from deeplearning_b200 import _lib
 
     lib = _lib.load()
-    rc = lib.b200_conv2d_fwd(None, None, None, 1, 8, 8, 64, 64, 5, 1, None, None, 0, None, None, 0, None)
+    rc = lib.b200_conv2d_fwd(None, None, None, 1, 8, 8, 64, 64, 5, 1, None, None, 0, None, None, 0, None, None, None)
     assert rc == -1  # B200_EINVAL: 5x5 is not supported, and nothing was launched
     assert "ksize" in _lib.last_error()
+
+
+def test_no_per_thread_setters():
+    """Every option of a call travels as an argument: the header declares no b200_*_set_* entry that arms the next call."""
+    assert [n for n in _declared() if "_set_" in n] == []
+
+
+def test_epilogue_options_are_checked_before_launch():
+    """Inconsistent epilogue options are rejected with B200_EINVAL and a message before any CUDA or driver call, so these
+    run without a device (the fake pointers are never dereferenced)."""
+    from deeplearning_b200 import _lib
+
+    lib = _lib.load()
+    fake = 256
+    for scale, shift in [(fake, None), (None, fake)]:   # the folded BatchNorm needs both coefficient vectors
+        rc = lib.b200_conv2d_fwd(None, None, None, 1, 8, 8, 64, 64, 1, 1, None, None, 0, None, None, 0, scale, shift, None)
+        assert rc == -1 and "bn_scale" in _lib.last_error(), _lib.last_error()
+    rc = lib.b200_conv2d_wgrad(None, None, None, None, 0, 1, 8, 8, 64, 64, 1, 1, 0, None, fake, None)
+    assert rc == -1 and "bias_partial" in _lib.last_error(), _lib.last_error()
+    mask = _lib.BnMask(fake, fake, fake, fake)
+    rc = lib.b200_conv2d_dgrad(None, None, None, 1, 8, 8, 64, 64, 3, 2, None, mask, None)
+    assert rc == -1 and "stride 1" in _lib.last_error(), _lib.last_error()
+    rc = lib.b200_gemm_dual(None, 64, None, 64, None, None, None, 128, 72, mask, None)
+    assert rc == -1 and "N % 64" in _lib.last_error(), _lib.last_error()
 
 
 def test_missing_library_fails_loudly(monkeypatch):

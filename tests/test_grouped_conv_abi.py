@@ -43,12 +43,13 @@ def test_grouped_wgrad_workspace_is_split_diagonal_blocks():
     (96, 24, 3, 1, "multiple of 64"),    # C % 64 != 0
     (128, 32, 1, 1, "ksize"),
     (128, 32, 3, 3, "stride"),
+    (128, 0, 3, 1, "multiple of 64"),    # groups = 0
 ])
-def test_grouped_entries_reject_out_of_scope(C, groups, ksize, stride, msg):
+def test_grouped_entries_reject_out_of_scope_shapes(C, groups, ksize, stride, msg):
     _l, lib = _lib()
-    rc = lib.b200_conv2d_grouped_fwd(None, None, None, 2, 8, 8, C, groups, ksize, stride, None, 0, None)
+    rc = lib.b200_conv2d_grouped_fwd(None, None, None, 2, 8, 8, C, groups, ksize, stride, None, 0, None, None, None)
     assert rc == -1 and msg in _l.last_error(), _l.last_error()
-    rc = lib.b200_conv2d_grouped_dgrad(None, None, None, 2, 8, 8, C, groups, ksize, stride, None)
+    rc = lib.b200_conv2d_grouped_dgrad(None, None, None, 2, 8, 8, C, groups, ksize, stride, None, None)
     assert rc == -1 and msg in _l.last_error(), _l.last_error()
     rc = lib.b200_conv2d_grouped_wgrad(None, None, None, None, 0, 2, 8, 8, C, groups, ksize, stride, 0, None)
     assert rc == -1 and msg in _l.last_error(), _l.last_error()

@@ -147,7 +147,7 @@ def chains(name, B, H, Cs, Cb):
                 sl = slice(i * b, (i + 1) * b)
                 _lib.check(lib.b200_bn_apply(p(c3[sl]), p(dzn[sl]), p(y_out[sl]), p(co.scale), p(co.shift), r, Cb, 1, st()), "bn_apply")
                 _lib.check(lib.b200_conv2d_fwd(p(y_out[sl]), p(w1f), p(c1[sl]), b, H, H, Cb, Cs, 1, 1, p(stats[i]), None, 0, None,
-                                               None, 0, st()), "conv")
+                                               None, 0, None, None, st()), "conv")
 
         t_fwd = timed_graph(fwd)
         chunk_mb = b * H * H * Cb * 2 / 1e6
