@@ -1,6 +1,5 @@
 // C-ABI entry points for the wgmma implicit-GEMM kernels (forward / dgrad / wgrad). Host side only builds tensor maps,
 // tap tables and tile geometry; see conv_gemm.cuh / wgrad_gemm.cuh for the device code.
-#include <stdlib.h>
 #include <string.h>
 #include "../../include/b200cls.h"
 #include "conv_gemm.cuh"
@@ -278,17 +277,10 @@ int epilogue_flags(const ConvGemmParams& p) {
   X(kEpiBnMask | kEpiBias)                                /* the same behind the BN-algebra dual GEMM (bias = k W) */
 
 // ---- 64 -> 64 channel convolutions with the weights resident in shared memory (conv_tap64.cuh): ResNet layer1's 3x3
-// forward / dgrad and the space-to-depth stem.  B200_TAP64=0 in the environment switches back to the generic kernel.
-bool tap64_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("B200_TAP64");
-    return e == nullptr || e[0] != '0';
-  }();
-  return on;
-}
+// forward / dgrad and the space-to-depth stem.
 bool tap64_ok(const ConvGemmParams& p) {
   const int f = epilogue_flags(p);
-  return tap64_enabled() && p.N == 64 && p.n_tiles == 1 && p.k_per_tap == 64 && p.k_blocks_per_tap == 1 && !p.var_taps && !p.chan_window &&
+  return p.N == 64 && p.n_tiles == 1 && p.k_per_tap == 64 && p.k_blocks_per_tap == 1 && !p.var_taps && !p.chan_window &&
          p.num_taps >= 2 && p.num_taps <= 9 && (f == 0 || f == kEpiStats) && p.dim1 % p.box1 == 0 && p.dim2 % p.box2 == 0 &&
          p.dim3 % p.box3 == 0;
 }
@@ -329,15 +321,8 @@ int launch_conv_gemm(const ConvGemmParams& p, cudaStream_t st) {
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Streaming kernel for the narrow-K -> wide-N 1x1 layers (conv1x1_stream.cuh): K in {64, 128, 256}, N % 256 == 0, pixels % 128 == 0.
-bool stream_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("B200_STREAM");
-    return e == nullptr || e[0] != '0';
-  }();
-  return on;
-}
 bool stream_ok(long long pixels, int K, int N) {
-  return stream_enabled() && (K == 64 || K == 128 || K == 256) && N % 256 == 0 && pixels % 128 == 0 && pixels / 128 < (1LL << 30);
+  return (K == 64 || K == 128 || K == 256) && N % 256 == 0 && pixels % 128 == 0 && pixels / 128 < (1LL << 30);
 }
 int stream_grid(long long pixels, int N) {
   const int n_tiles = N / 256;

@@ -78,8 +78,6 @@ int b200_layernorm_bwd(const void* dy, const void* x, int x_f32, const float* me
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int grid = ln_bwd_blocks(rows);
   const __nv_bfloat16* dyp = static_cast<const __nv_bfloat16*>(dy);
-  // B200_LN_BWD=1: first version of the kernel (the residual gradient fetched after the row reductions); default: version 2
-  static const bool ln_v1 = [] { const char* e = getenv("B200_LN_BWD"); return e != nullptr && e[0] == '1'; }();
 #define LN_BWD_V(TI, TO, MV, LPR)                                                                                   \
   do {                                                                                                              \
     static bool cfg = false;                                                                                        \
@@ -87,20 +85,12 @@ int b200_layernorm_bwd(const void* dy, const void* x, int x_f32, const float* me
       B200_CHECK_CUDA(cudaFuncSetAttribute(layernorm_bwd_kernel<TI, TO, MV, LPR>,                                   \
                                            cudaFuncAttributeMaxDynamicSharedMemorySize,                             \
                                            8 * 2 * 1024 * (int)sizeof(float)));                                     \
-      B200_CHECK_CUDA(cudaFuncSetAttribute(layernorm_bwd2_kernel<TI, TO, MV, LPR>,                                  \
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize,                             \
-                                           8 * 2 * 1024 * (int)sizeof(float)));                                     \
       cfg = true;                                                                                                   \
     }                                                                                                               \
     const size_t smem = static_cast<size_t>(8) * (32 / LPR) * 2 * C * sizeof(float);                                \
-    if (ln_v1)                                                                                                      \
-      B200_CHECK_CUDA(launch_pdl(layernorm_bwd_kernel<TI, TO, MV, LPR>, dim3(grid), dim3(256), smem, st, dyp,       \
-                                 static_cast<const TI*>(x), mean, rstd, gamma, static_cast<const TO*>(add),        \
-                                 static_cast<TO*>(dx), partial, rows, C));                                          \
-    else                                                                                                            \
-      B200_CHECK_CUDA(launch_pdl(layernorm_bwd2_kernel<TI, TO, MV, LPR>, dim3(grid), dim3(256), smem, st, dyp,      \
-                                 static_cast<const TI*>(x), mean, rstd, gamma, static_cast<const TO*>(add),        \
-                                 static_cast<TO*>(dx), partial, rows, C));                                          \
+    B200_CHECK_CUDA(launch_pdl(layernorm_bwd_kernel<TI, TO, MV, LPR>, dim3(grid), dim3(256), smem, st, dyp,         \
+                               static_cast<const TI*>(x), mean, rstd, gamma, static_cast<const TO*>(add),          \
+                               static_cast<TO*>(dx), partial, rows, C));                                            \
   } while (0)
 #define LN_BWD(TI, TO)                  \
   do {                                  \

@@ -34,7 +34,6 @@ namespace b200 {
 // (The one-thread-per-row version this replaces touched 32 different 128-byte lines per instruction: 2.9 TB/s.)
 __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __restrict__ dO, const __nv_bfloat16* __restrict__ O,
                                                          float* __restrict__ delta, int B, int T, int H) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long total = static_cast<long long>(B) * T * H;
   const int sub = threadIdx.x & 7;

@@ -41,7 +41,6 @@ constexpr int kAttnBwdThreads = 384;   // warpgroup 0: TMA producer (warp 0), wa
 static_assert(kAttnBwdSmemBytes <= 227 * 1024, "shared memory of one H100 block");
 
 __global__ void __launch_bounds__(kAttnBwdThreads, 1) attn_bwd_kernel(const __grid_constant__ AttnBwdParams p) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));

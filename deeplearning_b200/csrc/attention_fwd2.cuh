@@ -27,7 +27,6 @@ static_assert(kAttn2SmemBytes <= 227 * 1024, "shared memory of one H100 block");
 // NT = the key tile (p.Tpad: T rounded up to 64, <= 256)
 template <int NT>
 __global__ void __launch_bounds__(kAttn2Threads, 1) attn_fwd2_kernel(const __grid_constant__ AttnFwdParams p) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));

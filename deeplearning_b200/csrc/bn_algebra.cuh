@@ -87,7 +87,6 @@ __global__ void __launch_bounds__(256) bn_gram_stats_kernel(const float* __restr
                                                             float eps, float momentum, float* running_mean,
                                                             float* running_var, long long* num_batches, float* mean_out,
                                                             float* invstd_out, float* scale_out, float* shift_out) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float sm_gs[];   // [32][K] chunk of G | [8 warps][K] weights | [K] column means
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -141,7 +140,6 @@ __global__ void __launch_bounds__(256) bn_conv1x1_bwd_rows_kernel(
     const float* __restrict__ s, const __nv_bfloat16* __restrict__ Wb, const float* __restrict__ W, int N, int K, double count,
     const float* __restrict__ gamma, const float* __restrict__ mean, const float* __restrict__ invstd, float* dgamma,
     float* dbeta, float* dW, int accumulate, __nv_bfloat16* __restrict__ wcat, float2* __restrict__ coef) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float sm_f[];   // [32][K] chunk of G | [8 warps][K] bf16 weights (as float) of the warp's channel
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -220,7 +218,6 @@ __global__ void __launch_bounds__(256) bn_conv1x1_bwd_m_kernel(const float2* __r
                                                                const float* __restrict__ W, int N, int K,
                                                                __nv_bfloat16* __restrict__ wcat, float* __restrict__ bias,
                                                                unsigned int* __restrict__ tickets, float* __restrict__ partial) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float sa[32][33];   // b_o * Wb[o][j0 + .]
   __shared__ float sw[32][33];   // W[o][i0 + .]

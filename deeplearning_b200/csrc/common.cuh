@@ -18,22 +18,9 @@ constexpr int kNumSMs = 132;
 // pdl_wait() until the PREVIOUS kernel has completed and its memory is visible.  Every kernel executes the wait before it
 // touches global memory (and before it can exit), so completion stays transitive along the stream: the data dependencies
 // are exactly those of plain stream order, only launch latency and prologues overlap the predecessor's end.
-// No kernel triggers its dependents explicitly: dependents scheduled early pile onto the SMs that drain first and unbalance
-// the next grid (B200_PDL_TRIGGER selects the other two placements for experiments).
-#ifndef B200_PDL_TRIGGER
-#define B200_PDL_TRIGGER 0   // 0: never (implicit at grid completion), 1: at kernel entry, 2: right after the wait
-#endif
-__device__ __forceinline__ void pdl_launch_dependents() {
-#if B200_PDL_TRIGGER == 1
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void pdl_wait() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-#if B200_PDL_TRIGGER == 2
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-#endif
-}
+// No kernel triggers its dependents explicitly (griddepcontrol.launch_dependents), neither at kernel entry nor right after
+// the wait: dependents scheduled early pile onto the SMs that drain first and unbalance the next grid.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));

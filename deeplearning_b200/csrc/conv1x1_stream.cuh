@@ -72,7 +72,6 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src_
 
 template <int KB, int MODE>
 __global__ void __launch_bounds__(384, 1) conv1x1_stream_kernel(const __grid_constant__ StreamParams p) {
-  pdl_launch_dependents();
   using Cfg = StreamCfg<KB, MODE>;
   constexpr int STAGES = Cfg::STAGES, NBUF = Cfg::NBUF;
   extern __shared__ uint8_t smem_raw[];

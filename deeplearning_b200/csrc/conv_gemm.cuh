@@ -211,7 +211,6 @@ constexpr int kEpiBias = 1, kEpiColscale = 2, kEpiActShift = 2 /* 2 bits */, kEp
 
 template <int BLOCK_N, int EPI = kEpiGeneric>
 __global__ void __launch_bounds__(512, 1) conv_gemm_kernel(const __grid_constant__ ConvGemmParams p) {
-  pdl_launch_dependents();
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "64- or 128-column tiles");
   using Cfg = ConvGemmCfg<BLOCK_N>;
   constexpr int STAGES = Cfg::STAGES;

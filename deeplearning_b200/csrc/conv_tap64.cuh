@@ -23,7 +23,6 @@ static_assert(kTap64SmemBytes <= 227 * 1024, "shared memory of one H100 block");
 
 template <bool kStats>
 __global__ void __launch_bounds__(384, 1) conv_tap64_kernel(const __grid_constant__ ConvGemmParams p) {
-  pdl_launch_dependents();
   constexpr int STAGES = kTap64Stages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));

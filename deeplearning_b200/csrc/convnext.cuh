@@ -41,7 +41,6 @@ template <typename TIn, typename TOut, bool FLIP>
 __global__ void __launch_bounds__(128) dwconv7_kernel(const TIn* __restrict__ in, const float* __restrict__ wt,
                                                        const float* __restrict__ bias, const TOut* __restrict__ add,
                                                        TOut* __restrict__ out, int B, int H, int W, int C) {
-  pdl_launch_dependents();
   pdl_wait();
   const int c4n = C >> 2;
   const int wstrips = (W + 3) >> 2;
@@ -105,7 +104,6 @@ __global__ void __launch_bounds__(128) dwconv7_kernel(const TIn* __restrict__ in
 __global__ void __launch_bounds__(224) dwconv7_wgrad_kernel(const __nv_bfloat16* __restrict__ du, const float* __restrict__ x,
                                                             float* __restrict__ part, int B, int H, int W, int C,
                                                             int rows_per_block) {
-  pdl_launch_dependents();
   pdl_wait();
   const int cq = blockIdx.x * 32 + (threadIdx.x & 31);
   const int kh = threadIdx.x >> 5;  // 0..6
@@ -205,7 +203,6 @@ template <typename TIn, typename TOut, bool FLIP>
 __global__ void __launch_bounds__(128, 4) dwconv7_tile_kernel(const TIn* __restrict__ in, const float* __restrict__ wt,
                                                               const float* __restrict__ bias, const TOut* __restrict__ add,
                                                               TOut* __restrict__ out, int B, int H, int W, int C) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float dw_smem[];  // [20][20][32]
   const int cgroups = C / kDwCh, tiles_w = W / kDwTile, tiles_h = H / kDwTile;
@@ -265,7 +262,6 @@ __global__ void __launch_bounds__(128, 4) dwconv7_tile_kernel(const TIn* __restr
 __global__ void __launch_bounds__(128, 3) dwconv7_wgrad_tile_kernel(const __nv_bfloat16* __restrict__ du,
                                                                     const float* __restrict__ x, float* __restrict__ part,
                                                                     int B, int H, int W, int C, int tiles_per_cta) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float dw_smem[];  // x halo fp32 [20][20][32] | du tile bf16 [14][14][32]
   float* s_x = dw_smem;
@@ -328,7 +324,6 @@ __global__ void __launch_bounds__(128, 3) dwconv7_wgrad_tile_kernel(const __nv_b
 // dW[c][tap] (+)= sum_t part[t][tap][c]   ([C,1,7,7] parameter layout)
 __global__ void dwconv7_wgrad_finalize_kernel(const float* __restrict__ part, int T, int C, float* __restrict__ dw,
                                               int accumulate) {
-  pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;  // over tap*C + c (coalesced reads)
   if (i >= 49 * C) return;
@@ -341,7 +336,6 @@ __global__ void dwconv7_wgrad_finalize_kernel(const float* __restrict__ part, in
 
 // [C,1,7,7] fp32 parameter -> tap-major [49][C] copy
 __global__ void dwconv7_pack_kernel(const float* __restrict__ w, float* __restrict__ wt, int C) {
-  pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 49 * C) return;
@@ -352,7 +346,6 @@ __global__ void dwconv7_pack_kernel(const float* __restrict__ w, float* __restri
 // Global average pool of a [B][HW][C] tensor (fp32 or bf16) -> fp32 [B][C]; backward broadcasts g/HW (bf16 out).
 template <typename TIn>
 __global__ void avgpool_any_fwd_kernel(const TIn* __restrict__ x, float* __restrict__ y, int B, int HW, int C) {
-  pdl_launch_dependents();
   pdl_wait();
   const int c4n = C >> 2;
   const long long total = static_cast<long long>(B) * c4n;
@@ -373,7 +366,6 @@ __global__ void avgpool_any_fwd_kernel(const TIn* __restrict__ x, float* __restr
 // partial[slice][2][cols]: plane 0 = column sums of a[r][c] * b[r][c] (b optional), plane 1 = 0
 __global__ void colsum_prod_partial_kernel(const __nv_bfloat16* __restrict__ a, const __nv_bfloat16* __restrict__ bmat,
                                            long long rows, long long ld, int cols, float* __restrict__ partial) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float sh[4][64];
   const int cx = threadIdx.x & 63, ry = threadIdx.x >> 6;
@@ -402,7 +394,6 @@ __global__ void layerscale_grads_kernel(const float* __restrict__ G, const float
                                         const float* __restrict__ b2, const float* __restrict__ gsum,
                                         const float* __restrict__ gamma, float* __restrict__ dW2, float* __restrict__ db2,
                                         float* __restrict__ dgamma, int C, int K) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float sh[8];
   const int c = blockIdx.x;
@@ -431,7 +422,6 @@ __global__ void layerscale_grads_kernel(const float* __restrict__ G, const float
 // hyper = {lr, 1-beta1^t, 1-beta2^t, beta1^t, beta2^t}: advances t by one (single thread), entirely on the device so the
 // optimizer step can be replayed inside a CUDA graph.
 __global__ void adamw_tick_kernel(float* __restrict__ hyper, float beta1, float beta2) {
-  pdl_launch_dependents();
   pdl_wait();
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     const float p1 = hyper[3] * beta1, p2 = hyper[4] * beta2;
@@ -448,7 +438,6 @@ __global__ void adamw_tick_kernel(float* __restrict__ hyper, float beta1, float 
 //   clip[0] = min(1, max_norm / (total_norm + 1e-6)), clip[1] = total_norm;  the optimizer kernels multiply by clip[0].
 __global__ void __launch_bounds__(256) grad_sumsq_partial_kernel(const float* __restrict__ g, long long n,
                                                                  float* __restrict__ partial) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float red[8];
   float s = 0.f;
@@ -474,7 +463,6 @@ __global__ void __launch_bounds__(256) grad_sumsq_partial_kernel(const float* __
 }
 __global__ void __launch_bounds__(256) grad_clip_coef_kernel(const float* __restrict__ partial, int nblocks, float gscale,
                                                              float max_norm, float* __restrict__ clip) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ double red[8];
   double s = 0.0;
@@ -496,7 +484,6 @@ __global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g,
                              float* __restrict__ v, const float* __restrict__ wd, long long n,
                              const float* __restrict__ hyper, float beta1, float beta2, float eps, float gscale,
                              const float* __restrict__ clip) {
-  pdl_launch_dependents();
   pdl_wait();
   if (clip != nullptr) gscale *= __ldg(clip);
   const float lr = __ldg(hyper), bc1 = __ldg(hyper + 1), bc2 = __ldg(hyper + 2);

@@ -100,7 +100,6 @@ __global__ void bn_finalize_kernel(const float* __restrict__ partial, int T, int
                                    float momentum, float* running_mean, float* running_var, long long* num_batches,
                                    float* mean_out, float* invstd_out, float* scale_out, float* shift_out,
                                    void* scratch) {
-  pdl_launch_dependents();
   pdl_wait();
   double s, ss;
   const bool owner = reduce_partials_last_block(partial, T, C, scratch, s, ss);
@@ -128,7 +127,6 @@ __global__ void bn_finalize_kernel(const float* __restrict__ partial, int T, int
 __global__ void bn_eval_coeffs_kernel(int C, const float* __restrict__ gamma, const float* __restrict__ beta,
                                       const float* __restrict__ running_mean, const float* __restrict__ running_var,
                                       float eps, float* scale_out, float* shift_out) {
-  pdl_launch_dependents();
   pdl_wait();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c < C) {
@@ -143,7 +141,6 @@ __global__ void bn_eval_coeffs_kernel(int C, const float* __restrict__ gamma, co
 __global__ void __launch_bounds__(256) bn_apply_kernel(const uint4* __restrict__ x, const uint4* __restrict__ residual,
                                                        uint4* __restrict__ y, const float* __restrict__ scale,
                                                        const float* __restrict__ shift, long long nvec, int cvec, int relu) {
-  pdl_launch_dependents();
   pdl_wait();
   // four independent 16-byte vectors (plus their residuals) per thread and iteration: ~100 KB of loads in flight per SM,
   // which is what HBM3e needs to stay busy (one vector per iteration left the kernel at ~5.2 of 6.5 TB/s)
@@ -193,7 +190,6 @@ __global__ void __launch_bounds__(256, 2)
 bn_bwd_reduce_kernel(const uint4* __restrict__ g, const uint4* __restrict__ x, const uint4* __restrict__ y_out,
                      uint4* __restrict__ dz_out, const float* __restrict__ scale, const float* __restrict__ shift, int relu,
                      long long rows, int cvec, int rows_per_block, float* __restrict__ partial) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float red[];  // [256][17]
   const int tpr = cvec;                  // threads per row (power of two, <= 256)
@@ -284,7 +280,6 @@ __global__ void bn_bwd_finalize_kernel(const float* __restrict__ partial, int T,
                                        float* __restrict__ dgamma, float* __restrict__ dbeta, int accumulate,
                                        float* __restrict__ m1, float* __restrict__ m2, const float* __restrict__ mean,
                                        const float* __restrict__ invstd, void* scratch) {
-  pdl_launch_dependents();
   pdl_wait();
   double s, ss;
   const bool owner = reduce_partials_last_block(partial, T, C, scratch, s, ss);
@@ -307,7 +302,6 @@ __global__ void bn_bwd_apply_kernel(const uint4* __restrict__ g, const uint4* __
                                     const float* __restrict__ mean, const float* __restrict__ invstd,
                                     const float* __restrict__ m1, const float* __restrict__ m2, int relu,
                                     long long rows, int cvec, int rows_per_block) {
-  pdl_launch_dependents();
   pdl_wait();
   const int tpr = cvec, rpi = 256 / tpr;
   const int cg = threadIdx.x % tpr, rsub = threadIdx.x / tpr;
@@ -379,7 +373,6 @@ __global__ void __launch_bounds__(256) bn_relu_maxpool_fwd_kernel(const uint4* _
                                                                   unsigned long long* __restrict__ idx,
                                                                   const float* __restrict__ scale,
                                                                   const float* __restrict__ shift, int B, int H, int W, int cvec) {
-  pdl_launch_dependents();
   pdl_wait();
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
   const unsigned nvec = static_cast<unsigned>(B) * Ho * Wo * cvec;
@@ -441,7 +434,6 @@ __global__ void __launch_bounds__(256) bn_relu_maxpool_fwd_kernel(const uint4* _
 __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const uint4* __restrict__ g_out,
                                                           const unsigned long long* __restrict__ idx, uint4* __restrict__ g_in,
                                                           int B, int H, int W, int cvec) {
-  pdl_launch_dependents();
   pdl_wait();
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;   // = H / 2, W / 2
   const unsigned nblk = static_cast<unsigned>(B) * Ho * Wo * cvec;
@@ -489,7 +481,6 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const uint4* __restric
 
 // Global average pool over HW: x [B][HW][C] bf16 -> y [B][C] bf16.
 __global__ void avgpool_fwd_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int B, int HW, int cvec) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long nvec = static_cast<long long>(B) * cvec;
   const float inv = 1.0f / HW;
@@ -513,7 +504,6 @@ __global__ void avgpool_fwd_kernel(const uint4* __restrict__ x, uint4* __restric
 }
 // Backward: g_x[b][p][c] = g_y[b][c] / HW.
 __global__ void avgpool_bwd_kernel(const uint4* __restrict__ gy, uint4* __restrict__ gx, int B, int HW, int cvec) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long nvec = static_cast<long long>(B) * HW * cvec;
   const float inv = 1.0f / HW;
@@ -541,7 +531,6 @@ __global__ void softmax_xent_kernel(const float* __restrict__ logits, long long 
                                     int N, float gscale, float* __restrict__ loss_rows,
                                     __nv_bfloat16* __restrict__ dlogits, long long ld_d, int* __restrict__ correct,
                                     const float* __restrict__ soft, long long ld_soft, float smoothing) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float sh[32];
   __shared__ int shi[32];
@@ -654,7 +643,6 @@ __global__ void softmax_xent_kernel(const float* __restrict__ logits, long long 
 
 // mean of n floats -> out[0] (single block)
 __global__ void mean_kernel(const float* __restrict__ v, int n, float* __restrict__ out) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float sh[32];
   float s = 0.f;
@@ -672,7 +660,6 @@ __global__ void mean_kernel(const float* __restrict__ v, int n, float* __restric
 // Column sums of a bf16 matrix [rows][ld] -> fp32 out[cols] (bias gradients). One block per 64 columns.
 __global__ void colsum_kernel(const __nv_bfloat16* __restrict__ m, long long rows, long long ld, int cols,
                               float* __restrict__ out, int accumulate) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float sh[4][64];
   const int cx = threadIdx.x & 63, ry = threadIdx.x >> 6;
@@ -708,7 +695,6 @@ __device__ __forceinline__ float grouped_pack_value(const float* __restrict__ sr
 
 __global__ void pack_weight_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, int O, int I,
                                    int taps, int mode, long long ld_dst) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long rows = mode == 1 ? I : O;
   const long long total = rows * ld_dst;
@@ -736,14 +722,12 @@ __global__ void pack_weight_kernel(const float* __restrict__ src, __nv_bfloat16*
 
 // fp32 -> bf16 cast of a flat buffer (n multiple of 1 element; scalar tail-safe).
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n) {
-  pdl_launch_dependents();
   pdl_wait();
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
     dst[i] = __float2bfloat16_rn(src[i]);
 }
 __global__ void cast_bf16_f32_kernel(const __nv_bfloat16* __restrict__ src, float* __restrict__ dst, long long n) {
-  pdl_launch_dependents();
   pdl_wait();
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x)
@@ -755,7 +739,6 @@ __global__ void cast_bf16_f32_kernel(const __nv_bfloat16* __restrict__ src, floa
 // (zero padded left/right), then each thread assembles 16-byte output vectors from shared memory.
 __global__ void im2col_nchw_kernel(const float* __restrict__ x, uint4* __restrict__ a, int B, int Cin, int H, int W,
                                    int KH, int KW, int stride, int pad, int Ho, int Wo, int ldk) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float srow[];  // [Cin][KH][W + 2*pad] floats, then int lut[ldk]
   const int Wp = W + 2 * pad;
@@ -823,7 +806,6 @@ __device__ __forceinline__ void pack_zero_pad(__nv_bfloat16* dst, long long rows
 }
 
 __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const long long* __restrict__ table, int n_entries) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ int entry;
   __shared__ float sm[kPackTileFloats];
@@ -1035,7 +1017,6 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const long long
 // Stem weight gradient: patch-matrix layout [Cout][ldk] with k = tap*Cin + c  ->  OIHW [Cout][Cin][taps].
 __global__ void stem_wgrad_relayout_kernel(const float* __restrict__ src, float* __restrict__ dst, int Cout, int Cin,
                                            int taps, int ldk, int accumulate) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long total = static_cast<long long>(Cout) * Cin * taps;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
@@ -1054,7 +1035,6 @@ __global__ void stem_wgrad_relayout_kernel(const float* __restrict__ src, float*
 __global__ void sgd_momentum_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ buf,
                                     long long n, float lr, const float* __restrict__ lr_dev, float momentum, float wd,
                                     float gscale, int first_step, const float* __restrict__ clip) {
-  pdl_launch_dependents();
   pdl_wait();
   if (lr_dev != nullptr) lr = __ldg(lr_dev);  // device-resident learning rate: lets a captured CUDA graph follow a schedule
   if (clip != nullptr) gscale *= __ldg(clip);  // global-norm clipping coefficient (b200_grad_clip_coef)
@@ -1071,7 +1051,6 @@ __global__ void sgd_momentum_kernel(float* __restrict__ p, const float* __restri
 // Space-to-depth input of the stem: x fp32 NCHW [B][3][H][W] (H, W even) -> z bf16 [B][H/2+3][W/2+3][16],
 // z[b][Y][X][(dy*2+dx)*3 + c] = xpad[b][c][2Y+dy][2X+dx] with xpad = x zero-padded by 3 pixels; channels 12..15 = 0.
 __global__ void stem_s2d_kernel(const float* __restrict__ x, uint4* __restrict__ z, int B, int H, int W) {
-  pdl_launch_dependents();
   pdl_wait();
   const int Hz = H / 2 + 3, Wz = W / 2 + 3;
   const long long total = static_cast<long long>(B) * Hz * Wz;
@@ -1108,7 +1087,6 @@ __global__ void stem_s2d_kernel(const float* __restrict__ x, uint4* __restrict__
 // of x) as a flat GEMM, and its data gradient is added back onto the even pixels: gx[b][2i][2j][:] += gs[b][i][j][:].
 __global__ void __launch_bounds__(256) subsample2_kernel(const uint4* __restrict__ x, uint4* __restrict__ xs, int B, int H, int W,
                                                          int cvec) {
-  pdl_launch_dependents();
   pdl_wait();
   const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
   const unsigned total = static_cast<unsigned>(B) * Ho * Wo * cvec;
@@ -1124,7 +1102,6 @@ __global__ void __launch_bounds__(256) subsample2_kernel(const uint4* __restrict
 }
 __global__ void __launch_bounds__(256) add_even_pixels_kernel(uint4* __restrict__ gx, const uint4* __restrict__ gs, int B, int H,
                                                               int W, int cvec) {
-  pdl_launch_dependents();
   pdl_wait();
   const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
   const unsigned total = static_cast<unsigned>(B) * Ho * Wo * cvec;
@@ -1152,7 +1129,6 @@ __global__ void __launch_bounds__(256) add_even_pixels_kernel(uint4* __restrict_
 // fp32 NCHW batch never exists.
 __global__ void stem_s2d_u8_kernel(const unsigned char* __restrict__ x, uint4* __restrict__ z, int B, int H, int W, float a0,
                                    float a1, float a2, float b0, float b1, float b2) {
-  pdl_launch_dependents();
   pdl_wait();
   const int Hz = H / 2 + 3, Wz = W / 2 + 3;
   const long long total = static_cast<long long>(B) * Hz * Wz;
@@ -1189,7 +1165,6 @@ __global__ void stem_s2d_u8_kernel(const unsigned char* __restrict__ x, uint4* _
 // The same ToTensor + Normalize for the other families: uint8 NHWC -> fp32 NCHW (the layout their patch-embedding kernels read).
 __global__ void u8_nhwc_to_f32_nchw_kernel(const unsigned char* __restrict__ x, float* __restrict__ y, int B, int H, int W,
                                            float a0, float a1, float a2, float b0, float b1, float b2) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long total = static_cast<long long>(B) * H * W;
   const long long plane = static_cast<long long>(H) * W;
@@ -1206,7 +1181,6 @@ __global__ void u8_nhwc_to_f32_nchw_kernel(const unsigned char* __restrict__ x, 
 
 // Weight gradient of the space-to-depth stem: g[64][k64 = kx4*16 + (dy*2+dx)*3 + c][ky4] -> dW [64][3][7][7] (OIHW).
 __global__ void stem_s2d_wgrad_relayout_kernel(const float* __restrict__ g, float* __restrict__ dw, int accumulate) {
-  pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 64 * 3 * 49) return;
@@ -1222,7 +1196,6 @@ __global__ void stem_s2d_wgrad_relayout_kernel(const float* __restrict__ g, floa
 // lives in the GEMM epilogue (ConvGemmParams::rowscale).  vec_per_sample = elements per sample / 8.
 __global__ void __launch_bounds__(256) rowscale_bf16_kernel(const uint4* __restrict__ x, const float* __restrict__ scale,
                                                             uint4* __restrict__ y, long long nvec, long long vec_per_sample) {
-  pdl_launch_dependents();
   pdl_wait();
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nvec;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -1243,7 +1216,6 @@ __global__ void __launch_bounds__(256) rowscale_bf16_kernel(const uint4* __restr
 // backward) and its bf16 copy for the classifier GEMM;  backward: du = dt * (1 - t^2)  (bf16 in / out).
 __global__ void __launch_bounds__(256) tanh_fwd_kernel(const float* __restrict__ u, float* __restrict__ t,
                                                        __nv_bfloat16* __restrict__ t16, long long n) {
-  pdl_launch_dependents();
   pdl_wait();
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -1254,7 +1226,6 @@ __global__ void __launch_bounds__(256) tanh_fwd_kernel(const float* __restrict__
 }
 __global__ void __launch_bounds__(256) tanh_bwd_kernel(const __nv_bfloat16* __restrict__ dt, const float* __restrict__ t,
                                                        __nv_bfloat16* __restrict__ du, long long n) {
-  pdl_launch_dependents();
   pdl_wait();
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {

@@ -1,5 +1,4 @@
 #include "host_utils.h"
-#include <stdlib.h>
 
 #include <stdarg.h>
 #include <string.h>
@@ -87,14 +86,6 @@ static int encode_tmap_any(CUtensorMap* out, const void* base, int rank, const u
     return ECUDA_;
   }
   return OK;
-}
-
-bool pdl_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("B200_PDL");
-    return e == nullptr || e[0] != '0';
-  }();
-  return on;
 }
 
 int device_sm_count() {

@@ -53,8 +53,7 @@ extern unsigned long long g_launch_count;
 
 // Launch with programmatic stream serialization (see common.cuh pdl_wait): the kernel may be scheduled while its
 // predecessor in the stream drains; every kernel of the library waits for that predecessor (griddepcontrol.wait) before it
-// touches global memory.  B200_PDL=0 in the environment launches plainly.
-bool pdl_enabled();
+// touches global memory.
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg;
@@ -67,7 +66,7 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

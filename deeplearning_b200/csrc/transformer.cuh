@@ -50,7 +50,6 @@ __global__ void layernorm_fwd_kernel(const TIn* __restrict__ x, const float* __r
                                      const float* __restrict__ beta, TY* __restrict__ y,
                                      float* __restrict__ mean_out, float* __restrict__ rstd_out, long long rows, int C,
                                      float eps) {
-  pdl_launch_dependents();
   pdl_wait();
   constexpr int RPW = 32 / LPR;
   const int lane = threadIdx.x & 31, sub = lane % LPR, grp = lane / LPR;
@@ -107,100 +106,18 @@ __global__ void layernorm_fwd_kernel(const TIn* __restrict__ x, const float* __r
 }
 
 // dx = rstd * (dy*gamma - mean_c(dy*gamma) - xhat * mean_c(dy*gamma*xhat)) (+ add);  partial[block][2][C] = (sum dy, sum dy*xhat)
-// The per-column parameter-gradient accumulators live in shared memory (one private [2][C] slice per warp, updated with
-// conflict-free float4 read-modify-writes) so that the register budget only has to hold one row.
+//   * every load of a row - x, dy and a bf16 residual gradient `add` - is issued before anything is computed, so each row
+//     costs one exposed DRAM round trip.  The raw words stay in registers (x fp32 / dy, add bf16 packed) and xhat,
+//     dy*gamma are recomputed for the output phase - two more FMAs per element;
+//   * the per-column parameter-gradient accumulators live in shared memory (one private [2][C] slice per warp) so that the
+//     register budget only has to hold one row.  Each [C] is split into a plane of the low and a plane of the high float4 of
+//     every 8-channel vector, so that consecutive lanes touch consecutive 16-byte words (no bank conflict on the float4
+//     read-modify-writes).
 template <typename TIn, typename TOut, int MAXV, int LPR = 32>
 __global__ void __launch_bounds__(256, 3)
 layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const TIn* __restrict__ x, const float* __restrict__ mean,
                      const float* __restrict__ rstd, const float* __restrict__ gamma, const TOut* __restrict__ add,
                      TOut* __restrict__ dx, float* __restrict__ partial, long long rows, int C) {
-  pdl_launch_dependents();
-  pdl_wait();
-  extern __shared__ float red[];  // [warps][rows per warp][2][C]
-  constexpr int RPW = 32 / LPR;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  const int sub = lane % LPR, grp = lane / LPR;
-  const int nvec = C >> 3;
-  float* mine = red + (static_cast<long long>(warp) * RPW + grp) * 2 * C;
-  for (int i = sub; i < 2 * C; i += LPR) mine[i] = 0.f;
-  __syncwarp();
-  const long long warp0 = blockIdx.x * static_cast<long long>(nw) + warp;
-  const long long nwarps = static_cast<long long>(gridDim.x) * nw;
-  for (long long rb = warp0 * RPW; rb < rows; rb += nwarps * RPW) {
-    const long long r = rb + grp;
-    const bool live = r < rows;
-    const float mu = live ? mean[r] : 0.f, rs = live ? rstd[r] : 0.f;
-    float xh[MAXV][8], dg[MAXV][8];
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int i = 0; i < MAXV; ++i) {
-      const int vi = i * LPR + sub;
-      if (live && vi < nvec) {
-        float xv[8], dv[8], g[8];
-        load_row8<TIn>(x + r * C + vi * 8, xv);
-        unpack8(*reinterpret_cast<const uint4*>(dy + r * C + vi * 8), dv);
-        load8f(gamma + vi * 8, g);
-        float4* ab = reinterpret_cast<float4*>(mine + vi * 8);
-        float4* ag = reinterpret_cast<float4*>(mine + C + vi * 8);
-        float4 b0 = ab[0], b1 = ab[1], g0 = ag[0], g1 = ag[1];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          xh[i][j] = (xv[j] - mu) * rs;
-          dg[i][j] = dv[j] * g[j];
-          s1 += dg[i][j];
-          s2 = fmaf(dg[i][j], xh[i][j], s2);
-        }
-        b0.x += dv[0]; b0.y += dv[1]; b0.z += dv[2]; b0.w += dv[3];
-        b1.x += dv[4]; b1.y += dv[5]; b1.z += dv[6]; b1.w += dv[7];
-        g0.x = fmaf(dv[0], xh[i][0], g0.x); g0.y = fmaf(dv[1], xh[i][1], g0.y);
-        g0.z = fmaf(dv[2], xh[i][2], g0.z); g0.w = fmaf(dv[3], xh[i][3], g0.w);
-        g1.x = fmaf(dv[4], xh[i][4], g1.x); g1.y = fmaf(dv[5], xh[i][5], g1.y);
-        g1.z = fmaf(dv[6], xh[i][6], g1.z); g1.w = fmaf(dv[7], xh[i][7], g1.w);
-        ab[0] = b0; ab[1] = b1; ag[0] = g0; ag[1] = g1;
-      }
-    }
-    s1 = group_sum<LPR>(s1) / C;
-    s2 = group_sum<LPR>(s2) / C;
-#pragma unroll
-    for (int i = 0; i < MAXV; ++i) {
-      const int vi = i * LPR + sub;
-      if (live && vi < nvec) {
-        float o[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = rs * (dg[i][j] - s1 - xh[i][j] * s2);
-        if (add != nullptr) {
-          float a[8];
-          load_row8<TOut>(add + r * C + vi * 8, a);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) o[j] += a[j];
-        }
-        store_row8<TOut>(dx + r * C + vi * 8, o);
-      }
-    }
-  }
-  __syncthreads();
-  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) {
-    float s = 0.f;
-    for (int w = 0; w < nw * RPW; ++w) s += red[static_cast<long long>(w) * 2 * C + c];
-    partial[static_cast<long long>(blockIdx.x) * 2 * C + c] = s;
-  }
-}
-
-// Second version of the kernel above (the default; B200_LN_BWD=1 selects the first one), same arguments and results:
-//   * every load of a row - x, dy AND the residual gradient `add` - is issued before anything is computed; the first version
-//     fetched `add` only after the two row reductions, a second exposed DRAM round trip per row with nothing else in flight
-//     (24 warps per SM, one row each: 3.9 TB/s at C = 768).  The raw words stay in registers (x fp32 / dy, add bf16 packed:
-//     the same 48 registers the first version spends on xhat and dy*gamma) and xhat, dy*gamma are simply recomputed for the
-//     output phase - two more FMAs per element;
-//   * the per-warp parameter-gradient accumulators are split into a plane of the low and a plane of the high float4 of every
-//     8-channel vector, so that consecutive lanes touch consecutive 16-byte words (the interleaved layout was a 2-way bank
-//     conflict on every read-modify-write).
-template <typename TIn, typename TOut, int MAXV, int LPR = 32>
-__global__ void __launch_bounds__(256, 3)
-layernorm_bwd2_kernel(const __nv_bfloat16* __restrict__ dy, const TIn* __restrict__ x, const float* __restrict__ mean,
-                      const float* __restrict__ rstd, const float* __restrict__ gamma, const TOut* __restrict__ add,
-                      TOut* __restrict__ dx, float* __restrict__ partial, long long rows, int C) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float red[];  // [warps][rows per warp][2][C], each [C] = low float4 plane | high float4 plane
   constexpr int RPW = 32 / LPR;
@@ -312,7 +229,6 @@ __global__ void patch_merge_ln_fwd_kernel(const float* __restrict__ x, const flo
                                           const float* __restrict__ beta, __nv_bfloat16* __restrict__ y,
                                           float* __restrict__ mean_out, float* __restrict__ rstd_out, int B, int H, int W,
                                           int C, float eps) {
-  pdl_launch_dependents();
   pdl_wait();
   const int lane = threadIdx.x & 31;
   const int C4 = 4 * C, nvec = C4 >> 3, cvec = C >> 3;
@@ -379,7 +295,6 @@ __global__ void __launch_bounds__(256, 2)
 patch_merge_ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
                           const float* __restrict__ rstd, const float* __restrict__ gamma, __nv_bfloat16* __restrict__ dx,
                           float* __restrict__ partial, int B, int H, int W, int C) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float red[];  // [warps][2][4C]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -452,7 +367,6 @@ patch_merge_ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __r
 // (the flattening order of an OIHW conv weight, so the weight matrix is weight.view(D, -1) unchanged). ps % 8 == 0... or 4.
 __global__ void patchify_nchw_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ a, int B, int Cin, int H,
                                      int W, int ps) {
-  pdl_launch_dependents();
   pdl_wait();
   const int ph = H / ps, pw = W / ps;
   const int K = Cin * ps * ps;
@@ -480,7 +394,6 @@ __global__ void patchify_nchw_kernel(const float* __restrict__ x, __nv_bfloat16*
 // ViT class-token row: tokens[b][0][:] = cls[:] + pos[0][:]   (tokens fp32 [B][T][D])
 __global__ void cls_row_kernel(const float* __restrict__ cls, const float* __restrict__ pos, float* __restrict__ tokens,
                                int B, int T, int D) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long total = static_cast<long long>(B) * D;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
@@ -494,7 +407,6 @@ __global__ void cls_row_kernel(const float* __restrict__ cls, const float* __res
 // Strided 2-D copy of 16-byte vectors: dst[r][0:cols] = src[r][0:cols] with independent row pitches (in bytes).
 __global__ void copy_rows_kernel(const uint8_t* __restrict__ src, long long src_pitch, uint8_t* __restrict__ dst,
                                  long long dst_pitch, long long rows, long long row_bytes) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long vecs = row_bytes >> 4;
   const long long total = rows * vecs;
@@ -511,7 +423,6 @@ __global__ void copy_rows_kernel(const uint8_t* __restrict__ src, long long src_
 // through shared memory. (The first version read one bf16 per thread from ~128 blocks: 1 TB/s; this one is HBM bound.)
 __global__ void __launch_bounds__(256) colsum_partial_kernel(const __nv_bfloat16* __restrict__ m, long long rows, long long ld,
                                                              int cols, float* __restrict__ partial) {
-  pdl_launch_dependents();
   pdl_wait();
   __shared__ float sh[256 * 8];
   const int nvec = cols >> 3;                        // cols is a multiple of 8
@@ -571,7 +482,6 @@ __global__ void __launch_bounds__(256) colsum_partial_kernel(const __nv_bfloat16
 template <typename T>
 __global__ void batch_rowsum_kernel(const T* __restrict__ g, long long stride_b, int B, int D, float* __restrict__ out,
                                     int accumulate) {
-  pdl_launch_dependents();
   pdl_wait();
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= D) return;

@@ -66,7 +66,6 @@ constexpr int kWgradThreads = 384;   // warpgroup 0: TMA producer (warp 0), warp
 
 template <int BLOCK_NG, bool kBias = false, bool kGrouped = false>
 __global__ void __launch_bounds__(kWgradThreads, 1) wgrad_gemm_kernel(const __grid_constant__ WgradParams p) {
-  pdl_launch_dependents();
   static_assert(!kGrouped || (BLOCK_NG == 384 && !kBias), "grouped mode: two warpgroups x three 64-column taps");
   using Cfg = WgradCfg<BLOCK_NG>;
   constexpr int NW = kGrouped ? BLOCK_NG / 2 : BLOCK_NG;   // columns of one warpgroup's MMA
@@ -267,7 +266,6 @@ __global__ void __launch_bounds__(256) wgrad_reduce_rows_kernel(const float* __r
                                                                 int splits, int Cout, int Cin, int taps, int chunk, int SL,
                                                                 int accumulate, const float* __restrict__ bias_partial,
                                                                 float* __restrict__ bias_out) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float4 rows_sm4[];
   const int cout = blockIdx.x;
@@ -321,7 +319,6 @@ __global__ void __launch_bounds__(256) wgrad_reduce_rows_kernel(const float* __r
 __global__ void wgrad_reduce_flat_kernel(const float* __restrict__ partial, float* __restrict__ grad, int splits, int Cout,
                                     int Cin, int taps, int accumulate, const float* __restrict__ bias_partial,
                                     float* __restrict__ bias_out) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long total = static_cast<long long>(Cout) * Cin * taps;
   const long long slice = total;
@@ -351,7 +348,6 @@ __global__ void wgrad_reduce_flat_kernel(const float* __restrict__ partial, floa
 // in order (deterministic).
 __global__ void wgrad_reduce_grouped_kernel(const float* __restrict__ partial, float* __restrict__ grad, int splits, int C,
                                             int Cg, int taps, int accumulate) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long total = static_cast<long long>(C) * Cg * taps;
   const long long slice = static_cast<long long>(C) * taps * 64;

@@ -121,7 +121,6 @@ __device__ __forceinline__ uint64_t wdesc(uint32_t addr, uint32_t lbo) { return 
 //   soft-max group g (warpgroup 1 + g) owns the steps with n&1 == g: S = Q K^T -> P (bf16, block diagonal) -> O = P V ->
 //   write out, so the gathers of step n+1 and the two groups' steps overlap.
 __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_fwd_kernel(const WAttnParams p) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -290,7 +289,6 @@ constexpr int kWAttnBwdSmem = kWAttnFwdSmem;
 // accumulator image); each group issues its step's products itself: S = Q K^T, then dP = dO V^T with dV = P^T dO, then
 // dQ = dS K with dK = dS^T Q (block diagonal: only the two 64 x 64 window blocks are multiplied).
 __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WAttnParams p) {
-  pdl_launch_dependents();
   pdl_wait();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -559,7 +557,6 @@ __global__ void __launch_bounds__(kWAttnFwdThreads, 1) wattn_bwd_kernel(const WA
 // rows (one per query) that the soft-max threads read with 13 vector loads.
 __global__ void wattn_bias_gather_kernel(const float* __restrict__ table, const long long* __restrict__ index,
                                          const float* __restrict__ mask, int nWm, float* __restrict__ tab, int nH) {
-  pdl_launch_dependents();
   pdl_wait();
   const long long n = static_cast<long long>(nH) * nWm * kWT * 64;
   for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < n;
@@ -582,7 +579,6 @@ __global__ void wattn_bias_gather_kernel(const float* __restrict__ table, const 
 // dtable[index[i][j]][h] (+)= dbias[h][i][j]   (dtable zeroed / holding the running gradient)
 __global__ void wattn_bias_scatter_kernel(const float* __restrict__ dbias, const long long* __restrict__ index,
                                           float* __restrict__ dtable, int nH) {
-  pdl_launch_dependents();
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nH * kWT * kWT) return;
@@ -599,7 +595,6 @@ __global__ void wattn_bias_scatter_kernel(const float* __restrict__ dbias, const
 template <bool kMerge>
 __global__ void __launch_bounds__(256) window_permute_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, int B, int H,
                                                              int W, int cvec, int shift, int ws) {
-  pdl_launch_dependents();
   pdl_wait();
   const unsigned nWx = W / ws, nWy = H / ws;
   const unsigned total = static_cast<unsigned>(B) * H * W * cvec;

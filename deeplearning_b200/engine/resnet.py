@@ -116,9 +116,6 @@ def _algebra_enabled():
     return os.environ.get("B200_RESNET_ALGEBRA", "1") != "0"
 
 
-_FUSED_REDUCE = os.environ.get("B200_RESNET_FUSED_BN_REDUCE", "1") != "0"
-
-
 def _algebra_ok(block, train, want_tape):
     """Bottleneck whose tail can run with bn3 folded through conv3 (train mode, or a forward that records no tape)."""
     if not _algebra_enabled() or not hasattr(block, "conv3") or not (train or not want_tape):
@@ -335,8 +332,8 @@ def _unit_backward(u, g, grads, want_dz=False):
 
 def _fused_reduce_ok(u):
     """Can the dgrad GEMM that produces the gradient of unit u's output also do the reduce half of u's BN backward?
-    (relu(bn(c)) without a residual, 64-channel multiples; B200_RESNET_FUSED_BN_REDUCE=0 switches it off)"""
-    return _FUSED_REDUCE and u.relu and not u.has_res and u.c.shape[-1] % 64 == 0
+    (relu(bn(c)) without a residual, 64-channel multiples)"""
+    return u.relu and not u.has_res and u.c.shape[-1] % 64 == 0
 
 
 def _unit_backward_from_sums(u, dz, sums, grads):

@@ -3,8 +3,6 @@
 PyTorch is used for device memory and streams only; every arithmetic op below is a hand-written sm_90a kernel.
 Activations are NHWC bf16 tensors ``[B, H, W, C]`` (``[rows, C]`` for linear layers); parameters and statistics fp32.
 """
-import os
-
 import torch
 
 from . import _lib
@@ -472,21 +470,14 @@ def bn_backward_from_sums(dz, partial, x, co, dgamma=None, dbeta=None, sync=None
 
 
 # ------------------------------------------------------------------------------ BatchNorm folded through a 1x1 convolution
-_GRAM_BIAS_SUM = os.environ.get("B200_GRAM_BIAS_SUM", "1") != "0"
-
-
 def gram_colsum(y2):
     """y2 bf16 [..., K] -> (G = y2^T y2 fp32 [K, K], s = column sums fp32 [K]): everything train-mode BatchNorm needs to know
     about the output of a 1x1 convolution of y2 (csrc/bn_algebra.cuh)."""
     K = y2.shape[-1]
     flat = y2.view(-1, 1, 1, K)
-    if _GRAM_BIAS_SUM:
-        # the column sums come from the tiles the Gram kernel already stages (its bias-gradient warps): no second pass over y2
-        s = torch.empty(K, dtype=F32, device=y2.device)
-        G = conv2d_wgrad(flat, flat, bias_out=s).view(K, K)
-        return G, s
-    G = conv2d_wgrad(flat, flat).view(K, K)
-    s = colsum_tall(y2.view(-1, K))
+    # the column sums come from the tiles the Gram kernel already stages (its bias-gradient warps): no second pass over y2
+    s = torch.empty(K, dtype=F32, device=y2.device)
+    G = conv2d_wgrad(flat, flat, bias_out=s).view(K, K)
     return G, s
 
 

@@ -87,14 +87,9 @@ def _train_step_check(layers, B, hw, grad_slack, kw=X32):
 
 
 @pytest.mark.parametrize("algebra", ["0", "1"])
-@pytest.mark.parametrize("fused", [False, True])
-def test_resnext_shallow_train_step_parity(monkeypatch, algebra, fused):
-    """[1,1,1,1] ResNeXt 32x4d at bs 32, 128x128, on both bottleneck-tail schedules and with / without the BN-backward reduce
-    fused into the grouped dgrad"""
-    from deeplearning_b200.engine import resnet as engine
-
+def test_resnext_shallow_train_step_parity(monkeypatch, algebra):
+    """[1,1,1,1] ResNeXt 32x4d at bs 32, 128x128, on both bottleneck-tail schedules"""
     monkeypatch.setenv("B200_RESNET_ALGEBRA", algebra)
-    monkeypatch.setattr(engine, "_FUSED_REDUCE", fused)
     _train_step_check((1, 1, 1, 1), 32, 128, grad_slack=2.0)
 
 

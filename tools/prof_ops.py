@@ -134,7 +134,7 @@ def vit_fc2_dgrad():  # d_pre = (g W2) * saved GELU'(pre) with column sums (fc1 
     return lambda: ops.gemm(g, wd, act=3, aux_in=pre, want_stats=True)
 
 
-def vit_ln_bwd():      # ViT-B/16 LayerNorm backward: x fp32 [50432, 768], dy / residual gradient bf16 (layernorm_bwd2_kernel)
+def vit_ln_bwd():      # ViT-B/16 LayerNorm backward: x fp32 [50432, 768], dy / residual gradient bf16 (layernorm_bwd_kernel)
     x = rnd(256 * 197, 768, dtype=torch.float32)
     g = torch.rand(768, device=dev) + 0.5
     y, mean, rstd = ops.layernorm_fwd(x, g, torch.zeros(768, device=dev), 1e-6)

@@ -80,7 +80,7 @@ _SPANS = {"wgrad_gemm": ("wgrad_gemm_kernel", "wgrad_reduce_rows_kernel", "wgrad
           "bn_apply": ("bn_apply_kernel",), "attention_fwd": ("attn_fwd2_kernel",),
           "attention_bwd": ("attn_bwd_kernel", "attn_delta_kernel"),
           "window_attention_fwd": ("wattn_fwd_kernel",), "window_attention_bwd": ("wattn_bwd_kernel",),
-          "layernorm_fwd": ("layernorm_fwd_kernel",), "layernorm_bwd": ("layernorm_bwd_kernel", "layernorm_bwd2_kernel"),
+          "layernorm_fwd": ("layernorm_fwd_kernel",), "layernorm_bwd": ("layernorm_bwd_kernel",),
           "dwconv7": ("dwconv7_tile_kernel", "dwconv7_kernel"), "dwconv7_wgrad": ("dwconv7_wgrad_tile_kernel",)}
 
 

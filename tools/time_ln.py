@@ -1,5 +1,5 @@
 """Time LayerNorm backward alone at the shapes of the three transformer-style families (CUDA events; ops.Profiler spans so that
-the finalize launch is not counted).  B200_LN_BWD=1 selects the first kernel version.
+the finalize launch is not counted).
 python tools/time_ln.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -27,4 +27,4 @@ for name, rows, C, xdt, has_add in CASES:
     ts = [e0.elapsed_time(e1) * 1e3 for (n, fl, nb, e0, e1) in prof.records if n == "layernorm_bwd"]
     nbytes = x.numel() * x.element_size() + dy.numel() * 2 * (3 if has_add else 2)
     t = sorted(ts)[len(ts) // 2]
-    print(f"layernorm_bwd v{os.environ.get('B200_LN_BWD', '2')} {name:22s} rows {rows:7d} C {C:4d}: {t:7.1f} us  {nbytes / t / 1e6:6.2f} TB/s")
+    print(f"layernorm_bwd {name:22s} rows {rows:7d} C {C:4d}: {t:7.1f} us  {nbytes / t / 1e6:6.2f} TB/s")
