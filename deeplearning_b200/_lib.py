@@ -131,6 +131,12 @@ SIGNATURES = {
     "b200_tanh_fwd": (_I, [_P, _P, _P, _L, _P]),
     "b200_tanh_bwd": (_I, [_P, _P, _P, _L, _P]),
     "b200_sgd_momentum": (_I, [_P, _P, _P, _L, _F, _P, _F, _F, _F, _I, _P, _P]),
+    "b200_se_squeeze": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "b200_se_excite": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "b200_se_apply": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "b200_se_bwd_reduce": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "b200_se_bwd_coeffs": (_I, [_P] * 12 + [_I, _I, _I, _I] + [_P] * 9),
+    "b200_se_bwd_apply": (_I, [_P] * 10 + [_I, _I, _I, _P]),
 }
 
 

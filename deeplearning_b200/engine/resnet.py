@@ -18,6 +18,14 @@ conv3 output is never written, normalised or re-read -
 
 which removes the bn3 apply pass of the forward and both bn3 passes (reduce, apply) of the backward: 8 of the 17 passes a
 bottleneck makes over its block-width tensors.  ``B200_RESNET_ALGEBRA=0`` selects the plain conv -> BN pass schedule.
+
+A block with an ``se`` module (SEBottleneck / SEBasicBlock, classification/seNet/models/se_resnet.py:74-84 / :32-42) runs its
+last unit as a squeeze-and-excitation tail (csrc/se.cuh) on the pass schedule under both settings:
+
+    forward   c = conv(x) (+ statistics)  ->  squeeze: pool = mean_p bn(c)  ->  excite: gate = sigmoid(W2 relu(W1 pool))
+              ->  y = relu(bn(c) * gate + identity)
+    backward  reduce: dz = g * [y > 0], per-image sums of dz and dz * c  ->  SE / BN coefficients (dW1, dW2, dgamma, dbeta)
+              ->  dc = BatchNorm backward of du = dz * gate + dpool / HW
 """
 import os
 
@@ -109,7 +117,7 @@ class _Unit:
     """Saved state of one conv -> BN (-> ReLU) (-> + residual) application.  ``algebra`` units (bottleneck conv3 with the
     BatchNorm folded through the convolution) have no raw conv output ``c``; they keep the Gram matrix ``G`` and the column
     sums ``s`` of their input instead."""
-    __slots__ = ("conv", "bn", "x", "c", "co", "y", "relu", "has_res", "algebra", "G", "s")
+    __slots__ = ("conv", "bn", "x", "c", "co", "y", "relu", "has_res", "algebra", "G", "s", "se")
 
 
 def _algebra_enabled():
@@ -119,6 +127,8 @@ def _algebra_enabled():
 def _algebra_ok(block, train, want_tape):
     """Bottleneck whose tail can run with bn3 folded through conv3 (train mode, or a forward that records no tape)."""
     if not _algebra_enabled() or not hasattr(block, "conv3") or not (train or not want_tape):
+        return False
+    if getattr(block, "se", None) is not None:   # the SE gate needs sum_p dz * u per image, hence the raw conv output
         return False
     if isinstance(block.bn3, nn.SyncBatchNorm) and train:
         return False
@@ -207,6 +217,50 @@ def _conv_bn(pack, tape, x, conv, bn, train, relu, residual=None, name=""):
     return y
 
 
+def _check_se(se, C, name):
+    """SELayer(C, reduction) of the reference (classification/seNet/models/se_module.py:4-19): avg_pool, then
+    fc = Linear(C, Cr, bias=False), ReLU, Linear(Cr, C, bias=False), Sigmoid, with C % 64 == 0 and 1 <= Cr <= 256."""
+    fc, pool = getattr(se, "fc", None), getattr(se, "avg_pool", None)
+    ok = (isinstance(pool, nn.AdaptiveAvgPool2d) and pool.output_size in (1, (1, 1))
+          and isinstance(fc, nn.Sequential) and len(fc) == 4 and type(fc[0]) is nn.Linear and isinstance(fc[1], nn.ReLU)
+          and type(fc[2]) is nn.Linear and isinstance(fc[3], nn.Sigmoid) and fc[0].bias is None and fc[2].bias is None)
+    if ok:
+        Cr = fc[0].out_features
+        ok = (fc[0].in_features == C and fc[2].out_features == C and fc[2].in_features == Cr and C % 64 == 0
+              and 1 <= Cr <= 256)
+    if not ok:
+        raise NotImplementedError(f"{name}: the GPU engine runs SELayer(C, reduction) as avg_pool -> Linear(C, Cr, bias=False) "
+                                  f"-> ReLU -> Linear(Cr, C, bias=False) -> Sigmoid with C % 64 == 0 and 1 <= Cr <= 256 "
+                                  f"on a {C}-channel tail (got {se})")
+
+
+def _conv_bn_se(pack, tape, x, conv, bn, se, train, identity, name=""):
+    """SE tail ``out = relu(bn(conv(x)) * gate + identity)``, gate = se(bn(conv(x))): conv (+ statistics) -> squeeze ->
+    excite -> gated apply.  Eval mode runs the same kernels with the running-statistics coefficients."""
+    _check_conv(conv, name)
+    _check_bn(bn, name)
+    _check_se(se, conv.out_channels, name)
+    if train and _bn_sync(bn) is not None:
+        raise NotImplementedError(f"{name}: SyncBatchNorm in front of a squeeze-and-excitation gate is not implemented")
+    wp = pack.get(conv.weight, _pack_modes(conv)[0])
+    c, st = ops.conv2d_fwd(x, wp, conv.kernel_size[0], conv.stride[0], want_stats=train, groups=conv.groups)
+    if train:
+        co = ops.bn_finalize(st, c.numel() // c.shape[-1], bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean,
+                             bn.running_var, bn.num_batches_tracked)
+    else:
+        co = ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+    csum, pool = ops.se_squeeze(c, co)
+    h, gate = ops.se_excite(pool, se.fc[0].weight, se.fc[2].weight)
+    y = ops.se_apply(c, co, gate, identity)
+    if tape is not None:
+        u = _Unit()
+        u.conv, u.bn, u.x, u.c, u.co, u.y, u.relu, u.has_res = conv, bn, x, c, co, y, True, True
+        u.algebra, u.G, u.s = False, None, None
+        u.se = (se, csum, pool, h, gate)
+        tape.append(u)
+    return y
+
+
 def _algebra_ok_dgrad(conv1):
     return (conv1.kernel_size == (1, 1) and conv1.stride == (1, 1) and conv1.in_channels % 64 == 0
             and conv1.out_channels % 64 == 0)
@@ -275,7 +329,10 @@ def forward(model, x, train, want_tape):
             else:
                 identity = x_in
             conv, bn = pairs[-1]
-            if _algebra_ok(block, train, want_tape):
+            se = getattr(block, "se", None)
+            if se is not None:
+                h = _conv_bn_se(pack, units, h, conv, bn, se, train, identity, name=f"{name}.conv{len(pairs)}")
+            elif _algebra_ok(block, train, want_tape):
                 _check_conv(conv, f"{name}.conv3")
                 h = _conv3_bn_res_relu(pack, units, h, conv, bn, train, identity, name=f"{name}.conv3")
             else:
@@ -325,6 +382,21 @@ def _unit_backward(u, g, grads, want_dz=False):
     dc, dgamma, dbeta, dz = ops.bn_backward(g, u.c, u.co, relu=u.relu, y_out=u.y if (u.relu and u.has_res) else None,
                                             want_dz=want_dz, dgamma=grads.dest(u.bn.weight), dbeta=grads.dest(u.bn.bias),
                                             sync=_bn_sync(u.bn))
+    grads.put(u.bn.weight, dgamma)
+    grads.put(u.bn.bias, dbeta)
+    return dc, dz
+
+
+def _se_unit_backward(u, g, grads):
+    """Backward of an SE tail for the gradient g of its output; returns (dc, dz) like _unit_backward(want_dz=True) and
+    records the gradients of the BatchNorm and of both SE weights."""
+    se, csum, pool, h, gate = u.se
+    w1, w2 = se.fc[0].weight, se.fc[2].weight
+    dc, dz, dw1, dw2, dgamma, dbeta = ops.se_backward(
+        g, u.y, u.c, u.co, csum, pool, h, gate, w1, w2, dw1=grads.dest(w1), dw2=grads.dest(w2),
+        dgamma=grads.dest(u.bn.weight), dbeta=grads.dest(u.bn.bias))
+    grads.put(w2, dw2)
+    grads.put(w1, dw1)
     grads.put(u.bn.weight, dgamma)
     grads.put(u.bn.bias, dbeta)
     return dc, dz
@@ -406,6 +478,9 @@ def backward(model, tape, dlogits, sink=None):
                 g_prev = ops.gemm_dual(dz, y2, wcat, wbias)
                 dc, _ = _unit_backward(u2, g_prev, grads)
             first = len(units) - 2
+        elif getattr(last, "se", None) is not None:
+            dc, dz = _se_unit_backward(last, g, grads)
+            first = len(units) - 1
         else:
             # out = relu(bn_last(c) + identity): dz is the gradient of the pre-ReLU sum, shared by both branches
             dc, dz = _unit_backward(last, g, grads, want_dz=True)

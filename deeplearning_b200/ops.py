@@ -469,6 +469,104 @@ def bn_backward_from_sums(dz, partial, x, co, dgamma=None, dbeta=None, sync=None
     return dx, dgamma, dbeta
 
 
+# ------------------------------------------------------------------------------ squeeze-and-excitation tail (csrc/se.cuh)
+def _f32_param(w):
+    w = w.detach()
+    return w if (w.dtype == F32 and w.is_contiguous()) else w.float().contiguous()
+
+
+def se_squeeze(c, co):
+    """c: raw conv output bf16 [B,H,W,C]; co: BnCoeffs of the BatchNorm after it.  Returns (csum, pool), fp32 [B, C]:
+    per-image channel sums of c and the mean of u = c * scale + shift (SELayer.avg_pool of the BatchNorm output)."""
+    lib = _lib.load()
+    _chk_act(c, "c")
+    B, H, W, C = c.shape
+    out = torch.empty(2, B, C, dtype=F32, device=c.device)
+    sp = _span("se_squeeze", float(c.numel()), _nb(c, out))
+    rc = lib.b200_se_squeeze(_p(c), _p(co.scale), _p(co.shift), _p(out[0]), _p(out[1]), B, H * W, C, _stream())
+    _lib.check(rc, "b200_se_squeeze")
+    if sp:
+        sp.end()
+    return out[0], out[1]
+
+
+def se_excite(pool, w1, w2):
+    """SELayer.fc on fp32 [B, C]: h = relu(pool w1^T) [B, Cr], gate = sigmoid(h w2^T) [B, C] (w1 [Cr, C], w2 [C, Cr])."""
+    lib = _lib.load()
+    w1, w2 = _f32_param(w1), _f32_param(w2)
+    B, C = pool.shape
+    Cr = w1.shape[0]
+    if tuple(w1.shape) != (Cr, C) or tuple(w2.shape) != (C, Cr):
+        raise ValueError(f"se_excite: weights {tuple(w1.shape)} / {tuple(w2.shape)} do not match C={C}")
+    h = torch.empty(B, Cr, dtype=F32, device=pool.device)
+    gate = torch.empty(B, C, dtype=F32, device=pool.device)
+    sp = _span("se_excite", 4.0 * B * C * Cr, _nb(pool, w1, w2, h, gate))
+    _lib.check(lib.b200_se_excite(_p(pool), _p(w1), _p(w2), _p(h), _p(gate), B, C, Cr, _stream()), "b200_se_excite")
+    if sp:
+        sp.end()
+    return h, gate
+
+
+def se_apply(c, co, gate, identity):
+    """y = relu((c * scale + shift) * gate[b] + identity), bf16 [B,H,W,C]: bn_apply with a per-(image, channel) multiplier."""
+    lib = _lib.load()
+    _chk_act(c, "c")
+    _chk_act(identity, "identity")
+    B, H, W, C = c.shape
+    y = torch.empty_like(c)
+    sp = _span("se_apply", 0.0, _nb(c, identity, y))
+    rc = lib.b200_se_apply(_p(c), _p(identity), _p(y), _p(co.scale), _p(co.shift), _p(gate), B, H * W, C, _stream())
+    _lib.check(rc, "b200_se_apply")
+    if sp:
+        sp.end()
+    return y
+
+
+def se_backward(g, y, c, co, csum, pool, h, gate, w1, w2, dw1=None, dw2=None, dgamma=None, dbeta=None):
+    """Backward of y = relu(bn(c) * gate + identity) with the SE gate (train-mode BatchNorm), for g = dL/dy.
+    Returns (dc, dz, dw1, dw2, dgamma, dbeta): dc = dL/dc, dz = dL/d(identity) (bf16); the four parameter gradients are
+    written into the given buffers when passed (not accumulated)."""
+    lib = _lib.load()
+    _chk_act(g, "g")
+    w1, w2 = _f32_param(w1), _f32_param(w2)
+    B, H, W, C = c.shape
+    HW, Cr = H * W, w1.shape[0]
+    dev = c.device
+    dz = torch.empty_like(c)
+    sums = torch.empty(2, B, C, dtype=F32, device=dev)
+    sp = _span("se_bwd_reduce", 0.0, _nb(g, y, c, dz))
+    rc = lib.b200_se_bwd_reduce(_p(g), _p(y), _p(c), _p(dz), _p(sums[0]), _p(sums[1]), B, HW, C, _stream())
+    _lib.check(rc, "b200_se_bwd_reduce")
+    if sp:
+        sp.end()
+    if dw1 is None:
+        dw1 = torch.empty(Cr, C, dtype=F32, device=dev)
+    if dw2 is None:
+        dw2 = torch.empty(C, Cr, dtype=F32, device=dev)
+    if dgamma is None:
+        dgamma = torch.empty(C, dtype=F32, device=dev)
+    if dbeta is None:
+        dbeta = torch.empty(C, dtype=F32, device=dev)
+    dh = torch.empty(B, Cr, dtype=F32, device=dev)
+    dp = torch.empty(B, C, dtype=F32, device=dev)
+    m = torch.empty(2, C, dtype=F32, device=dev)
+    sp = _span("se_bwd_coeffs", 8.0 * B * C * Cr)
+    rc = lib.b200_se_bwd_coeffs(_p(sums[0]), _p(sums[1]), _p(csum), _p(pool), _p(h), _p(gate), _p(w1), _p(w2), _p(co.scale),
+                                _p(co.shift), _p(co.mean), _p(co.invstd), B, HW, C, Cr, _p(dh), _p(dp), _p(dw1), _p(dw2),
+                                _p(dgamma), _p(dbeta), _p(m[0]), _p(m[1]), _stream())
+    _lib.check(rc, "b200_se_bwd_coeffs")
+    if sp:
+        sp.end()
+    dc = torch.empty_like(c)
+    sp = _span("se_bwd_apply", 0.0, _nb(dz, c, dc))
+    rc = lib.b200_se_bwd_apply(_p(dz), _p(c), _p(dc), _p(gate), _p(dp), _p(co.scale), _p(co.mean), _p(co.invstd), _p(m[0]),
+                               _p(m[1]), B, HW, C, _stream())
+    _lib.check(rc, "b200_se_bwd_apply")
+    if sp:
+        sp.end()
+    return dc, dz, dw1, dw2, dgamma, dbeta
+
+
 # ------------------------------------------------------------------------------ BatchNorm folded through a 1x1 convolution
 def gram_colsum(y2):
     """y2 bf16 [..., K] -> (G = y2^T y2 fp32 [K, K], s = column sums fp32 [K]): everything train-mode BatchNorm needs to know

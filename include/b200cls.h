@@ -386,6 +386,38 @@ int b200_rowscale_bf16(const void* x, const float* scale, void* y, long long n_s
 int b200_tanh_fwd(const float* u, float* t, void* t_bf16, long long n, void* stream);
 int b200_tanh_bwd(const void* dt_bf16, const float* t, void* du_bf16, long long n, void* stream);
 
+/* ---- squeeze-and-excitation tail of an SE-ResNet block: SELayer (classification/seNet/models/se_module.py:15-19) between
+ * the last BatchNorm and the residual add of SEBottleneck / SEBasicBlock (se_resnet.py:74-84 / :32-42):
+ *     y = relu(u * gate[b][ch] + identity),  u = c * scale + shift,  gate = sigmoid(W2 relu(W1 mean_p(u)))
+ * c bf16 [B][HW][C] is the raw conv output, scale / shift the BatchNorm coefficients (batch statistics in train mode, running
+ * statistics in eval mode); per-image vectors are fp32 [B][C] (csum, pool, gate, A, R, dp) or [B][Cr] (h, dh); w1 = fc.0.weight
+ * fp32 [Cr][C], w2 = fc.2.weight fp32 [C][Cr].  Scope: C % 64 == 0, 1 <= Cr <= 256, HW >= 1, 1 <= B <= 65535; other shapes
+ * return B200_EINVAL with a message and launch nothing.  All sums are fp32 in a fixed order (no atomics).
+ * forward:  squeeze  csum = sum_p c, pool = csum / HW * scale + shift          (one read of c)
+ *           excite   h = relu(pool w1^T), gate = sigmoid(h w2^T)               (two small launches, fp32 CUDA cores)
+ *           apply    y = relu(u * gate + identity)                              (one read of c and identity, one write of y)
+ * backward (g = dL/dy):
+ *           reduce   dz = g * [y > 0] (bf16, the identity branch's gradient), A = sum_p dz, R = sum_p dz * c
+ *           coeffs   da = (scale R + shift A) gate (1 - gate), dW2 = da^T h, dh = (da w2) [h > 0], dW1 = dh^T pool,
+ *                    dp = dh w1, dbeta = sum_b (gate A + dp), dgamma = invstd (sum_b (gate R + dp csum / HW) - mean dbeta),
+ *                    m1 = dbeta / M, m2 = dgamma / M (M = B HW); dw1, dw2, dgamma, dbeta are written, not accumulated
+ *           apply    dc = scale (dz gate + dp / HW - m1 - (c - mean) invstd m2)  (bf16) */
+int b200_se_squeeze(const void* c, const float* scale, const float* shift, float* csum, float* pool, int B, int HW, int C,
+                    void* stream);
+int b200_se_excite(const float* pool, const float* w1, const float* w2, float* h, float* gate, int B, int C, int Cr,
+                   void* stream);
+int b200_se_apply(const void* c, const void* identity, void* y, const float* scale, const float* shift, const float* gate,
+                  int B, int HW, int C, void* stream);
+int b200_se_bwd_reduce(const void* g, const void* y, const void* c, void* dz, float* A, float* R, int B, int HW, int C,
+                       void* stream);
+int b200_se_bwd_coeffs(const float* A, const float* R, const float* csum, const float* pool, const float* h,
+                       const float* gate, const float* w1, const float* w2, const float* scale, const float* shift,
+                       const float* mean, const float* invstd, int B, int HW, int C, int Cr, float* dh, float* dp,
+                       float* dw1, float* dw2, float* dgamma, float* dbeta, float* m1, float* m2, void* stream);
+int b200_se_bwd_apply(const void* dz, const void* c, void* dc, const float* gate, const float* dp, const float* scale,
+                      const float* mean, const float* invstd, const float* m1, const float* m2, int B, int HW, int C,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
