@@ -50,6 +50,16 @@ CONV_CASES = [
     (2, 28, 28, 64, 128, 1, 2),
     (1, 9, 11, 64, 64, 3, 1),
     (1, 10, 6, 64, 64, 3, 2),
+    # odd grids into stride-2 layers (the phase views of the 3x3/s2 dgrad have different row counts): ResNet at 196 px reads
+    # 49 x 49, 25 x 25 and 13 x 13 in the first blocks of layer2, layer3 and layer4
+    (2, 49, 49, 128, 128, 3, 2),
+    (2, 25, 25, 256, 256, 3, 2),
+    (2, 13, 13, 512, 512, 3, 2),
+    (2, 49, 49, 256, 512, 1, 2),
+    (2, 25, 25, 512, 1024, 1, 2),
+    (2, 13, 13, 1024, 2048, 1, 2),
+    (3, 13, 8, 64, 64, 3, 2),
+    (3, 9, 14, 64, 128, 1, 2),
 ]
 
 
@@ -210,6 +220,54 @@ def test_softmax_xent_and_sgd():
         opt.step()
         ops.sgd_momentum_(p, g, buf, 0.1, 0.9, 5e-5, first_step=(step == 0))
     _close(p, pr.detach(), 1e-5, 1e-6, "sgd")
+    # the graph-friendly form: the learning rate read from device memory (the host argument is ignored), the gradient scaled by
+    # gscale and a global-norm clip coefficient; gradient norms below and above max_norm; against torch.optim on float64 copies
+    p = torch.randn(n, device="cuda")
+    buf = torch.zeros(n, device="cuda")
+    lr_dev = torch.empty(1, device="cuda")
+    pd = p.double().clone().requires_grad_(True)
+    opt = torch.optim.SGD([pd], lr=1.0, momentum=0.9, weight_decay=5e-5)
+    for step in range(4):
+        g = torch.randn(n, device="cuda") * (step + 1)
+        lr = 0.1 / (step + 1)
+        lr_dev.fill_(lr)
+        clip = ops.grad_clip_coef(g, 300.0, gscale=0.5)
+        ops.sgd_momentum_(p, g, buf, 123.0, 0.9, 5e-5, gscale=0.5, first_step=(step == 0), lr_dev=lr_dev, clip=clip)
+        norm = 0.5 * g.double().norm()
+        pd.grad = g.double() * 0.5 * torch.clamp(300.0 / (norm + 1e-6), max=1.0)
+        opt.param_groups[0]["lr"] = lr
+        opt.step()
+    _close(p, pd.detach(), 1e-5, 1e-6, "sgd lr_dev / clip")
+    # N not a multiple of 8: the padding columns [N, ld_d) of dlogits are exact zeros (the head's dgrad GEMM reads them);
+    # loss_scale multiplies the gradient only; logits of magnitude 1e4 (against a float64 reference)
+    from deeplearning_b200 import _lib
+
+    lib = _lib.load()
+    B, N, ld_d, loss_scale = 13, 1001, 1016, 0.25
+    labels = torch.randint(0, N, (B,), device="cuda")
+    for mag in (3.0, 1e4):
+        logits = torch.randn(B, N, device="cuda") * mag
+        rows = torch.empty(B, device="cuda")
+        correct = torch.empty(B, dtype=torch.int32, device="cuda")
+        d = torch.full((B, ld_d), float("nan"), dtype=torch.bfloat16, device="cuda")
+        gscale = loss_scale / B
+        rc = lib.b200_softmax_xent(logits.data_ptr(), logits.stride(0), labels.data_ptr(), B, N, gscale, rows.data_ptr(),
+                                   d.data_ptr(), ld_d, correct.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        _lib.check(rc, "b200_softmax_xent")
+        assert torch.equal(d[:, N:], torch.zeros(B, ld_d - N, dtype=torch.bfloat16, device="cuda"))
+        ld64 = logits.double()
+        lse = torch.logsumexp(ld64, 1)
+        x_lab = ld64.gather(1, labels[:, None])[:, 0]
+        ref_rows = lse - x_lab
+        err = (rows.double() - ref_rows).abs()
+        assert bool((err <= 2.0 ** -22 * (ld64.abs().amax(1) + x_lab.abs()) + 1e-6).all()), float(err.max())
+        ref_d = (torch.softmax(ld64, 1) - F.one_hot(labels, N).double()) * gscale
+        bound = 2.0 ** -8 * ref_d.abs() + 2.0 ** -18 * gscale
+        assert bool(((d[:, :N].double() - ref_d).abs() <= bound).all()), f"dlogits at |logits| ~ {mag}"
+        assert torch.equal(correct.bool(), logits.argmax(1) == labels)
+        loss, d2, _ = ops.softmax_xent(logits, labels, loss_scale=loss_scale)
+        assert abs(float(loss) - float(ref_rows.mean())) <= 2.0 ** -21 * float((ld64.abs().amax(1) + x_lab.abs()).mean()) + 1e-6
+        assert torch.equal(d2, d[:, :d2.shape[1]])
 
 
 def test_stem_im2col():

@@ -118,6 +118,14 @@ def test_resnet50_train_step_parity():
     _train_step_check((3, 4, 6, 3), 64, 224, grad_slack=2.0)
 
 
+@pytest.mark.parametrize("layers", [(1, 1, 1, 1), (3, 4, 6, 3)])
+def test_resnet_odd_grid_train_step_parity(layers):
+    """196 px: the max-pool output is 49 x 49, so the stride-2 layers of layer2, layer3 and layer4 (3x3 forward, wgrad and the
+    phase-split dgrad; layer2.0's downsample on the compact even-pixel grid, layer3.0 / layer4.0's plain 1x1/s2 conv) read
+    odd grids: 49, 25 and 13"""
+    _train_step_check(layers, 32, 196, grad_slack=2.0)
+
+
 def test_resnet50_head_surgery_and_small_classes():
     """model.fc = nn.Linear(2048, 5) as the reference fine-tune script does (classification/resnet/train.py:79-80)."""
     m, _ = _models()

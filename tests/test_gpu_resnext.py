@@ -93,6 +93,11 @@ def test_resnext_shallow_train_step_parity(monkeypatch, algebra):
     _train_step_check((1, 1, 1, 1), 32, 128, grad_slack=2.0)
 
 
+def test_resnext_shallow_odd_grid_train_step_parity():
+    """196 px: the grouped 3x3/s2 and the downsample convolutions of layer2 .. layer4 read 49 x 49, 25 x 25 and 13 x 13 grids"""
+    _train_step_check((1, 1, 1, 1), 32, 196, grad_slack=2.0)
+
+
 def test_resnext50_train_step_parity():
     _train_step_check((3, 4, 6, 3), 64, 224, grad_slack=2.0)
 

@@ -93,6 +93,11 @@ def test_senet_shallow_train_step_parity(monkeypatch, algebra):
     _train_step_check((1, 1, 1, 1), 32, 128)
 
 
+def test_senet_shallow_odd_grid_train_step_parity():
+    """196 px: the stride-2 layers of layer2 .. layer4 read 49 x 49, 25 x 25 and 13 x 13 grids"""
+    _train_step_check((1, 1, 1, 1), 32, 196)
+
+
 def test_se_resnet50_train_step_parity():
     _train_step_check((3, 4, 6, 3), 64, 224)
 
