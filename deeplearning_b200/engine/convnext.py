@@ -1,4 +1,4 @@
-"""Forward / backward schedule of the ConvNeXt family on the sm_90a kernels (one autograd.Function for the whole network).
+"""Forward / backward schedule of the ConvNeXt family on the sm_90a kernels (one autograd node for the whole network).
 
 Mirrors ``ConvNeXt.forward_features`` / ``Block.forward`` of the reference (classification/convNext/models/networks.py:160-170,
 :92-105).  The residual stream ``x`` is fp32 NHWC; everything feeding a tensor core is bf16:
@@ -15,15 +15,16 @@ so the pre-scale activation is never stored.  Stochastic depth (``drop_path``, r
 multiplier of engine/droppath.py scales the branch in the pwconv2 epilogue (before the shortcut add) and the gradient
 entering the branch in the backward pass.
 """
+import sys
 import weakref
 
 import torch
 import torch.nn as nn
 
 from .. import ops
-from . import droppath
+from . import common, droppath
+from .common import linear_grads, layernorm_backward
 from .packing import weight_cache
-from .resnet import _Grads
 
 BF16 = torch.bfloat16
 F32 = torch.float32
@@ -52,11 +53,7 @@ class _PackSpec:
                 specs.append((w2, 0, w2.shape[1], w2.shape[0]))
                 # dgrad operand of pwconv2 with the layer scale folded in: [4C][C] * gamma[c]
                 specs.append((w2, 1, w2.shape[0], w2.shape[1], None, blk.gamma))
-        head = model.head
-        n_pad = (head.out_features + 7) // 8 * 8
-        specs.append((head.weight, 0, head.in_features, n_pad))
-        specs.append((head.weight, 1, n_pad, head.in_features))
-        return specs
+        return specs + common.head_pack_specs(model.head)
 
 
 _pack_spec = _PackSpec()
@@ -91,9 +88,7 @@ _dw_cache = _DwCache()
 
 def forward(model, x, train, want_tape):
     _check(model)
-    if x.dtype == torch.uint8:      # GPU input pipeline: decoded uint8 NHWC batch -> ToTensor + Normalize on the device
-        x = ops.normalize_u8_nhwc(x, *getattr(model, "input_norm", (ops.IMAGENET_MEAN, ops.IMAGENET_STD)))
-    x = x.contiguous().float()
+    x = common.image_input(model, x)
     B = x.shape[0]
     pack = weight_cache.model_pack(model, _pack_spec)
     tape = {"stages": [], "pack": pack} if want_tape else None
@@ -132,69 +127,18 @@ def forward(model, x, train, want_tape):
     # ---- head
     pooled = ops.avgpool_any(h)                                    # fp32 [B, C]
     yc, mc, rc = ops.layernorm_fwd(pooled, model.norm.weight, model.norm.bias, model.norm.eps)
-    head = model.head
-    n_cls = head.out_features
-    n_pad = (n_cls + 7) // 8 * 8
-    bias = None
-    if head.bias is not None:
-        bias = head.bias.detach()
-        if n_pad != n_cls:
-            bias = torch.cat([bias, bias.new_zeros(n_pad - n_cls)])
-    D = pooled.shape[1]
-    logits, _ = ops.conv2d_fwd(yc.view(B, 1, 1, D), pack.get(head.weight, 0), bias=bias, out_f32=True)
-    logits = logits.view(B, n_pad)
+    logits = common.head_forward(pack, model.head, yc)
     if want_tape:
-        tape["head"] = (pooled, yc, mc, rc, n_cls, n_pad, tuple(h.shape))
-    return (logits[:, :n_cls] if n_pad != n_cls else logits), tape
-
-
-def _lin_wgrad(grads, lin, dy2d, x2d, dy_stats=None):
-    M, N = dy2d.shape
-    K = x2d.shape[1]
-    dst = grads.dest(lin.weight)
-    gb = None
-    if lin.bias is not None and dy_stats is None:
-        gb = grads.dest(lin.bias)      # bias gradient summed inside the wgrad kernel (no pass over dy)
-        if gb is None:
-            gb = torch.empty(N, dtype=F32, device=dy2d.device)
-    gw = ops.conv2d_wgrad(dy2d.view(M, 1, 1, N), x2d.view(M, 1, 1, K), out=dst.view(N, K, 1, 1) if dst is not None else None,
-                          bias_out=gb)
-    grads.put(lin.weight, gw)
-    if lin.bias is not None:
-        if dy_stats is not None:   # column sums already produced by the epilogue of the GEMM that wrote dy
-            grads.put(lin.bias, ops.stats_colsum(dy_stats, out=grads.dest(lin.bias)))
-        else:
-            grads.put(lin.bias, gb)
+        tape["head"] = (pooled, yc, mc, rc, tuple(h.shape))
+    return logits, tape
 
 
 def backward(model, tape, dlogits, sink=None):
-    grads = _Grads(sink)
+    grads = common.Grads(sink)
     pack = tape["pack"]
-    pooled, yc, mc, rc, n_cls, n_pad, (B, Hf, Wf, Cf) = tape["head"]
-    head = model.head
-    if dlogits.dtype == BF16 and dlogits.shape[1] == n_pad and dlogits.is_contiguous():
-        dl16 = dlogits
-    else:
-        dl = dlogits.contiguous().float()
-        if n_pad != n_cls:
-            dl = torch.cat([dl, dl.new_zeros(B, n_pad - n_cls)], 1).contiguous()
-        dl16 = ops.cast_bf16(dl)
-    dst = grads.dest(head.weight)
-    if dst is not None and n_pad == n_cls:
-        grads.put(head.weight, ops.conv2d_wgrad(dl16.view(B, 1, 1, n_pad), yc.view(B, 1, 1, Cf), out=dst.view(n_cls, Cf, 1, 1)))
-    else:
-        gw = ops.conv2d_wgrad(dl16.view(B, 1, 1, n_pad), yc.view(B, 1, 1, Cf)).view(n_pad, Cf)[:n_cls]
-        if dst is not None:
-            dst.copy_(gw)
-            gw = dst
-        grads.put(head.weight, gw)
-    if head.bias is not None:
-        grads.put(head.bias, ops.colsum(dl16, cols=n_cls, out=grads.dest(head.bias)))
-    d_yc = ops.conv2d_dgrad(dl16.view(B, 1, 1, n_pad), pack.get(head.weight, 1), (1, 1)).view(B, Cf)
-    d_pool, dgn, dbn = ops.layernorm_bwd(d_yc, pooled, mc, rc, model.norm.weight, dx_dtype=BF16,
-                                         dgamma=grads.dest(model.norm.weight), dbeta=grads.dest(model.norm.bias))
-    grads.put(model.norm.weight, dgn)
-    grads.put(model.norm.bias, dbn)
+    pooled, yc, mc, rc, (B, Hf, Wf, Cf) = tape["head"]
+    d_yc = common.head_backward(grads, pack, model.head, yc, dlogits)
+    d_pool = layernorm_backward(grads, model.norm, d_yc, pooled, mc, rc)
     g = ops.avgpool_bwd(d_pool, (Hf, Wf))                          # bf16 [B, Hf, Wf, Cf]: gradient of the stream
     for i in range(3, -1, -1):
         rec = tape["stages"][i]
@@ -215,12 +159,9 @@ def backward(model, tape, dlogits, sink=None):
                 grads.put(blk.gamma, dgam)
             # (g*gamma) W2, times GELU'(pre); the epilogue also sums the columns of d_pre (= pwconv1 bias gradient)
             d_pre, _, st_pre = ops.gemm(g2, pack.get(blk.pwconv2.weight, 1), act=3, aux_in=dact, want_stats=True)
-            _lin_wgrad(grads, blk.pwconv1, d_pre, y.view(M, C), dy_stats=st_pre)
+            linear_grads(grads, blk.pwconv1, d_pre, y.view(M, C), dy_stats=st_pre)
             d_y, _ = ops.gemm(d_pre, pack.get(blk.pwconv1.weight, 1))
-            du, dgl, dbl = ops.layernorm_bwd(d_y, u.view(M, C), m, r, blk.norm.weight, dx_dtype=BF16,
-                                             dgamma=grads.dest(blk.norm.weight), dbeta=grads.dest(blk.norm.bias))
-            grads.put(blk.norm.weight, dgl)
-            grads.put(blk.norm.bias, dbl)
+            du = layernorm_backward(grads, blk.norm, d_y, u.view(M, C), m, r)
             du4 = du.view(Bb, H, W, C)
             grads.put(blk.dwconv.weight, ops.dwconv7_wgrad(du4, h, out=grads.dest(blk.dwconv.weight)))
             grads.put(blk.dwconv.bias, ops.colsum_tall(du, out=grads.dest(blk.dwconv.bias)))
@@ -236,58 +177,15 @@ def backward(model, tape, dlogits, sink=None):
             grads.put(conv.bias, gb)
             d_y = ops.conv2d_dgrad(g, pack.get(conv.weight, 1), tuple(h_prev.shape[1:3]), 2, 2)
             Cp = h_prev.shape[3]
-            g2, dgl, dbl = ops.layernorm_bwd(d_y.view(-1, Cp), h_prev.view(-1, Cp), m, r, ln.weight, dx_dtype=BF16,
-                                             dgamma=grads.dest(ln.weight), dbeta=grads.dest(ln.bias))
-            grads.put(ln.weight, dgl)
-            grads.put(ln.bias, dbl)
-            g = g2.view(h_prev.shape)
+            g = layernorm_backward(grads, ln, d_y.view(-1, Cp), h_prev.view(-1, Cp), m, r).view(h_prev.shape)
     # ---- stem
     a, u0, m0, r0 = tape["stem"]
     stem_conv, stem_ln = model.downsample_layers[0][0], model.downsample_layers[0][1]
     C0 = stem_conv.out_channels
-    du0, dgl, dbl = ops.layernorm_bwd(g.view(-1, C0), u0.view(-1, C0), m0, r0, stem_ln.weight, dx_dtype=BF16,
-                                      dgamma=grads.dest(stem_ln.weight), dbeta=grads.dest(stem_ln.bias))
-    grads.put(stem_ln.weight, dgl)
-    grads.put(stem_ln.bias, dbl)
-    K0 = a.shape[-1]
-    Mp = du0.shape[0]
-    dst = grads.dest(stem_conv.weight)
-    gb = grads.dest(stem_conv.bias)
-    if gb is None:
-        gb = torch.empty(C0, dtype=F32, device=du0.device)
-    gw = ops.conv2d_wgrad(du0.view(Mp, 1, 1, C0), a.view(Mp, 1, 1, K0), out=dst.view(C0, K0, 1, 1) if dst is not None else None,
-                          bias_out=gb)
-    grads.put(stem_conv.weight, gw)
-    grads.put(stem_conv.bias, gb)
+    du0 = layernorm_backward(grads, stem_ln, g.view(-1, C0), u0.view(-1, C0), m0, r0)
+    linear_grads(grads, stem_conv, du0, a.view(du0.shape[0], a.shape[-1]))
     return grads
 
 
-class _Function(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, model, *params):
-        want_tape = any(ctx.needs_input_grad[2:])
-        logits, tape = forward(model, x, model.training, want_tape)
-        ctx.model, ctx.tape, ctx.params = model, tape, params
-        return logits
-
-    @staticmethod
-    def backward(ctx, dlogits):
-        if ctx.tape is None:
-            raise RuntimeError("backward called on a forward that recorded no tape")
-        grads = backward(ctx.model, ctx.tape, dlogits)
-        ctx.tape = None
-        out = []
-        for p, need in zip(ctx.params, ctx.needs_input_grad[2:]):
-            gp = grads.get(p.data_ptr()) if need else None
-            out.append(gp.reshape(p.shape) if gp is not None else None)
-        return (None, None, *out)
-
-
 def apply(model, x):
-    if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 ConvNeXt runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
-    params = tuple(model.parameters())
-    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
-        return _Function.apply(x, model, *params)
-    logits, _ = forward(model, x, model.training, False)
-    return logits
+    return common.apply(sys.modules[__name__], "ConvNeXt", model, x)

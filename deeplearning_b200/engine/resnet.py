@@ -1,6 +1,6 @@
 """Forward / backward schedule of the ResNet family on the sm_90a kernels.
 
-The whole network is ONE ``torch.autograd.Function``: forward runs conv(+BN statistics in the GEMM epilogue) -> finalize ->
+The whole network is ONE autograd node (common.apply): forward runs conv(+BN statistics in the GEMM epilogue) -> finalize ->
 apply(+ReLU)(+residual) per layer and records the tensors the backward needs on a tape; backward replays the tape with
 BN-backward reduce/apply passes, wgmma dgrad and wgrad GEMMs.  Residual additions never get their own pass: the identity
 gradient is added in the epilogue of the first conv's dgrad GEMM.
@@ -28,14 +28,14 @@ last unit as a squeeze-and-excitation tail (csrc/se.cuh) on the pass schedule un
               ->  dc = BatchNorm backward of du = dz * gate + dpool / HW
 """
 import os
+import sys
 
 import torch
 import torch.nn as nn
 
 from .. import ops
+from . import common
 from .packing import weight_cache
-
-BF16 = torch.bfloat16
 
 
 _GROUP_WIDTHS = (4, 8, 16, 32, 64)
@@ -81,6 +81,15 @@ def _bn_sync(bn):
     return (group, world) if world > 1 else None
 
 
+def _bn_coeffs(bn, stats, rows, train):
+    """BatchNorm coefficients: from the batch statistics (``rows`` values per channel, running statistics updated) in
+    train mode, from the running statistics in eval mode."""
+    if train:
+        return ops.bn_finalize(stats, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
+                               bn.num_batches_tracked, sync=_bn_sync(bn))
+    return ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+
+
 class _PackSpec:
     """Which bf16 operands a ResNet needs: forward [O][taps*I] and dgrad [I][taps*O] copies of every conv / fc weight."""
 
@@ -103,11 +112,7 @@ class _PackSpec:
                     continue
                 specs.append((w, 0, kh * kw * I, O))
                 specs.append((w, 1, kh * kw * O, I))
-        fc = model.fc
-        n_pad = (fc.out_features + 7) // 8 * 8
-        specs.append((fc.weight, 0, fc.in_features, n_pad))
-        specs.append((fc.weight, 1, n_pad, fc.in_features))
-        return specs
+        return specs + common.head_pack_specs(model.fc)
 
 
 _pack_spec = _PackSpec()
@@ -116,8 +121,12 @@ _pack_spec = _PackSpec()
 class _Unit:
     """Saved state of one conv -> BN (-> ReLU) (-> + residual) application.  ``algebra`` units (bottleneck conv3 with the
     BatchNorm folded through the convolution) have no raw conv output ``c``; they keep the Gram matrix ``G`` and the column
-    sums ``s`` of their input instead."""
+    sums ``s`` of their input instead.  ``se`` holds (module, saved tensors) of a squeeze-and-excitation tail."""
     __slots__ = ("conv", "bn", "x", "c", "co", "y", "relu", "has_res", "algebra", "G", "s", "se")
+
+    def __init__(self, conv, bn, x, c, co, y, relu, has_res, algebra=False, G=None, s=None, se=None):
+        self.conv, self.bn, self.x, self.c, self.co, self.y = conv, bn, x, c, co, y
+        self.relu, self.has_res, self.algebra, self.G, self.s, self.se = relu, has_res, algebra, G, s, se
 
 
 def _algebra_enabled():
@@ -153,10 +162,7 @@ def _conv3_bn_res_relu(pack, tape, y2, conv, bn, train, identity, name=""):
         co = ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
     y = ops.conv1x1_bn_act(y2, wp, co, identity)
     if tape is not None:
-        u = _Unit()
-        u.conv, u.bn, u.x, u.c, u.co, u.y, u.relu, u.has_res = conv, bn, y2, None, co, y, True, True
-        u.algebra, u.G, u.s = True, G, s
-        tape.append(u)
+        tape.append(_Unit(conv, bn, y2, None, co, y, True, True, algebra=True, G=G, s=s))
     return y
 
 
@@ -185,10 +191,7 @@ def _ds_conv_bn_algebra(pack, tape, x_in, conv, bn, name=""):
                            bn.num_batches_tracked)
     ident = ops.conv1x1_bn(xs, wp, co)
     if tape is not None:
-        u = _Unit()
-        u.conv, u.bn, u.x, u.c, u.co, u.y, u.relu, u.has_res = conv, bn, xs, None, co, ident, False, False
-        u.algebra, u.G, u.s = True, G, s
-        tape.append(u)
+        tape.append(_Unit(conv, bn, xs, None, co, ident, False, False, algebra=True, G=G, s=s))
     return ident
 
 
@@ -202,18 +205,10 @@ def _conv_bn(pack, tape, x, conv, bn, train, relu, residual=None, name=""):
         co = ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
         return ops.conv2d_bn_act(x, wp, co, k, s, relu=relu, residual=residual, groups=g)
     c, st = ops.conv2d_fwd(x, wp, k, s, want_stats=train, groups=g)
-    if train:
-        rows = c.numel() // c.shape[-1]
-        co = ops.bn_finalize(st, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
-                             bn.num_batches_tracked, sync=_bn_sync(bn))
-    else:
-        co = ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+    co = _bn_coeffs(bn, st, c.numel() // c.shape[-1], train)
     y = ops.bn_apply(c, co, relu=relu, residual=residual)
     if tape is not None:
-        u = _Unit()
-        u.conv, u.bn, u.x, u.c, u.co, u.y, u.relu, u.has_res = conv, bn, x, c, co, y, relu, residual is not None
-        u.algebra, u.G, u.s = False, None, None
-        tape.append(u)
+        tape.append(_Unit(conv, bn, x, c, co, y, relu, residual is not None))
     return y
 
 
@@ -244,20 +239,12 @@ def _conv_bn_se(pack, tape, x, conv, bn, se, train, identity, name=""):
         raise NotImplementedError(f"{name}: SyncBatchNorm in front of a squeeze-and-excitation gate is not implemented")
     wp = pack.get(conv.weight, _pack_modes(conv)[0])
     c, st = ops.conv2d_fwd(x, wp, conv.kernel_size[0], conv.stride[0], want_stats=train, groups=conv.groups)
-    if train:
-        co = ops.bn_finalize(st, c.numel() // c.shape[-1], bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean,
-                             bn.running_var, bn.num_batches_tracked)
-    else:
-        co = ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+    co = _bn_coeffs(bn, st, c.numel() // c.shape[-1], train)
     csum, pool = ops.se_squeeze(c, co)
     h, gate = ops.se_excite(pool, se.fc[0].weight, se.fc[2].weight)
     y = ops.se_apply(c, co, gate, identity)
     if tape is not None:
-        u = _Unit()
-        u.conv, u.bn, u.x, u.c, u.co, u.y, u.relu, u.has_res = conv, bn, x, c, co, y, True, True
-        u.algebra, u.G, u.s = False, None, None
-        u.se = (se, csum, pool, h, gate)
-        tape.append(u)
+        tape.append(_Unit(conv, bn, x, c, co, y, True, True, se=(se, csum, pool, h, gate)))
     return y
 
 
@@ -302,11 +289,7 @@ def forward(model, x, train, want_tape):
     a = ops.stem_s2d_u8(x, *getattr(model, "input_norm", (ops.IMAGENET_MEAN, ops.IMAGENET_STD))) if u8 else ops.stem_s2d(x)
     Ho, Wo = a.shape[1] - 3, a.shape[2] - 3
     c1, st = ops.stem_s2d_conv_fwd(a, pack.get(conv1.weight, 2), want_stats=train)
-    if train:
-        co1 = ops.bn_finalize(st, B * Ho * Wo, bn1.weight, bn1.bias, bn1.eps, bn1.momentum, bn1.running_mean,
-                              bn1.running_var, bn1.num_batches_tracked, sync=_bn_sync(bn1))
-    else:
-        co1 = ops.bn_eval_coeffs(bn1.weight, bn1.bias, bn1.running_mean, bn1.running_var, bn1.eps)
+    co1 = _bn_coeffs(bn1, st, B * Ho * Wo, train)
     h, idx = ops.bn_relu_maxpool_fwd(c1, co1)
     if want_tape:
         tape["stem"] = (a, c1, co1, idx, (Ho, Wo))
@@ -341,40 +324,10 @@ def forward(model, x, train, want_tape):
                 tape["blocks"].append((units, ds_units[0] if ds_units else None, x_in))
     # ---- head: global average pool + fc (fp32 logits)
     pooled = ops.avgpool_fwd(h)
-    fc = model.fc
-    n_cls = fc.out_features
-    n_pad = (n_cls + 7) // 8 * 8
-    wfc = pack.get(fc.weight, 0)
-    bias = None
-    if fc.bias is not None:
-        bias = fc.bias.detach()
-        if n_pad != n_cls:
-            bias = torch.cat([bias, bias.new_zeros(n_pad - n_cls)])
-    logits, _ = ops.conv2d_fwd(pooled.view(B, 1, 1, -1), wfc, bias=bias, out_f32=True)
-    logits = logits.view(B, n_pad)
+    logits = common.head_forward(pack, model.fc, pooled)
     if want_tape:
-        tape["head"] = (pooled, h.shape[1:3], n_cls, n_pad)
-    return (logits[:, :n_cls] if n_pad != n_cls else logits), tape
-
-
-class _Grads(dict):
-    """{parameter.data_ptr(): fp32 gradient}. ``sink(param)`` may supply the destination buffer (a view of the flat
-    gradient arena of engine.trainer) so gradients are produced in place instead of in fresh tensors."""
-
-    def __init__(self, sink=None):
-        super().__init__()
-        self.sink = sink
-
-    def dest(self, param):
-        return self.sink(param) if self.sink is not None else None
-
-    def put(self, param, value):
-        """Record the (final) gradient of ``param``; a sink with a ``notify`` method is told so that the data-parallel
-        trainer can start all-reducing completed stretches of the gradient arena while the backward pass continues."""
-        self[param.data_ptr()] = value
-        notify = getattr(self.sink, "notify", None)
-        if notify is not None:
-            notify(param)
+        tape["head"] = (pooled, h.shape[1:3])
+    return logits, tape
 
 
 def _unit_backward(u, g, grads, want_dz=False):
@@ -416,36 +369,27 @@ def _unit_backward_from_sums(u, dz, sums, grads):
     return dc
 
 
+def _algebra_backward(u, dz, dz_stats, pack, grads):
+    """Parameter gradients of an algebra unit (BatchNorm folded through its 1x1 convolution) from dz, the gradient of the
+    BatchNorm output, and its column-sum partials; returns the packed operand ``wcat`` = [a W | M] and the bias ``wbias``
+    of the ops.gemm_dual call over [dz | x] that gives the gradient of the unit's input."""
+    D = ops.conv2d_wgrad(dz, u.x, 1, 1)                              # raw dz^T x [N, K, 1, 1]
+    dgamma, dbeta, dW, wcat, wbias = ops.bn_conv1x1_bwd(
+        dz_stats, D, u.G, u.s, pack.get(u.conv.weight, 0), u.conv.weight, dz.numel() // u.conv.out_channels, u.bn.weight,
+        u.co, dgamma=grads.dest(u.bn.weight), dbeta=grads.dest(u.bn.bias), dW=grads.dest(u.conv.weight))
+    grads.put(u.bn.weight, dgamma)
+    grads.put(u.bn.bias, dbeta)
+    grads.put(u.conv.weight, dW)
+    return wcat, wbias
+
+
 def backward(model, tape, dlogits, sink=None):
     """dlogits: fp32 [B, num_classes] (or the bf16 [B, n_pad] product of ops.softmax_xent).
     Returns {parameter.data_ptr(): fp32 gradient}; with ``sink`` the gradients are written into caller-owned buffers."""
-    grads = _Grads(sink)
-    pooled, hw, n_cls, n_pad = tape["head"]
-    B = pooled.shape[0]
-    fc = model.fc
-    if dlogits.dtype == BF16 and dlogits.shape[1] == n_pad and dlogits.is_contiguous():
-        dl16 = dlogits.view(B, 1, 1, n_pad)  # already produced by the fused soft-max/cross-entropy kernel
-    else:
-        dl = dlogits.contiguous().float()
-        if n_pad != n_cls:
-            dl = torch.cat([dl, dl.new_zeros(B, n_pad - n_cls)], 1).contiguous()
-        dl16 = ops.cast_bf16(dl).view(B, 1, 1, n_pad)
-    x_fc = pooled.view(B, 1, 1, -1)
-    dst = grads.dest(fc.weight)
-    if dst is not None and n_pad == n_cls:
-        grads.put(fc.weight, ops.conv2d_wgrad(dl16, x_fc, out=dst.view(n_cls, -1, 1, 1)))
-    else:
-        gw = ops.conv2d_wgrad(dl16, x_fc).view(n_pad, -1)[:n_cls]
-        if dst is not None:
-            dst.copy_(gw)
-            gw = dst
-        grads.put(fc.weight, gw)
-    if fc.bias is not None:
-        grads.put(fc.bias, ops.colsum(dl16.view(B, n_pad), cols=n_cls, out=grads.dest(fc.bias)))
+    grads = common.Grads(sink)
+    pooled, hw = tape["head"]
     pack = tape["pack"]
-    wfc_d = pack.get(fc.weight, 1)
-    dpooled = ops.conv2d_dgrad(dl16, wfc_d, (1, 1))
-    g = ops.avgpool_bwd(dpooled.view(B, -1), hw)
+    g = ops.avgpool_bwd(common.head_backward(grads, pack, model.fc, pooled, dlogits), hw)
 
     # The gradient of a block output travels either as the raw gradient ``g`` (then the block masks it itself) or, when the
     # consumer's conv1 dgrad epilogue already applied this block's ReLU mask, as ``dz`` with its partial column sums.
@@ -460,15 +404,7 @@ def backward(model, tape, dlogits, sink=None):
             if dz is None:
                 dz, dz_stats = ops.relu_mask_sum(g, last.y)
             y2 = last.x
-            N, K = last.conv.out_channels, last.conv.in_channels
-            D = ops.conv2d_wgrad(dz, y2, 1, 1)                       # raw dz^T y2 [N, K, 1, 1]
-            count = dz.numel() // N
-            dgamma, dbeta, dW, wcat, wbias = ops.bn_conv1x1_bwd(
-                dz_stats, D, last.G, last.s, pack.get(last.conv.weight, 0), last.conv.weight, count, last.bn.weight, last.co,
-                dgamma=grads.dest(last.bn.weight), dbeta=grads.dest(last.bn.bias), dW=grads.dest(last.conv.weight))
-            grads.put(last.bn.weight, dgamma)
-            grads.put(last.bn.bias, dbeta)
-            grads.put(last.conv.weight, dW)
+            wcat, wbias = _algebra_backward(last, dz, dz_stats, pack, grads)
             # dL/dy2 = [dz | y2] [a W3 | M]^T + k W3; its epilogue also masks with bn2's ReLU and sums for bn2's backward
             u2 = units[-2]
             if _fused_reduce_ok(u2):
@@ -478,7 +414,7 @@ def backward(model, tape, dlogits, sink=None):
                 g_prev = ops.gemm_dual(dz, y2, wcat, wbias)
                 dc, _ = _unit_backward(u2, g_prev, grads)
             first = len(units) - 2
-        elif getattr(last, "se", None) is not None:
+        elif last.se is not None:
             dc, dz = _se_unit_backward(last, g, grads)
             first = len(units) - 1
         else:
@@ -489,15 +425,7 @@ def backward(model, tape, dlogits, sink=None):
         # parameter gradients come from dz directly (no pass over a raw conv output, which does not exist)
         gxs = None
         if has_ds and ds.algebra:
-            Nd, Kd = ds.conv.out_channels, ds.conv.in_channels
-            Dd = ops.conv2d_wgrad(dz, ds.x, 1, 1)
-            dgd, dbd, dWd, wcat_d, wbias_d = ops.bn_conv1x1_bwd(
-                dz_stats, Dd, ds.G, ds.s, pack.get(ds.conv.weight, 0), ds.conv.weight, dz.numel() // Nd, ds.bn.weight, ds.co,
-                dgamma=grads.dest(ds.bn.weight), dbeta=grads.dest(ds.bn.bias), dW=grads.dest(ds.conv.weight))
-            grads.put(ds.bn.weight, dgd)
-            grads.put(ds.bn.bias, dbd)
-            grads.put(ds.conv.weight, dWd)
-            gxs = ops.gemm_dual(dz, ds.x, wcat_d, wbias_d)
+            gxs = ops.gemm_dual(dz, ds.x, *_algebra_backward(ds, dz, dz_stats, pack, grads))
         # does the producer of x_in (the previous block) take its gradient pre-masked from this block's conv1 dgrad?
         prev_masked = (bi > 0 and not has_ds and blocks[bi - 1][0][-1].algebra and _algebra_ok_dgrad(units[0].conv))
         dz_prev = dz_prev_stats = None
@@ -544,32 +472,5 @@ def backward(model, tape, dlogits, sink=None):
     return grads
 
 
-class _ResNetFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, model, *params):
-        want_tape = any(ctx.needs_input_grad[2:])
-        logits, tape = forward(model, x, model.training, want_tape)
-        ctx.model, ctx.tape, ctx.params = model, tape, params
-        return logits
-
-    @staticmethod
-    def backward(ctx, dlogits):
-        if ctx.tape is None:
-            raise RuntimeError("backward called on a forward that recorded no tape")
-        grads = backward(ctx.model, ctx.tape, dlogits)
-        ctx.tape = None
-        out = []
-        for p, need in zip(ctx.params, ctx.needs_input_grad[2:]):
-            gp = grads.get(p.data_ptr()) if need else None
-            out.append(gp.reshape(p.shape) if gp is not None else None)
-        return (None, None, *out)
-
-
 def apply(model, x):
-    if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 ResNet runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
-    params = tuple(model.parameters())
-    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
-        return _ResNetFunction.apply(x, model, *params)
-    logits, _ = forward(model, x, model.training, False)
-    return logits
+    return common.apply(sys.modules[__name__], "ResNet", model, x)

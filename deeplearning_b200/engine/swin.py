@@ -1,4 +1,4 @@
-"""Forward / backward schedule of the Swin Transformer on the sm_90a kernels (one autograd.Function for the whole network).
+"""Forward / backward schedule of the Swin Transformer on the sm_90a kernels (one autograd node for the whole network).
 
 Mirrors ``SwinTransformer.forward_features`` / ``BasicLayer.forward`` / ``SwinTransformerBlock.forward`` /
 ``WindowAttention.forward`` / ``PatchMerging.forward`` of the reference
@@ -10,16 +10,16 @@ Data flow per block (residual stream ``h`` fp32 [B, H*W, C] in natural pixel ord
     -> proj GEMM(+bias, +h, fp32 out) = h2 -> LN2 -> fc1 GEMM(+bias, GELU, keeps GELU'(pre)) -> fc2 GEMM(+bias, +h2) = h3
 PatchMerging = one gather+LayerNorm kernel (the 2x2 concat never exists in HBM) + the bias-free reduction GEMM (fp32 out).
 """
+import sys
+
 import torch
 import torch.nn as nn
 
 from .. import ops
-from . import droppath
+from . import common, droppath
+from .common import linear_grads, layernorm_backward
 from .packing import weight_cache
-from .resnet import _Grads
-from .vit import _lin_grads
 
-BF16 = torch.bfloat16
 F32 = torch.float32
 
 
@@ -49,11 +49,7 @@ class _PackSpec:
                 w = lin.weight
                 specs.append((w, 0, w.shape[1], w.shape[0]))
                 specs.append((w, 1, w.shape[0], w.shape[1]))
-        head = model.head
-        n_pad = (head.out_features + 7) // 8 * 8
-        specs.append((head.weight, 0, head.in_features, n_pad))
-        specs.append((head.weight, 1, n_pad, head.in_features))
-        return specs
+        return specs + common.head_pack_specs(model.head)
 
 
 _pack_spec = _PackSpec()
@@ -79,9 +75,7 @@ def _check(model):
 
 def forward(model, x, train, want_tape):
     _check(model)
-    if x.dtype == torch.uint8:      # GPU input pipeline: decoded uint8 NHWC batch -> ToTensor + Normalize on the device
-        x = ops.normalize_u8_nhwc(x, *getattr(model, "input_norm", (ops.IMAGENET_MEAN, ops.IMAGENET_STD)))
-    x = x.contiguous().float()
+    x = common.image_input(model, x)
     B, Cin, Hi, Wi = x.shape
     pe = model.patch_embed
     if (Hi, Wi) != tuple(pe.img_size):
@@ -133,56 +127,24 @@ def forward(model, x, train, want_tape):
     Cf = h.shape[-1]
     yn, mn, rn = ops.layernorm_fwd(h, model.norm.weight, model.norm.bias, model.norm.eps)
     pooled = ops.cast_bf16(ops.avgpool_any(yn.view(B, H, W, Cf)))
-    head = model.head
-    n_cls = head.out_features
-    n_pad = (n_cls + 7) // 8 * 8
-    bias = None
-    if head.bias is not None:
-        bias = head.bias.detach()
-        if n_pad != n_cls:
-            bias = torch.cat([bias, bias.new_zeros(n_pad - n_cls)])
-    logits, _ = ops.conv2d_fwd(pooled.view(B, 1, 1, Cf), pack.get(head.weight, 0), bias=bias, out_f32=True)
-    logits = logits.view(B, n_pad)
+    logits = common.head_forward(pack, model.head, pooled)
     if want_tape:
-        tape["head"] = (h, mn, rn, pooled, n_cls, n_pad, (B, H, W, Cf))
-    return (logits[:, :n_cls] if n_pad != n_cls else logits), tape
+        tape["head"] = (h, mn, rn, pooled, (B, H, W, Cf))
+    return logits, tape
 
 
 def backward(model, tape, dlogits, sink=None):
-    grads = _Grads(sink)
+    grads = common.Grads(sink)
     pack = tape["pack"]
-    h_last, mn, rn, pooled, n_cls, n_pad, (B, H, W, Cf) = tape["head"]
-    head = model.head
-    if dlogits.dtype == BF16 and dlogits.shape[1] == n_pad and dlogits.is_contiguous():
-        dl16 = dlogits
-    else:
-        dl = dlogits.contiguous().float()
-        if n_pad != n_cls:
-            dl = torch.cat([dl, dl.new_zeros(B, n_pad - n_cls)], 1).contiguous()
-        dl16 = ops.cast_bf16(dl)
-    dst = grads.dest(head.weight)
-    if dst is not None and n_pad == n_cls:
-        grads.put(head.weight, ops.conv2d_wgrad(dl16.view(B, 1, 1, n_pad), pooled.view(B, 1, 1, Cf), out=dst.view(n_cls, Cf, 1, 1)))
-    else:
-        gw = ops.conv2d_wgrad(dl16.view(B, 1, 1, n_pad), pooled.view(B, 1, 1, Cf)).view(n_pad, Cf)[:n_cls]
-        if dst is not None:
-            dst.copy_(gw)
-            gw = dst
-        grads.put(head.weight, gw)
-    if head.bias is not None:
-        grads.put(head.bias, ops.colsum(dl16, cols=n_cls, out=grads.dest(head.bias)))
-    d_pool = ops.conv2d_dgrad(dl16.view(B, 1, 1, n_pad), pack.get(head.weight, 1), (1, 1)).view(B, Cf)
-    d_yn = ops.avgpool_bwd(d_pool, (H, W))
-    g, dgn, dbn = ops.layernorm_bwd(d_yn.view(B, H * W, Cf), h_last, mn, rn, model.norm.weight, dx_dtype=BF16,
-                                    dgamma=grads.dest(model.norm.weight), dbeta=grads.dest(model.norm.bias))
-    grads.put(model.norm.weight, dgn)
-    grads.put(model.norm.bias, dbn)
+    h_last, mn, rn, pooled, (B, H, W, Cf) = tape["head"]
+    d_yn = ops.avgpool_bwd(common.head_backward(grads, pack, model.head, pooled, dlogits), (H, W))
+    g = layernorm_backward(grads, model.norm, d_yn.view(B, H * W, Cf), h_last, mn, rn)
     for recs, merge, (H, W, C) in reversed(tape["layers"]):
         if merge is not None:
             ds, h_in, ym, mm, rm = merge
             Mo = ym.shape[0]
             g2 = g.view(Mo, 2 * C)
-            _lin_grads(grads, ds.reduction, g2, ym)
+            linear_grads(grads, ds.reduction, g2, ym)
             d_ym, _ = ops.gemm(g2, pack.get(ds.reduction.weight, 1))
             g, dgm, dbm = ops.patch_merge_ln_bwd(d_ym, h_in.view(B, H, W, C), mm, rm, ds.norm.weight,
                                                  dgamma=grads.dest(ds.norm.weight), dbeta=grads.dest(ds.norm.bias))
@@ -195,16 +157,13 @@ def backward(model, tape, dlogits, sink=None):
             nH = att_m.num_heads
             # (stochastic depth: the branch sees the per-sample scaled gradient, the identity path - `add=g` - the full one)
             g2 = (g if dp2 is None else ops.rowscale(g, dp2)).view(M, C)
-            _lin_grads(grads, mlp.fc2, g2, post.view(M, -1))
+            linear_grads(grads, mlp.fc2, g2, post.view(M, -1))
             d_pre, _, st_pre = ops.gemm(g2, pack.get(mlp.fc2.weight, 1), act=3, aux_in=dact.view(M, -1), want_stats=True)
-            _lin_grads(grads, mlp.fc1, d_pre, y2.view(M, C), dy_stats=st_pre)
+            linear_grads(grads, mlp.fc1, d_pre, y2.view(M, C), dy_stats=st_pre)
             d_y2, _ = ops.gemm(d_pre, pack.get(mlp.fc1.weight, 1))
-            g, dg2, db2 = ops.layernorm_bwd(d_y2, h2, m2, r2, blk.norm2.weight, add=g, dx_dtype=BF16,
-                                            dgamma=grads.dest(blk.norm2.weight), dbeta=grads.dest(blk.norm2.bias))
-            grads.put(blk.norm2.weight, dg2)
-            grads.put(blk.norm2.bias, db2)
+            g = layernorm_backward(grads, blk.norm2, d_y2, h2, m2, r2, add=g)
             g2 = (g if dp1 is None else ops.rowscale(g, dp1)).view(M, C)
-            _lin_grads(grads, att_m.proj, g2, att.view(M, C))
+            linear_grads(grads, att_m.proj, g2, att.view(M, C))
             d_att, _ = ops.gemm(g2, pack.get(att_m.proj.weight, 1))
             dqkv, dbias = ops.window_attention_bwd(qkv.view(B, H, W, 3 * C), att, d_att.view(B, H, W, C), bias, lse, nH,
                                                    blk.shift_size, float(att_m.scale))
@@ -212,62 +171,19 @@ def backward(model, tape, dlogits, sink=None):
             dt = grads.dest(table)
             dt = dt.zero_() if dt is not None else torch.zeros_like(table, dtype=F32)
             grads.put(table, ops.window_bias_scatter(dbias, att_m.relative_position_index, dt))
-            _lin_grads(grads, att_m.qkv, dqkv.view(M, 3 * C), y1.view(M, C))
+            linear_grads(grads, att_m.qkv, dqkv.view(M, 3 * C), y1.view(M, C))
             d_y1, _ = ops.gemm(dqkv.view(M, 3 * C), pack.get(att_m.qkv.weight, 1))
-            g, dg1, db1 = ops.layernorm_bwd(d_y1, h, m1, r1, blk.norm1.weight, add=g, dx_dtype=BF16,
-                                            dgamma=grads.dest(blk.norm1.weight), dbeta=grads.dest(blk.norm1.bias))
-            grads.put(blk.norm1.weight, dg1)
-            grads.put(blk.norm1.bias, db1)
+            g = layernorm_backward(grads, blk.norm1, d_y1, h, m1, r1, add=g)
             g = g.view(B, H * W, C)
     # ---- patch embedding: h0 = LN(patches W^T + b)
     a, u0, m0, r0 = tape["embed"]
     pe = model.patch_embed
-    du0, dg0, db0 = ops.layernorm_bwd(g, u0, m0, r0, pe.norm.weight, dx_dtype=BF16,
-                                      dgamma=grads.dest(pe.norm.weight), dbeta=grads.dest(pe.norm.bias))
-    grads.put(pe.norm.weight, dg0)
-    grads.put(pe.norm.bias, db0)
-    D, K0 = u0.shape[-1], a.shape[-1]
+    du0 = layernorm_backward(grads, pe.norm, g, u0, m0, r0)
+    D = u0.shape[-1]
     rows = u0.numel() // D
-    dst = grads.dest(pe.proj.weight)
-    gb = None
-    if pe.proj.bias is not None:
-        gb = grads.dest(pe.proj.bias)
-        if gb is None:
-            gb = torch.empty(D, dtype=F32, device=du0.device)
-    gw = ops.conv2d_wgrad(du0.view(rows, 1, 1, D), a.view(rows, 1, 1, K0), out=dst.view(D, K0, 1, 1) if dst is not None else None,
-                          bias_out=gb)
-    grads.put(pe.proj.weight, gw)
-    if pe.proj.bias is not None:
-        grads.put(pe.proj.bias, gb)
+    linear_grads(grads, pe.proj, du0.view(rows, D), a.view(rows, a.shape[-1]))
     return grads
 
 
-class _SwinFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, model, *params):
-        want_tape = any(ctx.needs_input_grad[2:])
-        logits, tape = forward(model, x, model.training, want_tape)
-        ctx.model, ctx.tape, ctx.params = model, tape, params
-        return logits
-
-    @staticmethod
-    def backward(ctx, dlogits):
-        if ctx.tape is None:
-            raise RuntimeError("backward called on a forward that recorded no tape")
-        grads = backward(ctx.model, ctx.tape, dlogits)
-        ctx.tape = None
-        out = []
-        for p, need in zip(ctx.params, ctx.needs_input_grad[2:]):
-            gp = grads.get(p.data_ptr()) if need else None
-            out.append(gp.reshape(p.shape) if gp is not None else None)
-        return (None, None, *out)
-
-
 def apply(model, x):
-    if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 Swin runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
-    params = tuple(model.parameters())
-    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
-        return _SwinFunction.apply(x, model, *params)
-    logits, _ = forward(model, x, model.training, False)
-    return logits
+    return common.apply(sys.modules[__name__], "Swin", model, x)

@@ -18,6 +18,7 @@ import torch
 import torch.distributed as dist
 
 from .. import ops
+from .common import padded_classes
 from .packing import weight_cache
 
 
@@ -254,8 +255,7 @@ class TrainStep:
         With gradient accumulation only the ``last`` micro-batch of a group reduces (the sum of the group's gradients)."""
         model, arena = self.model, self.arena
         logits, tape = self.engine.forward(model, images, True, True)
-        n_pad = (logits.shape[1] + 7) // 8 * 8
-        loss, dlogits, correct = ops.softmax_xent(logits, labels, want_grad=True, ld_d=n_pad,
+        loss, dlogits, correct = ops.softmax_xent(logits, labels, want_grad=True, ld_d=padded_classes(logits.shape[1]),
                                                   label_smoothing=self.label_smoothing, loss_scale=1.0 / self.accum_steps)
         if self.accum_steps > 1:
             self.engine.backward(model, tape, dlogits, sink=arena.grad_view)

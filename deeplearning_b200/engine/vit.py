@@ -1,4 +1,4 @@
-"""Forward / backward schedule of the ViT family on the sm_90a kernels (one autograd.Function for the whole network).
+"""Forward / backward schedule of the ViT family on the sm_90a kernels (one autograd node for the whole network).
 
 Mirrors ``VisionTransformer.forward_features`` / ``Block.forward`` / ``Attention.forward`` / ``Mlp.forward`` of the
 reference (classification/vision_transformer/vit_model.py:240-268, :158-161, :88-111, :127-133).
@@ -10,13 +10,15 @@ Residual adds, biases, GELU, GELU' (backward) and the pos-embed add of the patch
 attention scores never touch HBM.  The gradient of the residual stream is carried in bf16 and accumulated inside the
 LayerNorm-backward kernel.
 """
+import sys
+
 import torch
 import torch.nn as nn
 
 from .. import ops
-from . import droppath
+from . import common, droppath
+from .common import linear_grads, layernorm_backward
 from .packing import weight_cache
-from .resnet import _Grads  # same gradient-sink protocol as the ResNet engine
 
 BF16 = torch.bfloat16
 F32 = torch.float32
@@ -45,11 +47,7 @@ class _PackSpec:
             w = lin.weight
             specs.append((w, 0, w.shape[1], w.shape[0]))
             specs.append((w, 1, w.shape[0], w.shape[1]))
-        head = model.head
-        n_pad = (head.out_features + 7) // 8 * 8
-        specs.append((head.weight, 0, head.in_features, n_pad))
-        specs.append((head.weight, 1, n_pad, head.in_features))
-        return specs
+        return specs + common.head_pack_specs(model.head)
 
 
 _pack_spec = _PackSpec()
@@ -75,9 +73,7 @@ def _check(model):
 
 def forward(model, x, train, want_tape):
     _check(model)
-    if x.dtype == torch.uint8:      # GPU input pipeline: decoded uint8 NHWC batch -> ToTensor + Normalize on the device
-        x = ops.normalize_u8_nhwc(x, *getattr(model, "input_norm", (ops.IMAGENET_MEAN, ops.IMAGENET_STD)))
-    x = x.contiguous().float()
+    x = common.image_input(model, x)
     B, Cin, Hh, Ww = x.shape
     pe = model.patch_embed
     ps = pe.patch_size[0]
@@ -122,83 +118,28 @@ def forward(model, x, train, want_tape):
     cls_rows = torch.empty(B, D, dtype=F32, device=x.device)
     ops.copy_rows(h, 0, T * D, cls_rows, 0, D, B, D)
     yc, mc, rc = ops.layernorm_fwd(cls_rows, model.norm.weight, model.norm.bias, model.norm.eps)
-    head = model.head
     feat, t32 = yc, None          # classifier input (bf16 [B, R])
     if model.has_logits:          # pre_logits: tanh(fc(cls row))  (vit_model.py:218-221,254)
         fc = model.pre_logits.fc
         u, _ = ops.gemm(yc, pack.get(fc.weight, 0), bias=fc.bias, out_f32=True)
         t32, feat = ops.tanh_fwd(u)
-    R = feat.shape[1]
-    n_cls = head.out_features
-    n_pad = (n_cls + 7) // 8 * 8
-    bias = None
-    if head.bias is not None:
-        bias = head.bias.detach()
-        if n_pad != n_cls:
-            bias = torch.cat([bias, bias.new_zeros(n_pad - n_cls)])
-    logits, _ = ops.conv2d_fwd(feat.view(B, 1, 1, R), pack.get(head.weight, 0), bias=bias, out_f32=True)
-    logits = logits.view(B, n_pad)
+    logits = common.head_forward(pack, model.head, feat)
     if want_tape:
-        tape["head"] = (cls_rows, yc, mc, rc, n_cls, n_pad, (B, T, D, P), feat, t32)
-    return (logits[:, :n_cls] if n_pad != n_cls else logits), tape
-
-
-def _lin_grads(grads, lin, dy2d, x2d, dy_stats=None):
-    """Weight / bias gradient of a Linear layer from dy [M, N] and its input x [M, K] (both bf16).
-    dy_stats: epilogue column-sum partials of dy when the GEMM that produced dy already summed its columns."""
-    M, N = dy2d.shape
-    K = x2d.shape[1]
-    dst = grads.dest(lin.weight)
-    gb = None
-    if lin.bias is not None and dy_stats is None:
-        # bias gradient = column sums of dy: summed inside the wgrad kernel from the dy tiles it already holds
-        gb = grads.dest(lin.bias)
-        if gb is None:
-            gb = torch.empty(N, dtype=F32, device=dy2d.device)
-    gw = ops.conv2d_wgrad(dy2d.view(M, 1, 1, N), x2d.view(M, 1, 1, K), out=dst.view(N, K, 1, 1) if dst is not None else None,
-                          bias_out=gb)
-    grads.put(lin.weight, gw)
-    if lin.bias is not None:
-        if dy_stats is not None:
-            grads.put(lin.bias, ops.stats_colsum(dy_stats, out=grads.dest(lin.bias)))
-        else:
-            grads.put(lin.bias, gb)
+        tape["head"] = (cls_rows, yc, mc, rc, (B, T, D, P), feat, t32)
+    return logits, tape
 
 
 def backward(model, tape, dlogits, sink=None):
-    grads = _Grads(sink)
+    grads = common.Grads(sink)
     pack = tape["pack"]
-    cls_rows, yc, mc, rc, n_cls, n_pad, (B, T, D, P), feat, t32 = tape["head"]
-    head = model.head
-    R = feat.shape[1]
-    if dlogits.dtype == BF16 and dlogits.shape[1] == n_pad and dlogits.is_contiguous():
-        dl16 = dlogits
-    else:
-        dl = dlogits.contiguous().float()
-        if n_pad != n_cls:
-            dl = torch.cat([dl, dl.new_zeros(B, n_pad - n_cls)], 1).contiguous()
-        dl16 = ops.cast_bf16(dl)
-    dst = grads.dest(head.weight)
-    if dst is not None and n_pad == n_cls:
-        grads.put(head.weight, ops.conv2d_wgrad(dl16.view(B, 1, 1, n_pad), feat.view(B, 1, 1, R), out=dst.view(n_cls, R, 1, 1)))
-    else:
-        gw = ops.conv2d_wgrad(dl16.view(B, 1, 1, n_pad), feat.view(B, 1, 1, R)).view(n_pad, R)[:n_cls]
-        if dst is not None:
-            dst.copy_(gw)
-            gw = dst
-        grads.put(head.weight, gw)
-    if head.bias is not None:
-        grads.put(head.bias, ops.colsum(dl16, cols=n_cls, out=grads.dest(head.bias)))
-    d_yc = ops.conv2d_dgrad(dl16.view(B, 1, 1, n_pad), pack.get(head.weight, 1), (1, 1)).view(B, R)
+    cls_rows, yc, mc, rc, (B, T, D, P), feat, t32 = tape["head"]
+    d_yc = common.head_backward(grads, pack, model.head, feat, dlogits)
     if model.has_logits:
         fc = model.pre_logits.fc
         du = ops.tanh_bwd(d_yc, t32)                      # bf16 [B, R]: d tanh
-        _lin_grads(grads, fc, du, yc)
+        linear_grads(grads, fc, du, yc)
         d_yc, _ = ops.gemm(du, pack.get(fc.weight, 1))    # bf16 [B, D]
-    d_cls, dgn, dbn = ops.layernorm_bwd(d_yc, cls_rows, mc, rc, model.norm.weight, dx_dtype=BF16,
-                                        dgamma=grads.dest(model.norm.weight), dbeta=grads.dest(model.norm.bias))
-    grads.put(model.norm.weight, dgn)
-    grads.put(model.norm.bias, dbn)
+    d_cls = layernorm_backward(grads, model.norm, d_yc, cls_rows, mc, rc)
     g = torch.zeros(B, T, D, dtype=BF16, device=d_cls.device)   # gradient of the residual stream
     ops.copy_rows(d_cls, 0, D, g, 0, T * D, B, D)
     M = B * T
@@ -208,26 +149,20 @@ def backward(model, tape, dlogits, sink=None):
         # (stochastic depth: the branch sees the per-sample scaled gradient, the identity path - `add=g` below - the full one)
         g2 = (g if dp2 is None else ops.rowscale(g, dp2)).view(M, D)
         # h3 = h2 + fc2(gelu(fc1(LN2(h2))))
-        _lin_grads(grads, mlp.fc2, g2, post.view(M, -1))
+        linear_grads(grads, mlp.fc2, g2, post.view(M, -1))
         # dgrad + GELU' in the epilogue, which also sums the columns of d_pre (= fc1 bias gradient) on the way out
         d_pre, _, st_pre = ops.gemm(g2, pack.get(mlp.fc2.weight, 1), act=3, aux_in=dact.view(M, -1), want_stats=True)
-        _lin_grads(grads, mlp.fc1, d_pre, y2.view(M, D), dy_stats=st_pre)
+        linear_grads(grads, mlp.fc1, d_pre, y2.view(M, D), dy_stats=st_pre)
         d_y2, _ = ops.gemm(d_pre, pack.get(mlp.fc1.weight, 1))
-        g, dg2, db2 = ops.layernorm_bwd(d_y2, h2, m2, r2, blk.norm2.weight, add=g, dx_dtype=BF16,
-                                        dgamma=grads.dest(blk.norm2.weight), dbeta=grads.dest(blk.norm2.bias))
-        grads.put(blk.norm2.weight, dg2)
-        grads.put(blk.norm2.bias, db2)
+        g = layernorm_backward(grads, blk.norm2, d_y2, h2, m2, r2, add=g)
         # h2 = h + proj(attention(qkv(LN1(h))))
         g2 = (g if dp1 is None else ops.rowscale(g, dp1)).view(M, D)
-        _lin_grads(grads, att_m.proj, g2, att.view(M, D))
+        linear_grads(grads, att_m.proj, g2, att.view(M, D))
         d_att, _ = ops.gemm(g2, pack.get(att_m.proj.weight, 1))
         dqkv = ops.attention_bwd(qkv, att, d_att.view(B, T, D), lse, H, float(att_m.scale))
-        _lin_grads(grads, att_m.qkv, dqkv.view(M, 3 * D), y1.view(M, D))
+        linear_grads(grads, att_m.qkv, dqkv.view(M, 3 * D), y1.view(M, D))
         d_y1, _ = ops.gemm(dqkv.view(M, 3 * D), pack.get(att_m.qkv.weight, 1))
-        g, dg1, db1 = ops.layernorm_bwd(d_y1, h, m1, r1, blk.norm1.weight, add=g, dx_dtype=BF16,
-                                        dgamma=grads.dest(blk.norm1.weight), dbeta=grads.dest(blk.norm1.bias))
-        grads.put(blk.norm1.weight, dg1)
-        grads.put(blk.norm1.bias, db1)
+        g = layernorm_backward(grads, blk.norm1, d_y1, h, m1, r1, add=g)
         g = g.view(B, T, D)
     # ---- embedding: tokens = [cls ; patches W^T + b] + pos
     grads.put(model.pos_embed, ops.batch_rowsum(g, T * D, B, T * D, out=_flat(grads.dest(model.pos_embed))))
@@ -235,19 +170,7 @@ def backward(model, tape, dlogits, sink=None):
     gp = torch.empty(B, P, D, dtype=BF16, device=g.device)
     ops.copy_rows(g, D, T * D, gp, 0, P * D, B, P * D)          # drop the class-token rows
     a = tape["patches"]
-    pe = model.patch_embed.proj
-    K0 = a.shape[-1]
-    dst = grads.dest(pe.weight)
-    gb = None
-    if pe.bias is not None:
-        gb = grads.dest(pe.bias)
-        if gb is None:
-            gb = torch.empty(D, dtype=F32, device=gp.device)
-    gw = ops.conv2d_wgrad(gp.view(B * P, 1, 1, D), a.view(B * P, 1, 1, K0), out=dst.view(D, K0, 1, 1) if dst is not None else None,
-                          bias_out=gb)
-    grads.put(pe.weight, gw)
-    if pe.bias is not None:
-        grads.put(pe.bias, gb)
+    linear_grads(grads, model.patch_embed.proj, gp.view(B * P, D), a.view(B * P, a.shape[-1]))
     return grads
 
 
@@ -255,32 +178,5 @@ def _flat(t):
     return None if t is None else t.view(-1)
 
 
-class _VitFunction(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, model, *params):
-        want_tape = any(ctx.needs_input_grad[2:])
-        logits, tape = forward(model, x, model.training, want_tape)
-        ctx.model, ctx.tape, ctx.params = model, tape, params
-        return logits
-
-    @staticmethod
-    def backward(ctx, dlogits):
-        if ctx.tape is None:
-            raise RuntimeError("backward called on a forward that recorded no tape")
-        grads = backward(ctx.model, ctx.tape, dlogits)
-        ctx.tape = None
-        out = []
-        for p, need in zip(ctx.params, ctx.needs_input_grad[2:]):
-            gp = grads.get(p.data_ptr()) if need else None
-            out.append(gp.reshape(p.shape) if gp is not None else None)
-        return (None, None, *out)
-
-
 def apply(model, x):
-    if not x.is_cuda:
-        raise RuntimeError("deeplearning_b200 ViT runs on CUDA (sm_90a) tensors only; there is no CPU fallback")
-    params = tuple(model.parameters())
-    if torch.is_grad_enabled() and any(p.requires_grad for p in params):
-        return _VitFunction.apply(x, model, *params)
-    logits, _ = forward(model, x, model.training, False)
-    return logits
+    return common.apply(sys.modules[__name__], "ViT", model, x)
