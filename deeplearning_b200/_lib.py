@@ -137,6 +137,11 @@ SIGNATURES = {
     "b200_se_bwd_reduce": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "b200_se_bwd_coeffs": (_I, [_P] * 12 + [_I, _I, _I, _I] + [_P] * 9),
     "b200_se_bwd_apply": (_I, [_P] * 10 + [_I, _I, _I, _P]),
+    "b200_repvgg_partial_rows": (_I, [_L, _I]),
+    "b200_repvgg_apply": (_I, [_P, _L, _P, _L, _P, _L, _P, _P, _P, _P, _L, _I, _P, _P]),
+    "b200_repvgg_bwd_reduce": (_I, [_P, _P, _P, _L, _P, _L, _P, _L, _L, _I, _P, _P]),
+    "b200_repvgg_bwd_apply": (_I, [_P, _P, _P, _L, _P, _L, _P, _L] + [_P] * 9 + [_L, _I, _P]),
+    "b200_repvgg_fold": (_I, [_P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _F, _P, _P, _P, _P, _F, _I, _I, _I, _P, _P, _P]),
 }
 
 

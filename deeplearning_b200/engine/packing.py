@@ -18,9 +18,15 @@ class ModelPack:
 
     def __init__(self, specs):
         # specs: list of (param, mode, ld, rows_out[, (O, I, taps) override for weights consumed as a flat [O][K] matrix
-        #                 [, oscale parameter: fp32 [O] multiplier folded into the packed copy]])
+        #                 [, oscale parameter: fp32 [O] multiplier folded into the packed copy
+        #                 [, (name, row, col, rows_total): write into the shared operand ``name`` at (row, col)]]])
+        # A shared operand is a zero-initialised [rows_total][ld] matrix that several entries fill (the RepVGG stem's
+        # [3x3 | 1x1] operand, read through ``shared(name)``).  An entry at a column offset also writes its zero padding of
+        # columns [I*taps, ld) there, which runs into the first ``col`` columns of the next row: those cells must be zero
+        # cells no other entry writes, and one spare row takes the last row's overrun.
         self.specs = specs
         self.outputs = {}
+        self._shared = {}
         self._ptrs = None
         self.stamp = None
         dev = specs[0][0].device
@@ -33,10 +39,23 @@ class ModelPack:
             else:
                 O, I = p.shape[0], p.shape[1]
                 taps = p.numel() // (O * I)
-            dst = torch.empty(rows_out, ld, dtype=torch.bfloat16, device=dev)
-            self.outputs[(id(p), mode)] = dst
+            into = spec[6] if len(spec) > 6 else None
+            if into is None:
+                dst = torch.empty(rows_out, ld, dtype=torch.bfloat16, device=dev)
+                self.outputs[(id(p), mode)] = dst
+                ptr = dst.data_ptr()
+            else:
+                name, row, col, rows_total = into
+                buf = self._shared.get(name)
+                if buf is None:
+                    buf = torch.zeros(rows_total + 1, ld, dtype=torch.bfloat16, device=dev)
+                    self._shared[name] = buf
+                if buf.shape[1] != ld or row + rows_out > rows_total or col + I * taps > ld:
+                    raise ValueError(f"ModelPack: entry at ({row}, {col}) of {rows_out} x {I * taps} does not fit the shared "
+                                     f"operand {name!r} [{rows_total}][{buf.shape[1]}]")
+                ptr = buf.data_ptr() + (row * ld + col) * buf.element_size()
             nblk = max(1, min(64, (rows_out * ld + 256 * 16 - 1) // (256 * 16)))
-            rows.append([0, dst.data_ptr(), O, I, taps, mode, ld, first, rows_out, 0])
+            rows.append([0, ptr, O, I, taps, mode, ld, first, rows_out, 0])
             first += nblk
         self.total_blocks = first
         self._rows = rows
@@ -66,6 +85,11 @@ class ModelPack:
 
     def get(self, param, mode):
         return self.outputs.get((id(param), mode))
+
+    def shared(self, name):
+        """The shared operand ``name`` [rows_total][ld] (without its spare row)."""
+        buf = self._shared[name]
+        return buf[: buf.shape[0] - 1]
 
 
 class _WeightCache:

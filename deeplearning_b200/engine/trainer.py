@@ -47,6 +47,12 @@ def _engine_for(model):
         from . import swin
 
         return swin
+    from ..classification.RepVGG.models.repvgg import RepVGG
+
+    if isinstance(model, RepVGG):
+        from . import repvgg
+
+        return repvgg
     raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 

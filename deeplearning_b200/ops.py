@@ -567,6 +567,138 @@ def se_backward(g, y, c, co, csum, pool, h, gate, w1, w2, dw1=None, dw2=None, dg
     return dc, dz, dw1, dw2, dgamma, dbeta
 
 
+# ------------------------------------------------------------------------------ RepVGG block passes (csrc/repvgg.cuh)
+def _pitched(t, C, name):
+    """(pointer, row pitch in elements, rows) of a bf16 CUDA tensor whose last dimension holds C channels and whose rows sit
+    at one constant pitch (a contiguous tensor, or a channel slice [..., a:a+C] of one)."""
+    if t.dtype != BF16 or not t.is_cuda or t.shape[-1] != C or t.stride(-1) != 1:
+        raise ValueError(f"{name}: expected a CUDA bf16 tensor [..., {C}] with unit channel stride, got {t.dtype} "
+                         f"{tuple(t.shape)} strides {t.stride()}")
+    ld = t.stride(-2) if t.dim() >= 2 else C
+    expect = ld
+    for d in range(t.dim() - 2, -1, -1):
+        if t.shape[d] != 1 and t.stride(d) != expect:
+            raise ValueError(f"{name}: rows of {tuple(t.shape)} strides {t.stride()} are not evenly pitched")
+        expect *= t.shape[d]
+    return t.data_ptr(), ld, t.numel() // C
+
+
+def repvgg_partial_rows(rows, C):
+    """T: the number of [2][C] partial rows repvgg_apply(want_stats=True) and repvgg_bwd_reduce write for (rows, C)."""
+    T = _lib.load().b200_repvgg_partial_rows(rows, C)
+    if T <= 0:
+        raise ValueError(f"repvgg: unsupported shape rows={rows} C={C}: {_lib.last_error()}")
+    return T
+
+
+def repvgg_apply(c3, c1, co3, co1, x=None, co_id=None, want_stats=False):
+    """y = relu(bn3(c3) + bn1(c1) [+ bn_id(x)]) with BnCoeffs co3 / co1 / co_id, bf16 contiguous, shaped like c3.  c3, c1, x
+    may be channel slices of wider tensors (the stem's [c3 | c1]).  Returns (y, stats) with stats fp32 [T, 2, C] = sums of
+    the stored y and y^2 when want_stats, else None."""
+    lib = _lib.load()
+    C = c3.shape[-1]
+    p3, ld3, rows = _pitched(c3, C, "c3")
+    p1, ld1, _ = _pitched(c1, C, "c1")
+    px, ldx = (None, 0) if x is None else _pitched(x, C, "x")[:2]
+    y = torch.empty(c3.shape, dtype=BF16, device=c3.device)
+    stats = torch.empty(repvgg_partial_rows(rows, C), 2, C, dtype=F32, device=c3.device) if want_stats else None
+    sp = _span("repvgg_apply", 0.0, _nb(c3, c1, x, y))
+    rc = lib.b200_repvgg_apply(p3, ld3, p1, ld1, px, ldx, _p(co3.mean), _p(co1.mean), None if co_id is None else _p(co_id.mean),
+                               _p(y), rows, C, _p(stats), _stream())   # co.mean starts the BnCoeffs [4][C] buffer
+    _lib.check(rc, "b200_repvgg_apply")
+    if sp:
+        sp.end()
+    return y, stats
+
+
+def repvgg_bwd_reduce(g, y, c3, c1, x=None):
+    """dz = g * [y > 0]; returns partial fp32 [nb, T, 2, C] (nb = 2, or 3 with x): {sum dz, sum dz * input} per branch (dense,
+    1x1, identity), each [T, 2, C] slab ready for bn_bwd_finalize."""
+    lib = _lib.load()
+    _chk_act(g, "g")
+    _chk_act(y, "y")
+    C = y.shape[-1]
+    p3, ld3, rows = _pitched(c3, C, "c3")
+    p1, ld1, _ = _pitched(c1, C, "c1")
+    px, ldx = (None, 0) if x is None else _pitched(x, C, "x")[:2]
+    nb = 2 if x is None else 3
+    partial = torch.empty(nb, repvgg_partial_rows(rows, C), 2, C, dtype=F32, device=y.device)
+    sp = _span("repvgg_bwd_reduce", 0.0, _nb(g, y, c3, c1, x))
+    rc = lib.b200_repvgg_bwd_reduce(_p(g), _p(y), p3, ld3, p1, ld1, px, ldx, rows, C, _p(partial), _stream())
+    _lib.check(rc, "b200_repvgg_bwd_reduce")
+    if sp:
+        sp.end()
+    return partial
+
+
+def bn_bwd_finalize(partial, count, co, dgamma=None, dbeta=None):
+    """dgamma, dbeta and m = {m1, m2} fp32 [2, C] of a train-mode BatchNorm from partial [T, 2, C] = {sum dz, sum dz * x}
+    (x the raw BatchNorm input, co its BnCoeffs)."""
+    lib = _lib.load()
+    T, _, C = partial.shape
+    dev = partial.device
+    if dgamma is None:
+        dgamma = torch.empty(C, dtype=F32, device=dev)
+    if dbeta is None:
+        dbeta = torch.empty(C, dtype=F32, device=dev)
+    m = torch.empty(2, C, dtype=F32, device=dev)
+    sc = _reduce_scratch(dev)
+    rc = lib.b200_bn_bwd_finalize(_p(partial), T, C, float(count), _p(dgamma), _p(dbeta), 0, _p(m[0]), _p(m[1]), _p(co.mean),
+                                  _p(co.invstd), _p(sc), sc.numel(), _stream())
+    _lib.check(rc, "b200_bn_bwd_finalize")
+    return dgamma, dbeta, m
+
+
+def repvgg_bwd_apply(g, y, c3, c1, co3, m3, co1, m1, x=None, co_id=None, m_id=None, out=None):
+    """(dc3, dc1, dx): BatchNorm backward of every branch of y = relu(bn3(c3) + bn1(c1) [+ bn_id(x)]) for g = dL/dy, with m_*
+    from bn_bwd_finalize.  dx (None without x) is the identity branch's data gradient.  ``out`` = (dc3, dc1, dx) buffers laid
+    out like c3, c1, x (the stem writes [dc3 | dc1] into one tensor); by default each is allocated with its input's strides."""
+    lib = _lib.load()
+    _chk_act(g, "g")
+    _chk_act(y, "y")
+    C = y.shape[-1]
+    p3, ld3, rows = _pitched(c3, C, "c3")
+    p1, ld1, _ = _pitched(c1, C, "c1")
+    px, ldx = (None, 0) if x is None else _pitched(x, C, "x")[:2]
+    if out is None:
+        out = tuple(None if t is None else torch.empty_strided(t.shape, t.stride(), dtype=BF16, device=y.device)
+                    for t in (c3, c1, x))
+    for o, ld, name in ((out[0], ld3, "dc3"), (out[1], ld1, "dc1")) + (((out[2], ldx, "dx"),) if x is not None else ()):
+        if _pitched(o, C, name)[1:] != (ld, rows):
+            raise ValueError(f"repvgg_bwd_apply: {name} must have the row pitch of its input ({ld})")
+    sp = _span("repvgg_bwd_apply", 0.0, _nb(g, y, c3, c1, x, out[0], out[1], out[2]))
+    rc = lib.b200_repvgg_bwd_apply(_p(g), _p(y), p3, ld3, p1, ld1, px, ldx, _p(co3.mean), _p(m3), _p(co1.mean), _p(m1),
+                                   None if co_id is None else _p(co_id.mean), _p(m_id), _p(out[0]), _p(out[1]), _p(out[2]),
+                                   rows, C, _stream())
+    _lib.check(rc, "b200_repvgg_bwd_apply")
+    if sp:
+        sp.end()
+    return out
+
+
+def _bn_fold_args(bn):
+    if bn is None:
+        return [None, None, None, None, 0.0]
+    return [_p(bn.weight), _p(bn.bias), _p(bn.running_mean), _p(bn.running_var), float(bn.eps)]
+
+
+def repvgg_fold(w3, w1, bn3, bn1, bn_id=None, ldk=None):
+    """Eval-mode re-parameterisation of a RepVGG block from its fp32 parameters and running statistics: the bf16 forward
+    operand [O][ldk] (k = tap * I + i, ldk defaults to 9 * I) of the equivalent 3x3 convolution and its fp32 bias [O]."""
+    lib = _lib.load()
+    w3, w1 = _f32_param(w3), _f32_param(w1)
+    O, I = w3.shape[0], w3.shape[1]
+    if tuple(w3.shape) != (O, I, 3, 3) or w1.numel() != O * I:
+        raise ValueError(f"repvgg_fold: weights {tuple(w3.shape)} / {tuple(w1.shape)} are not a 3x3 / 1x1 pair")
+    ldk = 9 * I if ldk is None else ldk
+    wp = torch.empty(O, ldk, dtype=BF16, device=w3.device)
+    bias = torch.empty(O, dtype=F32, device=w3.device)
+    rc = lib.b200_repvgg_fold(_p(w3), _p(w1), *_bn_fold_args(bn3), *_bn_fold_args(bn1), *_bn_fold_args(bn_id), O, I, ldk,
+                              _p(wp), _p(bias), _stream())
+    _lib.check(rc, "b200_repvgg_fold")
+    return wp, bias
+
+
 # ------------------------------------------------------------------------------ BatchNorm folded through a 1x1 convolution
 def gram_colsum(y2):
     """y2 bf16 [..., K] -> (G = y2^T y2 fp32 [K, K], s = column sums fp32 [K]): everything train-mode BatchNorm needs to know

@@ -418,6 +418,39 @@ int b200_se_bwd_apply(const void* dz, const void* c, void* dc, const float* gate
                       const float* mean, const float* invstd, const float* m1, const float* m2, int B, int HW, int C,
                       void* stream);
 
+/* ---- RepVGG block (classification/RepVGG/models/repvgg.py RepVGGBlock, train form):
+ *     y = relu(bn_dense(conv3x3(x)) + bn_1x1(conv1x1(x)) [+ bn_identity(x)])
+ * c3 / c1 are the raw bf16 outputs of the two convolutions and x the block input, each [rows] rows of C channels at a row
+ * pitch ld3 / ld1 / ldx (elements): the stem keeps [c3 | c1] in one [rows][2C] GEMM output.  co_* are fp32 [4][C] =
+ * {mean, invstd, scale, shift} of a BatchNorm (b200_bn_finalize's outputs, contiguous), m_* fp32 [2][C] = {m1, m2} of
+ * b200_bn_bwd_finalize.  The identity operands (x, co_id, m_id, dx) are all NULL for a block without an identity branch.
+ * Scope: C a multiple of 8 in [8, 8192], rows >= 1, pitches multiples of 8 and >= C, 16-byte aligned pointers; anything
+ * else returns B200_EINVAL with a message and launches nothing.  All sums are fp32 in a fixed order (no atomics).
+ * partial_rows: T, the number of [2][C] partial rows the apply (stats) and reduce passes write for (rows, C); -1 if invalid.
+ * apply:      y [rows][C] = relu(c3 s3 + c1 s1 [+ x s_id] + t3 + t1 [+ t_id]); stats (optional) fp32 [T][2][C] = sums of the
+ *             stored bf16 y and y^2 (the batch statistics of the next block's identity BatchNorm, for b200_bn_finalize)
+ * bwd_reduce: dz = g [y > 0]; partial fp32 [nb][T][2][C] (nb = 2, or 3 with x): branch b = dense, 1x1, identity holds
+ *             {sum dz, sum dz * input_b}, the rows b200_bn_bwd_finalize reads with that branch's mean / invstd
+ * bwd_apply:  dc_b = scale_b (dz - m1_b - (input_b - mean_b) invstd_b m2_b) for every branch (dz recomputed from g and y);
+ *             dc3, dc1, dx are written at the pitches of c3, c1, x
+ * fold:       eval-mode re-parameterisation (get_equivalent_kernel_bias, repvgg.py): wp bf16 [O][ldk], k = tap * I + i,
+ *             = W3 t3 + pad(W1) t1 [+ I t_id] (zero for k >= 9 I), bias fp32 [O] = sum_b (beta_b - mean_b t_b),
+ *             t = gamma / sqrt(running_var + eps); the identity BatchNorm (all four pointers NULL if absent) needs O == I */
+int b200_repvgg_partial_rows(long long rows, int C);
+int b200_repvgg_apply(const void* c3, long long ld3, const void* c1, long long ld1, const void* x, long long ldx,
+                      const float* co3, const float* co1, const float* co_id, void* y, long long rows, int C, float* stats,
+                      void* stream);
+int b200_repvgg_bwd_reduce(const void* g, const void* y, const void* c3, long long ld3, const void* c1, long long ld1,
+                           const void* x, long long ldx, long long rows, int C, float* partial, void* stream);
+int b200_repvgg_bwd_apply(const void* g, const void* y, const void* c3, long long ld3, const void* c1, long long ld1,
+                          const void* x, long long ldx, const float* co3, const float* m3, const float* co1, const float* m1,
+                          const float* co_id, const float* m_id, void* dc3, void* dc1, void* dx, long long rows, int C,
+                          void* stream);
+int b200_repvgg_fold(const float* w3, const float* w1, const float* gamma3, const float* beta3, const float* mean3,
+                     const float* var3, float eps3, const float* gamma1, const float* beta1, const float* mean1,
+                     const float* var1, float eps1, const float* gamma_id, const float* beta_id, const float* mean_id,
+                     const float* var_id, float eps_id, int O, int I, int ldk, void* wp, float* bias, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
