@@ -142,6 +142,20 @@ SIGNATURES = {
     "b200_repvgg_bwd_reduce": (_I, [_P, _P, _P, _L, _P, _L, _P, _L, _L, _I, _P, _P]),
     "b200_repvgg_bwd_apply": (_I, [_P, _P, _P, _L, _P, _L, _P, _L] + [_P] * 9 + [_L, _I, _P]),
     "b200_repvgg_fold": (_I, [_P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _F, _P, _P, _P, _P, _F, _I, _I, _I, _P, _P, _P]),
+    "b200_dw_partial_rows": (_I, [_L, _I]),
+    "b200_dw_fwd": (_I, [_P] * 6 + [_I] * 6 + [_P]),
+    "b200_dw_dgrad": (_I, [_P] * 8 + [_I] * 6 + [_P]),
+    "b200_dw_wgrad_workspace_bytes": (c_size_t, [_I] * 6),
+    "b200_dw_wgrad": (_I, [_P] * 6 + [c_size_t] + [_I] * 6 + [_P]),
+    "b200_silu_bn_squeeze": (_I, [_P] * 6 + [_I] * 3 + [_P]),
+    "b200_excite_fwd": (_I, [_P] * 7 + [_I] * 3 + [_P]),
+    "b200_excite_bwd": (_I, [_P] * 13 + [_I] * 3 + [_P]),
+    "b200_gate_apply": (_I, [_P] * 5 + [_I] * 3 + [_P]),
+    "b200_gate_reduce": (_I, [_P] * 5 + [_I] * 3 + [_P]),
+    "b200_silu_bn_bwd_reduce": (_I, [_P] * 8 + [_I] * 3 + [_P]),
+    "b200_tail_apply": (_I, [_P] * 6 + [_I] * 3 + [_P]),
+    "b200_tail_bwd_reduce": (_I, [_P] * 5 + [_I] * 3 + [_P]),
+    "b200_bn_bwd_apply_dz": (_I, [_P] * 5 + [_L, _I, _P]),
 }
 
 

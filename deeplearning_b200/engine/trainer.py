@@ -53,6 +53,12 @@ def _engine_for(model):
         from . import repvgg
 
         return repvgg
+    from ..classification.efficientNet.models.network import EfficientNet
+
+    if isinstance(model, EfficientNet):
+        from . import efficientnet
+
+        return efficientnet
     raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 

@@ -699,6 +699,233 @@ def repvgg_fold(w3, w1, bn3, bn1, bn_id=None, ldk=None):
     return wp, bias
 
 
+# ------------------------------------------------------------------------------ EfficientNet MBConv passes (csrc/mbconv.cuh)
+def _mb_rows(fn, rows, C):
+    T = fn(rows, C)
+    if T <= 0:
+        raise ValueError(f"mbconv: unsupported shape rows={rows} C={C}")
+    return T
+
+
+def _dw_args(x, k, stride):
+    _chk_act(x, "x")
+    B, H, W, C = x.shape
+    if k not in (3, 5) or stride not in (1, 2):
+        raise ValueError(f"depthwise: k must be 3 or 5 and stride 1 or 2 (got k={k} stride={stride})")
+    return B, H, W, C, (H - 1) // stride + 1, (W - 1) // stride + 1
+
+
+def dw_fwd(x, w, k, stride, co=None, want_stats=False):
+    """Depthwise k x k convolution (padding k // 2) of x bf16 [B,H,W,C] with the fp32 weight [C,1,k,k]; with BnCoeffs ``co``
+    the input is silu(x * scale + shift) (the previous BatchNorm + SiLU applied on load).  Returns (d bf16 [B,Ho,Wo,C],
+    stats fp32 [T,2,C] of the stored d, or None)."""
+    lib = _lib.load()
+    B, H, W, C, Ho, Wo = _dw_args(x, k, stride)
+    w = _f32_param(w)
+    d = torch.empty(B, Ho, Wo, C, dtype=BF16, device=x.device)
+    stats = None
+    if want_stats:
+        stats = torch.empty(_mb_rows(lib.b200_dw_partial_rows, B * Ho * Wo, C), 2, C, dtype=F32, device=x.device)
+    sp = _span("dw_fwd", 2.0 * d.numel() * k * k, _nb(x, d))
+    rc = lib.b200_dw_fwd(_p(x), _p(w), None if co is None else _p(co.scale), None if co is None else _p(co.shift), _p(d),
+                         _p(stats), B, H, W, C, k, stride, _stream())
+    _lib.check(rc, "b200_dw_fwd")
+    if sp:
+        sp.end()
+    return d, stats
+
+
+def dw_dgrad(dd, w, x, k, stride, co=None, residual=None):
+    """Data gradient of dw_fwd for dd = dL/dd.  With BnCoeffs ``co`` (x the raw input normalised on load) returns
+    (dz, partial): dz = g_in * silu'(x * scale + shift) bf16 and partial fp32 [T,2,C] = {sum dz, sum dz * x}; otherwise
+    (g_in (+ residual), None)."""
+    lib = _lib.load()
+    _chk_act(dd, "dd")
+    B, H, W, C, Ho, Wo = _dw_args(x, k, stride)
+    if tuple(dd.shape) != (B, Ho, Wo, C):
+        raise ValueError(f"dw_dgrad: dd {tuple(dd.shape)} does not match the output of x {tuple(x.shape)}")
+    w = _f32_param(w)
+    dx = torch.empty_like(x)
+    partial = None
+    if co is not None:
+        partial = torch.empty(_mb_rows(lib.b200_dw_partial_rows, B * H * W, C), 2, C, dtype=F32, device=x.device)
+    sp = _span("dw_dgrad", 2.0 * dd.numel() * k * k, _nb(dd, x if co is not None else None, residual, dx))
+    rc = lib.b200_dw_dgrad(_p(dd), _p(w), _p(x), None if co is None else _p(co.scale), None if co is None else _p(co.shift),
+                           _p(residual), _p(dx), _p(partial), B, H, W, C, k, stride, _stream())
+    _lib.check(rc, "b200_dw_dgrad")
+    if sp:
+        sp.end()
+    return dx, partial
+
+
+def dw_wgrad(dd, x, k, stride, co=None, out=None):
+    """Weight gradient fp32 [C, 1, k, k] of dw_fwd (``out`` receives it when given)."""
+    lib = _lib.load()
+    _chk_act(dd, "dd")
+    B, H, W, C, Ho, Wo = _dw_args(x, k, stride)
+    nbytes = lib.b200_dw_wgrad_workspace_bytes(B, H, W, C, k, stride)
+    ws = _workspace(nbytes, x.device)
+    if out is None:
+        out = torch.empty(C, 1, k, k, dtype=F32, device=x.device)
+    sp = _span("dw_wgrad", 2.0 * dd.numel() * k * k, _nb(dd, x))
+    rc = lib.b200_dw_wgrad(_p(dd), _p(x), None if co is None else _p(co.scale), None if co is None else _p(co.shift),
+                           _p(out), _p(ws), nbytes, B, H, W, C, k, stride, _stream())
+    _lib.check(rc, "b200_dw_wgrad")
+    if sp:
+        sp.end()
+    return out
+
+
+def silu_bn_squeeze(d, co, mask=None):
+    """pool fp32 [B, C] = mean over pixels of silu(d * scale + shift); with ``mask`` fp32 [B, C] also returns the bf16
+    [B, C] product pool * mask (the classifier input after dropout).  Returns (pool, masked or None)."""
+    lib = _lib.load()
+    _chk_act(d, "d")
+    B, H, W, C = d.shape
+    pool = torch.empty(B, C, dtype=F32, device=d.device)
+    out16 = torch.empty(B, C, dtype=BF16, device=d.device) if mask is not None else None
+    if mask is not None:
+        mask = mask.contiguous()
+    sp = _span("silu_bn_squeeze", 0.0, _nb(d, pool))
+    rc = lib.b200_silu_bn_squeeze(_p(d), _p(co.scale), _p(co.shift), _p(mask), _p(pool), _p(out16), B, H * W, C, _stream())
+    _lib.check(rc, "b200_silu_bn_squeeze")
+    if sp:
+        sp.end()
+    return pool, out16
+
+
+def excite_fwd(pool, w1, b1, w2, b2):
+    """SELayer.fc with biases on fp32 [B, C]: hpre = pool w1^T + b1 [B, Cr], gate = sigmoid(silu(hpre) w2^T + b2) [B, C]."""
+    lib = _lib.load()
+    B, C = pool.shape
+    w1, w2, b1, b2 = _f32_param(w1), _f32_param(w2), _f32_param(b1), _f32_param(b2)
+    Cr = w1.shape[0]
+    if w1.numel() != Cr * C or w2.numel() != C * Cr or b1.numel() != Cr or b2.numel() != C:
+        raise ValueError(f"excite_fwd: weights {tuple(w1.shape)} / {tuple(w2.shape)} do not match C={C}")
+    hpre = torch.empty(B, Cr, dtype=F32, device=pool.device)
+    gate = torch.empty(B, C, dtype=F32, device=pool.device)
+    sp = _span("excite_fwd", 4.0 * B * C * Cr, _nb(pool, w1, w2, gate))
+    rc = lib.b200_excite_fwd(_p(pool), _p(w1), _p(b1), _p(w2), _p(b2), _p(hpre), _p(gate), B, C, Cr, _stream())
+    _lib.check(rc, "b200_excite_fwd")
+    if sp:
+        sp.end()
+    return hpre, gate
+
+
+def excite_bwd(s, pool, hpre, gate, w1, w2, dw1=None, db1=None, dw2=None, db2=None):
+    """Backward of excite_fwd from s = sum_p dL/da * silu(u) [B, C] (gate_reduce).  Returns (dpool [B, C], dw1 [Cr, C],
+    db1 [Cr], dw2 [C, Cr], db2 [C]), written into the given buffers when passed."""
+    lib = _lib.load()
+    B, C = pool.shape
+    w1, w2 = _f32_param(w1), _f32_param(w2)
+    Cr = w1.shape[0]
+    dev = pool.device
+    dw1 = torch.empty(Cr, C, dtype=F32, device=dev) if dw1 is None else dw1
+    db1 = torch.empty(Cr, dtype=F32, device=dev) if db1 is None else db1
+    dw2 = torch.empty(C, Cr, dtype=F32, device=dev) if dw2 is None else dw2
+    db2 = torch.empty(C, dtype=F32, device=dev) if db2 is None else db2
+    scratch = torch.empty(B, C + Cr, dtype=F32, device=dev)
+    dpool = torch.empty(B, C, dtype=F32, device=dev)
+    sp = _span("excite_bwd", 8.0 * B * C * Cr)
+    rc = lib.b200_excite_bwd(_p(s), _p(pool), _p(hpre), _p(gate), _p(w1), _p(w2), _p(scratch), _p(scratch) + 4 * B * C,
+                             _p(dw1), _p(db1), _p(dw2), _p(db2), _p(dpool), B, C, Cr, _stream())
+    _lib.check(rc, "b200_excite_bwd")
+    if sp:
+        sp.end()
+    return dpool, dw1, db1, dw2, db2
+
+
+def gate_apply(d, co, gate):
+    """a = silu(d * scale + shift) * gate[b] bf16 [B,H,W,C] (SELayer's x * y on the depthwise BatchNorm + SiLU output)."""
+    lib = _lib.load()
+    _chk_act(d, "d")
+    B, H, W, C = d.shape
+    a = torch.empty_like(d)
+    sp = _span("gate_apply", 0.0, _nb(d, a))
+    rc = lib.b200_gate_apply(_p(d), _p(co.scale), _p(co.shift), _p(gate), _p(a), B, H * W, C, _stream())
+    _lib.check(rc, "b200_gate_apply")
+    if sp:
+        sp.end()
+    return a
+
+
+def gate_reduce(da, d, co):
+    """s fp32 [B, C] = sum over pixels of da * silu(d * scale + shift)."""
+    lib = _lib.load()
+    _chk_act(da, "da")
+    _chk_act(d, "d")
+    B, H, W, C = d.shape
+    s = torch.empty(B, C, dtype=F32, device=d.device)
+    sp = _span("gate_reduce", 0.0, _nb(da, d))
+    rc = lib.b200_gate_reduce(_p(da), _p(d), _p(co.scale), _p(co.shift), _p(s), B, H * W, C, _stream())
+    _lib.check(rc, "b200_gate_reduce")
+    if sp:
+        sp.end()
+    return s
+
+
+def silu_bn_bwd_reduce(d, co, dpool, da=None, gate=None):
+    """dz = (da * gate + dpool / HW) * silu'(d * scale + shift) bf16 and partial fp32 [T,2,C] = {sum dz, sum dz * d}."""
+    lib = _lib.load()
+    _chk_act(d, "d")
+    B, H, W, C = d.shape
+    dz = torch.empty_like(d)
+    partial = torch.empty(repvgg_partial_rows(B * H * W, C), 2, C, dtype=F32, device=d.device)
+    sp = _span("silu_bn_bwd_reduce", 0.0, _nb(da, d, dz))
+    rc = lib.b200_silu_bn_bwd_reduce(_p(da), _p(gate), _p(dpool), _p(d), _p(co.scale), _p(co.shift), _p(dz), _p(partial),
+                                     B, H * W, C, _stream())
+    _lib.check(rc, "b200_silu_bn_bwd_reduce")
+    if sp:
+        sp.end()
+    return dz, partial
+
+
+def tail_apply(c, co, rs=None, residual=None):
+    """y = (c * scale + shift) * rs[b] (+ residual) bf16: the project BatchNorm, drop-connect multiplier and shortcut."""
+    lib = _lib.load()
+    _chk_act(c, "c")
+    B, H, W, C = c.shape
+    y = torch.empty_like(c)
+    sp = _span("tail_apply", 0.0, _nb(c, residual, y))
+    rc = lib.b200_tail_apply(_p(c), _p(co.scale), _p(co.shift), _p(rs), _p(residual), _p(y), B, H * W, C, _stream())
+    _lib.check(rc, "b200_tail_apply")
+    if sp:
+        sp.end()
+    return y
+
+
+def tail_bwd_reduce(g, c, rs=None):
+    """dz = g * rs[b] (g itself without rs) and partial fp32 [T,2,C] = {sum dz, sum dz * c}.  Returns (dz, partial)."""
+    lib = _lib.load()
+    _chk_act(g, "g")
+    _chk_act(c, "c")
+    B, H, W, C = c.shape
+    dz = torch.empty_like(g) if rs is not None else None
+    partial = torch.empty(repvgg_partial_rows(B * H * W, C), 2, C, dtype=F32, device=c.device)
+    sp = _span("tail_bwd_reduce", 0.0, _nb(g, c, dz))
+    rc = lib.b200_tail_bwd_reduce(_p(g), _p(rs), _p(c), _p(dz), _p(partial), B, H * W, C, _stream())
+    _lib.check(rc, "b200_tail_bwd_reduce")
+    if sp:
+        sp.end()
+    return (g if dz is None else dz), partial
+
+
+def bn_bwd_apply_dz(dz, c, co, m):
+    """dc = scale * (dz - m1 - (c - mean) * invstd * m2) bf16: the BatchNorm backward apply from a stored dz (m from
+    bn_bwd_finalize)."""
+    lib = _lib.load()
+    _chk_act(dz, "dz")
+    _chk_act(c, "c")
+    C = c.shape[-1]
+    dc = torch.empty_like(c)
+    sp = _span("bn_bwd_apply_dz", 0.0, _nb(dz, c, dc))
+    rc = lib.b200_bn_bwd_apply_dz(_p(dz), _p(c), _p(co.mean), _p(m), _p(dc), c.numel() // C, C, _stream())
+    _lib.check(rc, "b200_bn_bwd_apply_dz")
+    if sp:
+        sp.end()
+    return dc
+
+
 # ------------------------------------------------------------------------------ BatchNorm folded through a 1x1 convolution
 def gram_colsum(y2):
     """y2 bf16 [..., K] -> (G = y2^T y2 fp32 [K, K], s = column sums fp32 [K]): everything train-mode BatchNorm needs to know

@@ -451,6 +451,68 @@ int b200_repvgg_fold(const float* w3, const float* w1, const float* gamma3, cons
                      const float* var1, float eps1, const float* gamma_id, const float* beta_id, const float* mean_id,
                      const float* var_id, float eps_id, int O, int I, int ldk, void* wp, float* bias, void* stream);
 
+/* ---- EfficientNet MBConv block (classification/efficientNet/models/network.py MBConv:176-242, SELayer:126-145,
+ * ConvBNAction:97-122).  Activations are NHWC bf16 [B][H][W][C] (rows = B*H*W), 16-byte aligned; scale / shift are the
+ * fp32 [C] coefficients of a BatchNorm (batch statistics in train mode, running statistics in eval mode), co fp32 [4][C] =
+ * {mean, invstd, scale, shift} (b200_bn_finalize's outputs, contiguous), m fp32 [2][C] = {m1, m2} of b200_bn_bwd_finalize;
+ * per-image vectors are fp32 [B][C] or [B][Cr].  Partial rows are fp32 [T][2][C] = {sum v, sum v * input}, the layout
+ * b200_bn_finalize / b200_bn_bwd_finalize read.  Scope: C a multiple of 8 in [8, 8192], 1 <= B <= 65535, HW >= 1,
+ * 1 <= Cr <= 256, depthwise k in {3, 5} with padding k/2 and stride 1 or 2 (any H, W >= 1); anything else returns
+ * B200_EINVAL with a message and launches nothing.  All sums are fp32 in a fixed order (no atomics).
+ * The streaming passes (silu_bn_bwd_reduce, tail_bwd_reduce) write b200_repvgg_partial_rows(rows, C) partial rows: they
+ * share the RepVGG passes' row geometry.
+ * dw_partial_rows: T of dw_fwd (rows = output pixels) and dw_dgrad (rows = input pixels); -1 if invalid
+ * dw_fwd:      the dwconv of ConvBNAction(groups=C) (network.py:113-120): d = dwconv_kxk(in), w = the fp32 weight [C][k*k];
+ *              in = silu(x * scale + shift) when scale is given (the previous BatchNorm + SiLU applied on load), else x;
+ *              stats (optional) = sums of the stored d and d^2
+ * dw_dgrad:    g_in = the data gradient of dw_fwd for dd = dL/dd; with scale (x = the raw input): dx = g_in silu'(x scale +
+ *              shift) and partial = {sum dx, sum dx x}; otherwise dx = g_in (+ residual)
+ * dw_wgrad:    dw fp32 [C][k*k] = sum over pixels of dd * in (in as in dw_fwd), written (not accumulated); ws is scratch of
+ *              dw_wgrad_workspace_bytes
+ * silu_bn_squeeze: SELayer.avg_pool / EfficientNet.avgpool (network.py:143, :359) of silu(d * scale + shift): pool fp32
+ *              [B][C]; with mask fp32 [B][C] also out16 bf16 [B][C] = pool * mask (the classifier dropout, :340)
+ * excite_fwd:  SELayer.fc (network.py:134-139): hpre = pool w1^T + b1 [B][Cr], gate = sigmoid(silu(hpre) w2^T + b2) [B][C];
+ *              w1 fp32 [Cr][C], w2 fp32 [C][Cr]
+ * excite_bwd:  from s = sum_p dL/da * silu(u) [B][C] (gate_reduce): dgp = s gate (1 - gate) [B][C] and dhp = (dgp w2)
+ *              silu'(hpre) [B][Cr] (scratch the caller provides), dw1 [Cr][C], db1 [Cr], dw2 [C][Cr], db2 [C] (written,
+ *              not accumulated) and dpool = dhp w1 [B][C]
+ * gate_apply:  SELayer.forward's x * y (network.py:145): a = silu(d * scale + shift) * gate
+ * gate_reduce: s [B][C] = sum_p da * silu(d * scale + shift)
+ * silu_bn_bwd_reduce: dz = (da * gate + dpool / HW) * silu'(d * scale + shift) (da and gate optional together) stored bf16,
+ *              partial = {sum dz, sum dz d}
+ * tail_apply:  project BatchNorm, DropPath and shortcut (network.py:237-242): y = (c * scale + shift) * rs[b] (+ residual);
+ *              rs fp32 [B] (the per-sample drop-connect multiplier) and residual optional
+ * tail_bwd_reduce: dz = g * rs[b] stored bf16 (dz and rs both or neither; without them dz = g), partial = {sum dz, sum dz c}
+ * bn_bwd_apply_dz: train-mode BatchNorm backward apply from a stored dz: dc = scale (dz - m1 - (c - mean) invstd m2) */
+int b200_dw_partial_rows(long long rows, int C);
+int b200_dw_fwd(const void* x, const float* w, const float* scale, const float* shift, void* d, float* stats, int B, int H,
+                int W, int C, int k, int stride, void* stream);
+int b200_dw_dgrad(const void* dd, const float* w, const void* x, const float* scale, const float* shift,
+                  const void* residual, void* dx, float* partial, int B, int H, int W, int C, int k, int stride,
+                  void* stream);
+size_t b200_dw_wgrad_workspace_bytes(int B, int H, int W, int C, int k, int stride);
+int b200_dw_wgrad(const void* dd, const void* x, const float* scale, const float* shift, float* dw, void* ws,
+                  size_t ws_bytes, int B, int H, int W, int C, int k, int stride, void* stream);
+int b200_silu_bn_squeeze(const void* d, const float* scale, const float* shift, const float* mask, float* pool,
+                         void* out16, int B, int HW, int C, void* stream);
+int b200_excite_fwd(const float* pool, const float* w1, const float* b1, const float* w2, const float* b2, float* hpre,
+                    float* gate, int B, int C, int Cr, void* stream);
+int b200_excite_bwd(const float* s, const float* pool, const float* hpre, const float* gate, const float* w1,
+                    const float* w2, float* dgp, float* dhp, float* dw1, float* db1, float* dw2, float* db2, float* dpool,
+                    int B, int C, int Cr, void* stream);
+int b200_gate_apply(const void* d, const float* scale, const float* shift, const float* gate, void* a, int B, int HW, int C,
+                    void* stream);
+int b200_gate_reduce(const void* da, const void* d, const float* scale, const float* shift, float* s, int B, int HW, int C,
+                     void* stream);
+int b200_silu_bn_bwd_reduce(const void* da, const float* gate, const float* dpool, const void* d, const float* scale,
+                            const float* shift, void* dz, float* partial, int B, int HW, int C, void* stream);
+int b200_tail_apply(const void* c, const float* scale, const float* shift, const float* rs, const void* residual, void* y,
+                    int B, int HW, int C, void* stream);
+int b200_tail_bwd_reduce(const void* g, const float* rs, const void* c, void* dz, float* partial, int B, int HW, int C,
+                         void* stream);
+int b200_bn_bwd_apply_dz(const void* dz, const void* c, const float* co, const float* m, void* dc, long long rows, int C,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif
