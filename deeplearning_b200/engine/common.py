@@ -111,6 +111,18 @@ def linear_grads(grads, lin, dy2d, x2d, dy_stats=None):
             grads.put(lin.bias, gb)
 
 
+def check_layernorm_widths(named_widths, want_tape):
+    """NotImplementedError naming the first LayerNorm (``(name, width)`` pairs) wider than the forward kernel takes, or,
+    when a backward pass will follow (``want_tape``), wider than the backward kernel takes."""
+    for name, C in named_widths:
+        if C > ops.LAYERNORM_FWD_MAX_C:
+            raise NotImplementedError(f"{name}: LayerNorm over {C} channels; the LayerNorm kernel takes at most "
+                                      f"{ops.LAYERNORM_FWD_MAX_C}")
+        if want_tape and C > ops.LAYERNORM_BWD_MAX_C:
+            raise NotImplementedError(f"{name}: LayerNorm over {C} channels; the LayerNorm backward kernel takes at most "
+                                      f"{ops.LAYERNORM_BWD_MAX_C}, so the GPU engine runs this model without gradients only")
+
+
 def layernorm_backward(grads, norm, dy, x, mean, rstd, add=None):
     """bf16 dx (+ ``add``) of LayerNorm ``norm``; records the weight and then the bias gradient."""
     dx, dgamma, dbeta = ops.layernorm_bwd(dy, x, mean, rstd, norm.weight, add=add, dx_dtype=BF16,

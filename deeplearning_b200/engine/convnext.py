@@ -59,9 +59,11 @@ class _PackSpec:
 _pack_spec = _PackSpec()
 
 
-def _check(model):
+def _check(model, want_tape=False):
     if not isinstance(model.head, nn.Linear):
         raise NotImplementedError("model.head must be an nn.Linear")
+    common.check_layernorm_widths(((name, m.normalized_shape[-1]) for name, m in model.named_modules()
+                                   if hasattr(m, "normalized_shape")), want_tape)
 
 
 class _DwCache:
@@ -87,7 +89,7 @@ _dw_cache = _DwCache()
 
 
 def forward(model, x, train, want_tape):
-    _check(model)
+    _check(model, want_tape)
     x = common.image_input(model, x)
     B = x.shape[0]
     pack = weight_cache.model_pack(model, _pack_spec)

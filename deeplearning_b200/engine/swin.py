@@ -55,7 +55,7 @@ class _PackSpec:
 _pack_spec = _PackSpec()
 
 
-def _check(model):
+def _check(model, want_tape=False):
     if model.ape:
         raise NotImplementedError("absolute position embedding (ape=True) is not implemented on this engine")
     if model.patch_embed.norm is None:
@@ -71,10 +71,18 @@ def _check(model):
             raise NotImplementedError("the window-attention kernel is built for window_size 7 and head_dim 32")
         if not isinstance(blk.mlp.act, nn.GELU):
             raise NotImplementedError("Mlp activation must be nn.GELU (exact erf)")
+    for i, layer in enumerate(model.layers):
+        if layer.downsample is not None and 4 * layer.dim > ops.PATCH_MERGE_LN_MAX_C:
+            raise NotImplementedError(f"layers.{i}.downsample: patch merging of {layer.dim} channels runs a LayerNorm over "
+                                      f"4 * {layer.dim} = {4 * layer.dim}; the patch-merge kernels take at most "
+                                      f"{ops.PATCH_MERGE_LN_MAX_C}")
+    # (a patch merge's own LayerNorm runs on the patch-merge kernels, checked above)
+    common.check_layernorm_widths(((name, m.normalized_shape[-1]) for name, m in model.named_modules()
+                                   if isinstance(m, nn.LayerNorm) and not name.endswith("downsample.norm")), want_tape)
 
 
 def forward(model, x, train, want_tape):
-    _check(model)
+    _check(model, want_tape)
     x = common.image_input(model, x)
     B, Cin, Hi, Wi = x.shape
     pe = model.patch_embed

@@ -53,7 +53,7 @@ class _PackSpec:
 _pack_spec = _PackSpec()
 
 
-def _check(model):
+def _check(model, want_tape=False):
     if model.dist_token is not None:
         raise NotImplementedError("distilled ViT (dist_token) is not implemented on this engine")
     if model.has_logits and not (isinstance(getattr(model.pre_logits, "fc", None), nn.Linear)
@@ -69,10 +69,12 @@ def _check(model):
             raise NotImplementedError("the attention kernel is built for head_dim 64")
         if not isinstance(blk.mlp.act, nn.GELU):
             raise NotImplementedError("Mlp activation must be nn.GELU (exact erf)")
+    common.check_layernorm_widths(((name, m.normalized_shape[-1]) for name, m in model.named_modules()
+                                   if isinstance(m, nn.LayerNorm)), want_tape)
 
 
 def forward(model, x, train, want_tape):
-    _check(model)
+    _check(model, want_tape)
     x = common.image_input(model, x)
     B, Cin, Hh, Ww = x.shape
     pe = model.patch_embed

@@ -1403,6 +1403,13 @@ def tanh_bwd(dt16, t):
 
 
 # --------------------------------------------------------------------------------------------------------- layer norm
+# Widest rows the kernels take (b200_layernorm_fwd / _bwd, b200_patch_merge_ln_fwd / _bwd): the schedules reject a model
+# with a wider LayerNorm before launching anything.
+LAYERNORM_FWD_MAX_C = 3072
+LAYERNORM_BWD_MAX_C = 1024
+PATCH_MERGE_LN_MAX_C = 2048   # the merged width 4C
+
+
 def layernorm_fwd(x, gamma, beta, eps, out_dtype=BF16):
     """x [..., C] fp32 or bf16 -> (y bf16 (or fp32), mean, rstd)."""
     lib = _lib.load()

@@ -91,11 +91,11 @@ def test_layerscale_block_tail():
     _close(dgam, gg, 5e-3, 5e-3 * float(gg.abs().max()), "dgamma")
 
 
-def _build(depths=(3, 3, 9, 3), std=None, gamma_init=None, seed=0):
+def _build(depths=(3, 3, 9, 3), std=None, gamma_init=None, seed=0, dims=(96, 192, 384, 768)):
     from deeplearning_b200.classification.convNext.models.networks import ConvNeXt
 
     torch.manual_seed(seed)
-    m = ConvNeXt(depths=list(depths), dims=[96, 192, 384, 768], num_classes=1000, drop_path_rate=0.0)
+    m = ConvNeXt(depths=list(depths), dims=list(dims), num_classes=1000, drop_path_rate=0.0)
     state = {k: v.clone() for k, v in m.state_dict().items()}
     if std is not None:  # SURVEY D5: the reference init (std 0.2) gives |logit| ~ 20; also test a std 0.02 re-init
         g = torch.Generator().manual_seed(7)
@@ -126,9 +126,19 @@ def test_convnext_tiny_eval_parity(std, gamma):
 
 @pytest.mark.parametrize("depths,std,gamma", [((1, 1, 1, 1), 0.02, 0.5), ((3, 3, 9, 3), None, None), ((3, 3, 9, 3), 0.02, 0.5)])
 def test_convnext_train_step_parity(depths, std, gamma):
+    _train_step_parity(depths, std, gamma)
+
+
+def test_convnext_base_widths_train_step_parity():
+    """ConvNeXt-B widths (128 .. 1024: depthwise 7x7 and LayerNorm at 1024 channels), one block per stage - the kernel
+    shapes depend only on the widths."""
+    _train_step_parity((1, 1, 1, 1), 0.02, 0.5, dims=(128, 256, 512, 1024))
+
+
+def _train_step_parity(depths, std, gamma, dims=(96, 192, 384, 768)):
     from oracle.convnext import train_step_grads
 
-    m, state = _build(depths=depths, std=std, gamma_init=gamma)
+    m, state = _build(depths=depths, std=std, gamma_init=gamma, dims=dims)
     m.train()
     B = 8
     x = torch.randn(B, 3, 224, 224, generator=torch.Generator().manual_seed(1))
@@ -139,7 +149,7 @@ def test_convnext_train_step_parity(depths, std, gamma):
     loss.backward()
     err = float((out.detach().float().cpu() - ref_logits).abs().max())
     scale = float(ref_logits.abs().max())
-    print(f"depths {depths} std {std}: train logits err {err:.4g} (|ref| max {scale:.3g}); loss {float(loss.detach()):.4f} vs {float(ref_loss):.4f}")
+    print(f"depths {depths} dims {dims} std {std}: train logits err {err:.4g} (|ref| max {scale:.3g}); loss {float(loss.detach()):.4f} vs {float(ref_loss):.4f}")
     assert err <= 1e-2 * max(1.0, scale)
     assert abs(float(loss.detach()) - float(ref_loss)) <= 1e-2 * max(1.0, abs(float(ref_loss)))
     worst = (0.0, "")

@@ -7,11 +7,12 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 
-def _build(depths=(2, 2, 6, 2), num_classes=1000, seed=0):
+def _build(depths=(2, 2, 6, 2), num_classes=1000, seed=0, embed_dim=96, num_heads=(3, 6, 12, 24)):
     from deeplearning_b200.classification.swin_transformer.models.swin_transformer import SwinTransformer
 
     torch.manual_seed(seed)
-    m = SwinTransformer(depths=list(depths), num_heads=[3, 6, 12, 24][:len(depths)], num_classes=num_classes, drop_path_rate=0.0)
+    m = SwinTransformer(embed_dim=embed_dim, depths=list(depths), num_heads=list(num_heads)[:len(depths)],
+                        num_classes=num_classes, drop_path_rate=0.0)
     state = {k: v.clone() for k, v in m.state_dict().items()}
     return m.cuda(), state
 
@@ -53,21 +54,31 @@ def test_swin_tiny_eval_logits_parity(randomize):
 
 @pytest.mark.parametrize("depths,randomize", [((2, 2), True), ((2, 2, 6, 2), False), ((2, 2, 6, 2), True)])
 def test_swin_train_step_parity(depths, randomize):
+    _train_step_parity(depths, randomize)
+
+
+def test_swin_base_widths_train_step_parity():
+    """Swin-B widths (embed 128, heads 4/8/16/32: LayerNorm up to 1024, patch merges up to 4C = 2048), one block per
+    stage - the kernel shapes depend only on the widths."""
+    _train_step_parity((1, 1, 1, 1), True, embed_dim=128, num_heads=(4, 8, 16, 32))
+
+
+def _train_step_parity(depths, randomize, embed_dim=96, num_heads=(3, 6, 12, 24)):
     from oracle.swin import train_step_grads
 
-    m, state = _build(depths=depths)
+    m, state = _build(depths=depths, embed_dim=embed_dim, num_heads=num_heads)
     if randomize:
         _randomize(m, state)
     m.train()
     B = 4
     x = torch.randn(B, 3, 224, 224, generator=torch.Generator().manual_seed(1))
     y = torch.randint(0, 1000, (B,), generator=torch.Generator().manual_seed(2))
-    ref_logits, ref_loss, ref_grads = train_step_grads(state, x, y, depths=depths, num_heads=(3, 6, 12, 24)[:len(depths)])
+    ref_logits, ref_loss, ref_grads = train_step_grads(state, x, y, depths=depths, num_heads=tuple(num_heads)[:len(depths)])
     out = m(x.cuda())
     loss = F.cross_entropy(out, y.cuda())
     loss.backward()
     err = float((out.detach().float().cpu() - ref_logits).abs().max())
-    print(f"depths {depths} rand={randomize}: train logits err {err:.4g} (|ref| max {float(ref_logits.abs().max()):.3g}); "
+    print(f"depths {depths} embed {embed_dim} rand={randomize}: train logits err {err:.4g} (|ref| max {float(ref_logits.abs().max()):.3g}); "
           f"loss {float(loss.detach()):.5f} vs {float(ref_loss):.5f}")
     assert err <= 1e-2 * max(1.0, float(ref_logits.abs().max()))
     assert abs(float(loss.detach()) - float(ref_loss)) < 1e-2

@@ -6,11 +6,12 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 
-def _build(depth=12, num_classes=1000, seed=0):
+def _build(depth=12, num_classes=1000, seed=0, patch=16, embed_dim=768, num_heads=12):
     from deeplearning_b200.classification.vision_transformer.vit_model import VisionTransformer
 
     torch.manual_seed(seed)
-    m = VisionTransformer(img_size=224, patch_size=16, embed_dim=768, depth=depth, num_heads=12, num_classes=num_classes)
+    m = VisionTransformer(img_size=224, patch_size=patch, embed_dim=embed_dim, depth=depth, num_heads=num_heads,
+                          num_classes=num_classes)
     state = {k: v.clone() for k, v in m.state_dict().items()}
     return m.cuda(), state
 
@@ -48,21 +49,33 @@ def test_vit_b16_eval_logits_parity(randomize):
 
 @pytest.mark.parametrize("depth,randomize", [(2, True), (12, False), (12, True)])
 def test_vit_train_step_parity(depth, randomize):
+    _train_step_parity(depth, randomize)
+
+
+# ViT-L/16 (1024 wide, 16 heads: the 768 < C <= 1024 LayerNorm backward) and ViT-B/32 (50 tokens); the kernel shapes
+# depend only on the widths, so two blocks are enough
+@pytest.mark.parametrize("patch,embed_dim,num_heads", [(16, 1024, 16), (32, 768, 12)])
+def test_vit_wide_and_patch32_train_step_parity(patch, embed_dim, num_heads):
+    _train_step_parity(2, True, patch=patch, embed_dim=embed_dim, num_heads=num_heads)
+
+
+def _train_step_parity(depth, randomize, **arch):
     from oracle.vit import train_step_grads
 
-    m, state = _build(depth=depth)
+    m, state = _build(depth=depth, **arch)
     if randomize:
         _randomize(m, state)
     m.train()
     B = 8
     x = torch.randn(B, 3, 224, 224, generator=torch.Generator().manual_seed(1))
     y = torch.randint(0, 1000, (B,), generator=torch.Generator().manual_seed(2))
-    ref_logits, ref_loss, ref_grads = train_step_grads(state, x, y)
+    kw = {k: arch[k] for k in ("patch", "num_heads") if k in arch}
+    ref_logits, ref_loss, ref_grads = train_step_grads(state, x, y, **kw)
     out = m(x.cuda())
     loss = F.cross_entropy(out, y.cuda())
     loss.backward()
     err = float((out.detach().float().cpu() - ref_logits).abs().max())
-    print(f"depth {depth} rand={randomize}: train logits err {err:.4g} (|ref| max {float(ref_logits.abs().max()):.3g}); loss {float(loss.detach()):.5f} vs {float(ref_loss):.5f}")
+    print(f"depth {depth} {arch} rand={randomize}: train logits err {err:.4g} (|ref| max {float(ref_logits.abs().max()):.3g}); loss {float(loss.detach()):.5f} vs {float(ref_loss):.5f}")
     assert err <= 1e-2 * max(1.0, float(ref_logits.abs().max()))
     assert abs(float(loss.detach()) - float(ref_loss)) < 1e-2
     worst = (0.0, "")
