@@ -156,6 +156,14 @@ SIGNATURES = {
     "b200_tail_apply": (_I, [_P] * 6 + [_I] * 3 + [_P]),
     "b200_tail_bwd_reduce": (_I, [_P] * 5 + [_I] * 3 + [_P]),
     "b200_bn_bwd_apply_dz": (_I, [_P] * 5 + [_L, _I, _P]),
+    "b200_vgg_pool_partial_rows": (_I, [_I, _I, _I, _I]),
+    "b200_vgg_pool_fwd": (_I, [_P] * 5 + [_I] * 4 + [_P]),
+    "b200_vgg_pool_bwd": (_I, [_P] * 8 + [_I] * 4 + [_P]),
+    "b200_vgg_avgpool7_fwd": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "b200_vgg_avgpool7_bwd": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "b200_vgg_dropout_fwd": (_I, [_P, _P, _P, _L, _P]),
+    "b200_vgg_dropout_bwd": (_I, [_P, _P, _F, _P, _L, _P]),
+    "b200_adam": (_I, [_P, _P, _P, _P, _L, _P, _F, _F, _F, _F, _F, _P, _P]),
 }
 
 

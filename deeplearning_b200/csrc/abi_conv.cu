@@ -274,7 +274,9 @@ int epilogue_flags(const ConvGemmParams& p) {
   X(kEpiAffine)                                           /* eval mode: bn(conv) (downsample branch)     */ \
   X(kEpiMask | kEpiResBf16 | kEpiStats)                   /* dgrad + identity gradient, ReLU mask, sum dz */ \
   X(kEpiBnMask)                                           /* 3x3 dgrad + reduce half of the producer's BN backward */ \
-  X(kEpiBnMask | kEpiBias)                                /* the same behind the BN-algebra dual GEMM (bias = k W) */
+  X(kEpiBnMask | kEpiBias)                                /* the same behind the BN-algebra dual GEMM (bias = k W) */ \
+  X(kEpiBias | (1 << kEpiActShift))                       /* VGG conv / classifier Linear + bias + ReLU  */ \
+  X(kEpiBias | kEpiStats)                                 /* VGG _bn conv: + bias, BN statistics     */
 
 // ---- 64 -> 64 channel convolutions with the weights resident in shared memory (conv_tap64.cuh): ResNet layer1's 3x3
 // forward / dgrad and the space-to-depth stem.

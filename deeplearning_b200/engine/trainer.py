@@ -59,6 +59,12 @@ def _engine_for(model):
         from . import efficientnet
 
         return efficientnet
+    from ..classification.vggNet.models.network import VGG
+
+    if isinstance(model, VGG):
+        from . import vgg
+
+        return vgg
     raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 
@@ -215,6 +221,8 @@ class TrainStep:
         """optimizer="sgd": torch.optim.SGD(momentum, weight_decay on every parameter) - resnet/vit train.py:96,94.
         optimizer="adamw": torch.optim.AdamW(betas, eps, weight_decay) with the reference's decay / no-decay groups
         (``no_decay(name, param) -> bool``, default ``no_decay_rule``) - convNext/train.py:96,102.
+        optimizer="adam": torch.optim.Adam(lr, betas, eps, weight_decay) in one group, every parameter decayed by an L2 term
+        added to the gradient (not AdamW's decoupled decay) - vggNet/train.py:133-136.
         clip_grad: max global L2 norm of the (all-reduced, averaged) gradient, ``clip_grad_norm_`` of the Swin recipe
         (swin_transformer/main.py:197, config TRAIN.CLIP_GRAD = 5.0); the norm of the last step is ``self.grad_norm``.
         label_smoothing: LabelSmoothingCrossEntropy of the Swin recipe (main.py:114-115); floating-point ``labels`` of
@@ -226,7 +234,7 @@ class TrainStep:
         self.engine = _engine_for(model)
         self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
         self.optimizer, self.betas, self.eps = optimizer, betas, eps
-        if optimizer not in ("sgd", "adamw"):
+        if optimizer not in ("sgd", "adamw", "adam"):
             raise ValueError(f"unknown optimizer {optimizer!r}")
         bucket_mb = float(os.environ.get("B200_BUCKET_MB", bucket_mb))   # tuning knob (see DESIGN.md section 5)
         self.arena = FlatArena(model.parameters(), process_group, world_size, bucket_mb=bucket_mb)
@@ -251,11 +259,13 @@ class TrainStep:
             arena = self.arena
             rule = no_decay or model_no_decay_rule(model)
             names = {p.data_ptr(): n for n, p in model.named_parameters()}
-            arena.flat_v = torch.zeros_like(arena.flat_p)
             arena.flat_wd = torch.zeros_like(arena.flat_p)
             for p, o in zip(arena.params, arena.offsets):
                 if not rule(names.get(p.data_ptr(), ""), p):
                     arena.flat_wd[o:o + p.numel()] = weight_decay
+        if optimizer in ("adamw", "adam"):
+            arena = self.arena
+            arena.flat_v = torch.zeros_like(arena.flat_p)
             self._hyper = torch.tensor([lr, 0.0, 0.0, 1.0, 1.0], dtype=torch.float32, device=arena.flat_p.device)
         if broadcast:
             self.arena.broadcast(model.buffers())
@@ -302,6 +312,14 @@ class TrainStep:
                 self._hyper_lr_value = float(lr)
             ops.adamw_(arena.flat_p, arena.flat_g, arena.flat_m, arena.flat_v, arena.flat_wd, self._hyper, self.betas[0],
                        self.betas[1], self.eps, gscale=arena.grad_scale, clip=self._clip)
+            weight_cache.bump()
+            return
+        if self.optimizer == "adam":
+            if lr != self._hyper_lr():
+                self._hyper[0:1].fill_(float(lr))
+                self._hyper_lr_value = float(lr)
+            ops.adam_(arena.flat_p, arena.flat_g, arena.flat_m, arena.flat_v, self._hyper, self.betas[0], self.betas[1],
+                      self.eps, self.weight_decay, gscale=arena.grad_scale, clip=self._clip)
             weight_cache.bump()
             return
         # momentum buffer starts at zero, so "buf = mu*buf + g" already equals torch's first-step "buf = g"
@@ -396,7 +414,7 @@ class TrainStep:
         if lr is not None and lr != self.lr:
             self.lr = lr
             self._lr_dev.fill_(float(lr))
-            if self.optimizer == "adamw":
+            if self.optimizer in ("adamw", "adam"):
                 self._hyper[0:1].fill_(float(lr))
                 self._hyper_lr_value = float(lr)
         if self._micro + 1 < self.accum_steps:
@@ -430,10 +448,14 @@ class TrainStep:
                 if self.steps > 0:
                     state[i] = {"step": torch.tensor(float(self.steps)), "exp_avg": arena.flat_m[o:o + n].view_as(prm).clone(),
                                 "exp_avg_sq": arena.flat_v[o:o + n].view_as(prm).clone()}
-                (decay if float(arena.flat_wd[o]) != 0.0 else nodecay).append(i)
+                if self.optimizer == "adamw":
+                    (decay if float(arena.flat_wd[o]) != 0.0 else nodecay).append(i)
         if self.optimizer == "sgd":
             groups = [{"lr": self.lr, "momentum": self.momentum, "dampening": 0, "weight_decay": self.weight_decay,
                        "nesterov": False, "params": list(range(len(arena.params)))}]
+        elif self.optimizer == "adam":
+            groups = [{"lr": self._hyper_lr(), "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay,
+                       "amsgrad": False, "params": list(range(len(arena.params)))}]
         else:
             base = {"lr": self._hyper_lr(), "betas": tuple(self.betas), "eps": self.eps, "amsgrad": False}
             groups = [dict(base, weight_decay=self.weight_decay, params=decay), dict(base, weight_decay=0.0, params=nodecay)]
@@ -461,7 +483,7 @@ class TrainStep:
                     steps = max(steps, int(float(st["step"])))
         lr = sd["param_groups"][0]["lr"]
         self.lr = float(lr)
-        if self.optimizer == "adamw":
+        if self.optimizer in ("adamw", "adam"):
             b1, b2 = self.betas
             self._hyper.copy_(torch.tensor([self.lr, 1.0 - b1 ** steps, 1.0 - b2 ** steps, b1 ** steps, b2 ** steps],
                                            dtype=torch.float32))

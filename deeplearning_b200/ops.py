@@ -1765,3 +1765,101 @@ def patch_merge_ln_bwd(dy, x, mean, rstd, gamma, dgamma=None, dbeta=None):
                                   sc.numel(), _stream())
     _lib.check(rc, "b200_bn_bwd_finalize")
     return dx, dgamma, dbeta
+
+
+# ------------------------------------------------------------------------------------------------- VGG passes (csrc/vgg.cuh)
+def vgg_pool_fwd(x, co=None, want_idx=True):
+    """MaxPool2d(2, 2) of x (plain: x = relu(conv + b)) or of relu(x * scale + shift) (co = BnCoeffs: x the raw conv output).
+    Returns (y [B, H/2, W/2, C], idx uint8 of y's shape or None): idx holds the window tap of each maximum."""
+    lib = _lib.load()
+    _chk_act(x, "x")
+    B, H, W, C = x.shape
+    y = torch.empty(B, H // 2, W // 2, C, dtype=BF16, device=x.device)
+    idx = torch.empty(y.shape, dtype=torch.uint8, device=x.device) if want_idx else None
+    sp = _span("vgg_pool_fwd", 0.0, _nb(x, y, idx))
+    rc = lib.b200_vgg_pool_fwd(_p(x), _p(co.scale) if co else None, _p(co.shift) if co else None, _p(y), _p(idx), B, H, W, C,
+                               _stream())
+    _lib.check(rc, "b200_vgg_pool_fwd")
+    if sp:
+        sp.end()
+    return y, idx
+
+
+def vgg_pool_bwd(g, idx, in_hw, y=None, c=None, co=None):
+    """Gradient [B, H, W, C] of vgg_pool_fwd's input from the pooled gradient g: plain (y = the pooled output) returns dx;
+    BN (c = the raw conv output, co its BnCoeffs) returns (dz, partial [T, 2, C] = {sum dz, sum dz c})."""
+    lib = _lib.load()
+    _chk_act(g, "g")
+    B, _, _, C = g.shape
+    H, W = in_hw
+    dx = torch.empty(B, H, W, C, dtype=BF16, device=g.device)
+    partial = None
+    if c is not None:
+        T = lib.b200_vgg_pool_partial_rows(B, H, W, C)
+        _lib.check(min(T, 0), "b200_vgg_pool_partial_rows")
+        partial = torch.empty(T, 2, C, dtype=F32, device=g.device)
+    sp = _span("vgg_pool_bwd", 0.0, _nb(g, idx, y, c, dx))
+    rc = lib.b200_vgg_pool_bwd(_p(g), _p(idx), _p(y), _p(c), _p(co.scale) if co else None, _p(co.shift) if co else None,
+                               _p(dx), _p(partial), B, H, W, C, _stream())
+    _lib.check(rc, "b200_vgg_pool_bwd")
+    if sp:
+        sp.end()
+    return dx if c is None else (dx, partial)
+
+
+def vgg_avgpool7_fwd(x):
+    """AdaptiveAvgPool2d((7, 7)) + torch.flatten of NHWC x: bf16 [B, C * 49] in NCHW flatten order (k = c * 49 + i * 7 + j)."""
+    lib = _lib.load()
+    _chk_act(x, "x")
+    B, H, W, C = x.shape
+    y = torch.empty(B, C * 49, dtype=BF16, device=x.device)
+    sp = _span("vgg_avgpool7_fwd", 0.0, _nb(x, y))
+    _lib.check(lib.b200_vgg_avgpool7_fwd(_p(x), _p(y), B, H, W, C, _stream()), "b200_vgg_avgpool7_fwd")
+    if sp:
+        sp.end()
+    return y
+
+
+def vgg_avgpool7_bwd(gy, in_shape):
+    """Gradient [B, H, W, C] of vgg_avgpool7_fwd's input from gy [B, C * 49]."""
+    lib = _lib.load()
+    _chk_act(gy, "gy")
+    B, H, W, C = in_shape
+    gx = torch.empty(B, H, W, C, dtype=BF16, device=gy.device)
+    sp = _span("vgg_avgpool7_bwd", 0.0, _nb(gy, gx))
+    _lib.check(lib.b200_vgg_avgpool7_bwd(_p(gy), _p(gx), B, H, W, C, _stream()), "b200_vgg_avgpool7_bwd")
+    if sp:
+        sp.end()
+    return gx
+
+
+def vgg_dropout_fwd(x, mask):
+    """x * mask (bf16 x, fp32 mask of x's shape: 0 or 1 / (1 - p))."""
+    lib = _lib.load()
+    _chk_act(x, "x")
+    mask = mask.contiguous()
+    assert mask.dtype == F32 and mask.shape == x.shape
+    y = torch.empty_like(x)
+    _lib.check(lib.b200_vgg_dropout_fwd(_p(x), _p(mask), _p(y), x.numel(), _stream()), "b200_vgg_dropout_fwd")
+    return y
+
+
+def vgg_dropout_bwd(g, h, p):
+    """Gradient of pre in h = dropout_p(relu(pre)) from dL/dh and the stored h: h > 0 ? g / (1 - p) : 0."""
+    lib = _lib.load()
+    _chk_act(g, "g")
+    _chk_act(h, "h")
+    dx = torch.empty_like(g)
+    _lib.check(lib.b200_vgg_dropout_bwd(_p(g), _p(h), 1.0 / (1.0 - p), _p(dx), g.numel(), _stream()), "b200_vgg_dropout_bwd")
+    return dx
+
+
+def adam_(p, g, m, v, hyper, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0, gscale=1.0, tick=True, clip=None):
+    """torch.optim.Adam step (L2 decay added to the gradient) over flat fp32 tensors; hyper as adamw_'s, tick advances t first.
+    clip: optional output of grad_clip_coef (the gradient is additionally scaled by clip[0])."""
+    lib = _lib.load()
+    if tick:
+        _lib.check(lib.b200_adamw_tick(_p(hyper), beta1, beta2, _stream()), "b200_adamw_tick")
+    rc = lib.b200_adam(_p(p), _p(g), _p(m), _p(v), p.numel(), _p(hyper), beta1, beta2, eps, weight_decay, gscale, _p(clip),
+                       _stream())
+    _lib.check(rc, "b200_adam")

@@ -513,6 +513,39 @@ int b200_tail_bwd_reduce(const void* g, const float* rs, const void* c, void* dz
 int b200_bn_bwd_apply_dz(const void* dz, const void* c, const float* co, const float* m, void* dc, long long rows, int C,
                          void* stream);
 
+/* ---- VGG (classification/vggNet/models/network.py) passes the convolution GEMMs do not cover, and torch.optim.Adam.
+ * Activations are NHWC bf16 [B][H][W][C], 16-byte aligned; scale / shift fp32 [C] are a BatchNorm's coefficients (batch
+ * statistics in train mode, running statistics in eval mode).  Scope: 1 <= B <= 65535, C a multiple of 8 in [8, 8192]
+ * (the adaptive pool: a multiple of 64), H, W >= 1 (the 2x2 pool: >= 2); anything else returns B200_EINVAL with a message
+ * and launches nothing.  All sums are fp32 in a fixed order (no atomics).
+ * pool_fwd:  MaxPool2d(2, 2) (floor mode) of x (plain: x = relu(conv + b), written by the GEMM) or of relu(x * scale + shift)
+ *            (BN: x = the raw conv output; the full-resolution activation is never stored): y [B][H/2][W/2][C]; idx
+ *            (optional, 8-byte aligned) one byte per element of y = the window tap 0..3 (row-major) of the maximum, ties
+ *            resolved to the first
+ * pool_bwd:  dx [B][H][W][C] = the pooled gradient g at the arg-max pixel of each window where the activation was positive,
+ *            0 elsewhere (also in the row / column of an odd H / W that no window covers).  Plain: y = the pooled output
+ *            (the mask is y > 0), c / scale / shift / partial NULL.  BN: y NULL, the mask is c * scale + shift > 0 and
+ *            partial fp32 [pool_partial_rows][2][C] = {sum dx, sum dx c}, the rows b200_bn_bwd_finalize reads
+ * avgpool7:  AdaptiveAvgPool2d((7, 7)) + torch.flatten: y bf16 [B][C * 49] with k = c * 49 + i * 7 + j, bin i spanning
+ *            rows floor(i H / 7) .. ceil((i + 1) H / 7) - 1 (likewise columns); _bwd scatters gy [B][C * 49] back to
+ *            gx [B][H][W][C]
+ * dropout_fwd: y = x * mask over n elements (mask fp32, 0 or 1 / (1 - p)); n a multiple of 8
+ * dropout_bwd: the backward of h = dropout(relu(pre)) from the stored h: dx = h > 0 ? g * scale : 0, scale = 1 / (1 - p)
+ * adam:      torch.optim.Adam (L2 weight decay added to the gradient, every element decays by weight_decay) over flat
+ *            fp32 arenas: g' = g gscale [clip_coef[0]] + weight_decay p, then b200_adamw's moments and bias-corrected step;
+ *            hyper as b200_adamw's, advanced by b200_adamw_tick */
+int b200_vgg_pool_partial_rows(int B, int H, int W, int C);
+int b200_vgg_pool_fwd(const void* x, const float* scale, const float* shift, void* y, void* idx, int B, int H, int W, int C,
+                      void* stream);
+int b200_vgg_pool_bwd(const void* g, const void* idx, const void* y, const void* c, const float* scale, const float* shift,
+                      void* dx, float* partial, int B, int H, int W, int C, void* stream);
+int b200_vgg_avgpool7_fwd(const void* x, void* y, int B, int H, int W, int C, void* stream);
+int b200_vgg_avgpool7_bwd(const void* gy, void* gx, int B, int H, int W, int C, void* stream);
+int b200_vgg_dropout_fwd(const void* x, const float* mask, void* y, long long n, void* stream);
+int b200_vgg_dropout_bwd(const void* g, const void* h, float scale, void* dx, long long n, void* stream);
+int b200_adam(float* p, const float* g, float* m, float* v, long long n, const float* hyper, float beta1, float beta2,
+              float eps, float weight_decay, float gscale, const float* clip_coef, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,6 +1,6 @@
 """One small launch of every wgmma / TMA kernel family, for `compute-sanitizer --tool {memcheck,racecheck,synccheck}`:
 implicit-GEMM conv (forward + statistics, dgrad + residual, affine / mask epilogues, dual-source K), the streaming 1x1 kernel
-(both modes), wgrad, ViT attention forward / backward, window attention forward / backward, BN-algebra kernels.
+(both modes), wgrad, ViT attention forward / backward, window attention forward / backward, BN-algebra kernels, the VGG passes.
 usage: compute-sanitizer --tool racecheck python tools/sanitize_ops.py [family ...]"""
 import os
 import sys
@@ -12,7 +12,7 @@ from deeplearning_b200 import ops
 
 dev = torch.device("cuda")
 BF = torch.bfloat16
-fam = set(sys.argv[1:]) or {"conv", "stream", "wgrad", "attn", "attn2", "ln", "wattn", "algebra"}
+fam = set(sys.argv[1:]) or {"conv", "stream", "wgrad", "attn", "attn2", "ln", "wattn", "algebra", "vgg"}
 
 
 def r(*shape, scale=1.0):
@@ -92,5 +92,21 @@ if "ln" in fam:
         y, mean, rstd = ops.layernorm_fwd(x, g, torch.zeros(C, device=dev), 1e-6)
         dx, dg, db = ops.layernorm_bwd(r(rows, C, scale=0.1), x, mean, rstd, g, add=r(rows, C, scale=0.1) if dt != BF else None)
         print("ln ok", rows, C, float(dx.float().abs().mean()), float(dg.abs().mean()))
+if "vgg" in fam:
+    # VGG passes (vgg.cuh): 2x2 pool forward / backward, plain and BatchNorm (odd H / W), adaptive 7x7 pool, dropout, Adam
+    c = r(2, 9, 7, 128)
+    co = ops.BnCoeffs(128, dev)
+    co.scale.fill_(1.0), co.shift.fill_(0.1), co.mean.zero_(), co.invstd.fill_(1.0)
+    for cc in (None, co):
+        y, idx = ops.vgg_pool_fwd(c if cc is not None else torch.relu(c), cc)
+        g = r(*y.shape)
+        d = ops.vgg_pool_bwd(g, idx, (9, 7), y=y) if cc is None else ops.vgg_pool_bwd(g, idx, (9, 7), c=c, co=cc)[0]
+    f = ops.vgg_avgpool7_fwd(r(2, 5, 9, 128))
+    gx = ops.vgg_avgpool7_bwd(f, (2, 5, 9, 128))
+    h = ops.vgg_dropout_fwd(r(4, 64), torch.full((4, 64), 2.0, device=dev))
+    dh = ops.vgg_dropout_bwd(r(4, 64), h, 0.5)
+    p, gg = torch.randn(1001, device=dev), torch.randn(1001, device=dev)
+    ops.adam_(p, gg, torch.zeros_like(p), torch.zeros_like(p), torch.tensor([1e-3, 0, 0, 1, 1.0], device=dev), weight_decay=1e-3)
+    print("vgg ok", float(d.float().abs().mean()), float(gx.float().abs().mean()), float(dh.float().abs().mean()))
 torch.cuda.synchronize()
 print("done")
