@@ -156,6 +156,11 @@ SIGNATURES = {
     "b200_tail_apply": (_I, [_P] * 6 + [_I] * 3 + [_P]),
     "b200_tail_bwd_reduce": (_I, [_P] * 5 + [_I] * 3 + [_P]),
     "b200_bn_bwd_apply_dz": (_I, [_P] * 5 + [_L, _I, _P]),
+    "b200_dw_relu_fwd": (_I, [_P] * 6 + [_I] * 5 + [_P]),
+    "b200_dw_relu_dgrad": (_I, [_P] * 7 + [_I] * 5 + [_P]),
+    "b200_dw_relu_wgrad": (_I, [_P] * 6 + [c_size_t] + [_I] * 5 + [_P]),
+    "b200_shuffle_tail_s2_fwd": (_I, [_P] * 5 + [_I] * 5 + [_P]),
+    "b200_shuffle_relu_bwd": (_I, [_P] * 8 + [_I] * 7 + [_P]),
     "b200_vgg_pool_partial_rows": (_I, [_I, _I, _I, _I]),
     "b200_vgg_pool_fwd": (_I, [_P] * 5 + [_I] * 4 + [_P]),
     "b200_vgg_pool_bwd": (_I, [_P] * 8 + [_I] * 4 + [_P]),

@@ -43,6 +43,13 @@ cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
     else { CALL(5, 2); }                              \
   } while (0)
 
+// CALL(S) with the compile-time stride of the runtime stride (3x3 kernels)
+#define DW_STRIDE_DISPATCH(stride, CALL) \
+  do {                                   \
+    if ((stride) == 1) { CALL(1); }      \
+    else { CALL(2); }                    \
+  } while (0)
+
 extern "C" {
 
 int b200_dw_partial_rows(long long rows, int C) {
@@ -152,6 +159,77 @@ int b200_dw_wgrad(const void* dd, const void* x, const float* scale, const float
   const long long n = static_cast<long long>(k) * k * C;
   B200_CHECK_CUDA(launch_pdl(dw_wgrad_reduce_kernel, dim3(static_cast<unsigned>((n + 31) / 32)), dim3(256), 0,
                              as_stream(stream), static_cast<const float*>(pws), dw, gm.blocks, k * k, C));
+  B200_LAUNCHED();
+  return OK;
+}
+
+// ShuffleNet's depthwise convolution: the kDwRelu mode of the same kernels, k = 3
+int b200_dw_relu_fwd(const void* x, const float* w, const float* scale, const float* shift, void* d, float* stats, int B,
+                     int H, int W, int C, int stride, void* stream) {
+  MB_REQUIRE_SHAPE("dw_relu_fwd", dw_bad_shape(B, H, W, C, 3, stride));
+  B200_REQUIRE(aligned16(x) && w != nullptr && aligned16(d) && aligned16(scale) && aligned16(shift),
+               "dw_relu_fwd: x, d, scale, shift must be non-null and 16-byte aligned, w non-null");
+  const int Ho = out_size(H, stride), Wo = out_size(W, stride);
+  const DwGeom gm = dw_geom(static_cast<long long>(B) * Ho * Wo, C);
+  const dim3 grid(gm.blocks, gm.nchunk);
+  const auto* px = static_cast<const __nv_bfloat16*>(x);
+  auto* pd = static_cast<__nv_bfloat16*>(d);
+#define DWR_FWD(S)                                                                                                        \
+  if (stats != nullptr)                                                                                                   \
+    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<3, S, kDwRelu, true>, grid, dim3(256), 0, as_stream(stream), px, w, scale,  \
+                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block));                                 \
+  else                                                                                                                    \
+    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<3, S, kDwRelu, false>, grid, dim3(256), 0, as_stream(stream), px, w, scale, \
+                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block))
+  DW_STRIDE_DISPATCH(stride, DWR_FWD);
+#undef DWR_FWD
+  B200_LAUNCHED();
+  return OK;
+}
+
+int b200_dw_relu_dgrad(const void* dd, const float* w, const void* x, const float* scale, const float* shift, void* dx,
+                       float* partial, int B, int H, int W, int C, int stride, void* stream) {
+  MB_REQUIRE_SHAPE("dw_relu_dgrad", dw_bad_shape(B, H, W, C, 3, stride));
+  B200_REQUIRE(aligned16(dd) && w != nullptr && aligned16(x) && aligned16(scale) && aligned16(shift) && aligned16(dx) &&
+                   partial != nullptr,
+               "dw_relu_dgrad: dd, x, scale, shift, dx must be non-null and 16-byte aligned, w and partial non-null");
+  const int Ho = out_size(H, stride), Wo = out_size(W, stride);
+  const DwGeom gm = dw_geom(static_cast<long long>(B) * H * W, C);
+  const dim3 grid(gm.blocks, gm.nchunk);
+  const auto* pdd = static_cast<const __nv_bfloat16*>(dd);
+  const auto* px = static_cast<const __nv_bfloat16*>(x);
+  const __nv_bfloat16* none = nullptr;
+  auto* pdx = static_cast<__nv_bfloat16*>(dx);
+#define DWR_DGRAD(S)                                                                                                      \
+  B200_CHECK_CUDA(launch_pdl(dw_dgrad_kernel<3, S, kDwRelu, false>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,   \
+                             scale, shift, none, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block))
+  DW_STRIDE_DISPATCH(stride, DWR_DGRAD);
+#undef DWR_DGRAD
+  B200_LAUNCHED();
+  return OK;
+}
+
+int b200_dw_relu_wgrad(const void* dd, const void* x, const float* scale, const float* shift, float* dw, void* ws,
+                       size_t ws_bytes, int B, int H, int W, int C, int stride, void* stream) {
+  MB_REQUIRE_SHAPE("dw_relu_wgrad", dw_bad_shape(B, H, W, C, 3, stride));
+  B200_REQUIRE(aligned16(dd) && aligned16(x) && aligned16(scale) && aligned16(shift) && dw != nullptr && ws != nullptr,
+               "dw_relu_wgrad: dd, x, scale, shift must be non-null and 16-byte aligned, dw and ws non-null");
+  const size_t need = b200_dw_wgrad_workspace_bytes(B, H, W, C, 3, stride);
+  B200_REQUIRE(ws_bytes >= need, "dw_relu_wgrad: workspace of %zu bytes, need %zu", ws_bytes, need);
+  const int Ho = out_size(H, stride), Wo = out_size(W, stride);
+  const DwGeom gm = dw_geom(static_cast<long long>(B) * Ho * Wo, C);
+  const dim3 grid(gm.blocks, gm.nchunk, 3);
+  const auto* pdd = static_cast<const __nv_bfloat16*>(dd);
+  const auto* px = static_cast<const __nv_bfloat16*>(x);
+  float* pws = static_cast<float*>(ws);
+#define DWR_WGRAD(S)                                                                                                      \
+  B200_CHECK_CUDA(launch_pdl(dw_wgrad_kernel<3, S, kDwRelu>, grid, dim3(256), 0, as_stream(stream), pdd, px, scale, shift,\
+                             pws, B, H, W, Ho, Wo, C, gm.rows_per_block))
+  DW_STRIDE_DISPATCH(stride, DWR_WGRAD);
+#undef DWR_WGRAD
+  const long long n = 9ll * C;
+  B200_CHECK_CUDA(launch_pdl(dw_wgrad_reduce_kernel, dim3(static_cast<unsigned>((n + 31) / 32)), dim3(256), 0,
+                             as_stream(stream), static_cast<const float*>(pws), dw, gm.blocks, 9, C));
   B200_LAUNCHED();
   return OK;
 }

@@ -66,21 +66,35 @@ __device__ __forceinline__ void dw_tap8(const float (*ws)[64], int tap, int lane
   t[4] = b.x; t[5] = b.y; t[6] = b.z; t[7] = b.w;
 }
 
-// 8 input channels at (b, ih, iw), with silu(x * sc + sh) applied when PRE
-template <bool PRE>
+// What the depthwise passes apply to their input on load (template argument PRE): nothing, the previous BatchNorm + SiLU
+// (EfficientNet), or the previous BatchNorm + ReLU (ShuffleNet, shufflenet.cuh).  A bool true selects kDwSilu.
+constexpr int kDwRaw = 0, kDwSilu = 1, kDwRelu = 2;
+
+// 8 input channels at (b, ih, iw), with silu / relu(x * sc + sh) applied when PRE
+template <int PRE>
 __device__ __forceinline__ void dw_load_in(const __nv_bfloat16* __restrict__ x, long long pix, int C, int cg,
                                            const float (&sc)[8], const float (&sh)[8], float (&v)[8]) {
   unpack8(__ldg(reinterpret_cast<const uint4*>(x + pix * C) + cg), v);
-  if constexpr (PRE) {
+  if constexpr (PRE == kDwSilu) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) v[j] = mb_silu(fmaf(v[j], sc[j], sh[j]));
+  } else if constexpr (PRE == kDwRelu) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = fmaxf(fmaf(v[j], sc[j], sh[j]), 0.f);
   }
+}
+
+// derivative of the on-load activation at u = x * sc + sh (relu'(0) = 0, as torch's ReLU backward)
+template <int PRE>
+__device__ __forceinline__ float dw_dact(float u) {
+  if constexpr (PRE == kDwRelu) return u > 0.f ? 1.f : 0.f;
+  else return mb_dsilu(u);
 }
 
 // ---------------------------------------------------------------------------------------------- depthwise forward
 // d[b][oh][ow][c] = sum_taps in(b, oh*S - K/2 + kh, ow*S - K/2 + kw, c) w[c][kh][kw]; stats [T][2][C] = sums of the stored
 // bf16 d and d^2 per CTA row range.
-template <int K, int S, bool PRE, bool STATS>
+template <int K, int S, int PRE, bool STATS>
 __global__ void __launch_bounds__(256, 2) dw_fwd_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w,
                                                      const float* __restrict__ scale, const float* __restrict__ shift,
                                                      __nv_bfloat16* __restrict__ d, float* __restrict__ stats, int B, int H,
@@ -150,9 +164,9 @@ __global__ void __launch_bounds__(256, 2) dw_fwd_kernel(const __nv_bfloat16* __r
 
 // --------------------------------------------------------------------------------------------- depthwise data gradient
 // g_in[b][ih][iw][c] = sum over the taps that read (ih, iw) of dd[b][oh][ow][c] w[c][kh][kw], rows = input pixels.
-// PRE (the input was normalised on load): dx = g_in silu'(x sc + sh) and partial [T][2][C] = {sum dx, sum dx x} of the
+// PRE (the input was normalised on load): dx = g_in act'(x sc + sh) and partial [T][2][C] = {sum dx, sum dx x} of the
 // stored bf16 dx; RES: dx = g_in + residual.
-template <int K, int S, bool PRE, bool RES>
+template <int K, int S, int PRE, bool RES>
 __global__ void __launch_bounds__(256, 2) dw_dgrad_kernel(const __nv_bfloat16* __restrict__ dd, const float* __restrict__ w,
                                                        const __nv_bfloat16* __restrict__ x, const float* __restrict__ scale,
                                                        const float* __restrict__ shift,
@@ -208,7 +222,7 @@ __global__ void __launch_bounds__(256, 2) dw_dgrad_kernel(const __nv_bfloat16* _
         float xv[8];
         unpack8(__ldg(reinterpret_cast<const uint4*>(x + r * C) + cg), xv);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] *= mb_dsilu(fmaf(xv[j], sc[j], sh[j]));
+        for (int j = 0; j < 8; ++j) o[j] *= dw_dact<PRE>(fmaf(xv[j], sc[j], sh[j]));
         const uint4 q = pack8(o);
         reinterpret_cast<uint4*>(dx + r * C)[cg] = q;
         unpack8(q, o);
@@ -241,8 +255,9 @@ __global__ void __launch_bounds__(256, 2) dw_dgrad_kernel(const __nv_bfloat16* _
 // ------------------------------------------------------------------------------------------- depthwise weight gradient
 // CTA (row range, 64-channel block, kernel row kh = blockIdx.z): ws[T][kh][kw][C] = sum over its output pixels of
 // dd[b][oh][ow][c] in(b, oh*S - K/2 + kh, ow*S - K/2 + kw, c); dw_wgrad_reduce_kernel sums the T slabs in order.
-template <int K, int S, bool PRE>
-__global__ void __launch_bounds__(256) dw_wgrad_kernel(const __nv_bfloat16* __restrict__ dd,
+// (ptxas' default register budget spills the ReLU mode; a one-CTA minimum lifts it and leaves the other modes' code as is)
+template <int K, int S, int PRE>
+__global__ void __launch_bounds__(256, PRE == kDwRelu ? 1 : 0) dw_wgrad_kernel(const __nv_bfloat16* __restrict__ dd,
                                                        const __nv_bfloat16* __restrict__ x, const float* __restrict__ scale,
                                                        const float* __restrict__ shift, float* __restrict__ ws, int B, int H,
                                                        int W, int Ho, int Wo, int C, int rows_per_block) {

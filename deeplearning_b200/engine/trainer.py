@@ -65,6 +65,12 @@ def _engine_for(model):
         from . import vgg
 
         return vgg
+    from ..classification.ShuffleNet.models.shufflenetv1 import ShuffleNetv1
+
+    if isinstance(model, ShuffleNetv1):
+        from . import shufflenet
+
+        return shufflenet
     raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 

@@ -1863,3 +1863,111 @@ def adam_(p, g, m, v, hyper, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0,
     rc = lib.b200_adam(_p(p), _p(g), _p(m), _p(v), p.numel(), _p(hyper), beta1, beta2, eps, weight_decay, gscale, _p(clip),
                        _stream())
     _lib.check(rc, "b200_adam")
+
+
+# ------------------------------------------------------------------------------ ShuffleNet v1 passes (csrc/shufflenet.cuh)
+def dw_relu_fwd(x, w, stride, co, want_stats=False):
+    """3x3 depthwise convolution (padding 1) of relu(x * scale + shift) (BnCoeffs ``co``: the previous BatchNorm + ReLU
+    applied on load), fp32 weight [C, 1, 3, 3].  Returns (d bf16 [B,Ho,Wo,C], stats fp32 [T,2,C] of the stored d, or None)."""
+    lib = _lib.load()
+    B, H, W, C, Ho, Wo = _dw_args(x, 3, stride)
+    w = _f32_param(w)
+    d = torch.empty(B, Ho, Wo, C, dtype=BF16, device=x.device)
+    stats = None
+    if want_stats:
+        stats = torch.empty(_mb_rows(lib.b200_dw_partial_rows, B * Ho * Wo, C), 2, C, dtype=F32, device=x.device)
+    sp = _span("dw_relu_fwd", 18.0 * d.numel(), _nb(x, d))
+    rc = lib.b200_dw_relu_fwd(_p(x), _p(w), _p(co.scale), _p(co.shift), _p(d), _p(stats), B, H, W, C, stride, _stream())
+    _lib.check(rc, "b200_dw_relu_fwd")
+    if sp:
+        sp.end()
+    return d, stats
+
+
+def dw_relu_dgrad(dd, w, x, stride, co):
+    """Data gradient of dw_relu_fwd for dd = dL/dd: (dz, partial) with dz = g_in * [x * scale + shift > 0] bf16 and
+    partial fp32 [T,2,C] = {sum dz, sum dz * x}, the rows bn_bwd_finalize reads for the BatchNorm applied on load."""
+    lib = _lib.load()
+    _chk_act(dd, "dd")
+    B, H, W, C, Ho, Wo = _dw_args(x, 3, stride)
+    if tuple(dd.shape) != (B, Ho, Wo, C):
+        raise ValueError(f"dw_relu_dgrad: dd {tuple(dd.shape)} does not match the output of x {tuple(x.shape)}")
+    w = _f32_param(w)
+    dx = torch.empty_like(x)
+    partial = torch.empty(_mb_rows(lib.b200_dw_partial_rows, B * H * W, C), 2, C, dtype=F32, device=x.device)
+    sp = _span("dw_relu_dgrad", 18.0 * dd.numel(), _nb(dd, x, dx))
+    rc = lib.b200_dw_relu_dgrad(_p(dd), _p(w), _p(x), _p(co.scale), _p(co.shift), _p(dx), _p(partial), B, H, W, C, stride,
+                                _stream())
+    _lib.check(rc, "b200_dw_relu_dgrad")
+    if sp:
+        sp.end()
+    return dx, partial
+
+
+def dw_relu_wgrad(dd, x, stride, co, out=None):
+    """Weight gradient fp32 [C, 1, 3, 3] of dw_relu_fwd (``out`` receives it when given)."""
+    lib = _lib.load()
+    _chk_act(dd, "dd")
+    B, H, W, C, Ho, Wo = _dw_args(x, 3, stride)
+    nbytes = lib.b200_dw_wgrad_workspace_bytes(B, H, W, C, 3, stride)
+    ws = _workspace(nbytes, x.device)
+    if out is None:
+        out = torch.empty(C, 1, 3, 3, dtype=F32, device=x.device)
+    sp = _span("dw_relu_wgrad", 18.0 * dd.numel(), _nb(dd, x))
+    rc = lib.b200_dw_relu_wgrad(_p(dd), _p(x), _p(co.scale), _p(co.shift), _p(out), _p(ws), nbytes, B, H, W, C, stride,
+                                _stream())
+    _lib.check(rc, "b200_dw_relu_wgrad")
+    if sp:
+        sp.end()
+    return out
+
+
+def shuffle_tail_s2_fwd(x, c3, co):
+    """Stride-2 ShuffleNet block output bf16 [B,Ho,Wo,Cin+Cc] = cat(relu(avg_pool3x3/2/p1(x)), relu(c3 * scale + shift))."""
+    lib = _lib.load()
+    _chk_act(x, "x")
+    _chk_act(c3, "c3")
+    B, H, W, Cin = x.shape
+    Cc = c3.shape[-1]
+    Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    if tuple(c3.shape) != (B, Ho, Wo, Cc):
+        raise ValueError(f"shuffle_tail_s2_fwd: c3 {tuple(c3.shape)} does not match the pooled x {(B, Ho, Wo)}")
+    y = torch.empty(B, Ho, Wo, Cin + Cc, dtype=BF16, device=x.device)
+    sp = _span("shuffle_tail_s2_fwd", 0.0, _nb(x, c3, y))
+    rc = lib.b200_shuffle_tail_s2_fwd(_p(x), _p(c3), _p(co.scale), _p(co.shift), _p(y), B, H, W, Cin, Cc, _stream())
+    _lib.check(rc, "b200_shuffle_tail_s2_fwd")
+    if sp:
+        sp.end()
+    return y
+
+
+def shuffle_relu_bwd(g, c, y=None, co=None, in_hw=None):
+    """ReLU-masked gradient of a ShuffleNet BatchNorm output c (bf16 [B,Ho,Wo,Cc]).  Returns (dz, partial, gx):
+    dz = g * mask bf16 [B,Ho,Wo,Cc], partial fp32 [T,2,Cc] = {sum dz, sum dz * c}.
+    - y given (block output, [B,Ho,Wo,Cin+Cc], g of the same shape): mask = y[..., Cin:] > 0.  With Cin > 0 (stride-2
+      tail, ``in_hw`` = (H, W) of the block input) gx bf16 [B,H,W,Cin] is the avg-pool backward of g * [y > 0] over the
+      first Cin channels; else gx is None.
+    - co given (stem): mask = c * scale + shift > 0, g shaped like c."""
+    lib = _lib.load()
+    _chk_act(g, "g")
+    _chk_act(c, "c")
+    B, Ho, Wo, Cc = c.shape
+    Cin = 0 if y is None else y.shape[-1] - Cc
+    if y is not None:
+        _chk_act(y, "y")
+        if tuple(g.shape) != tuple(y.shape) or tuple(y.shape[:3]) != (B, Ho, Wo):
+            raise ValueError(f"shuffle_relu_bwd: g {tuple(g.shape)} / y {tuple(y.shape)} / c {tuple(c.shape)} disagree")
+    elif tuple(g.shape) != tuple(c.shape):
+        raise ValueError(f"shuffle_relu_bwd: g {tuple(g.shape)} must be shaped like c {tuple(c.shape)}")
+    H, W = in_hw if Cin > 0 else (0, 0)
+    dz = torch.empty_like(c)
+    partial = torch.empty(repvgg_partial_rows(B * Ho * Wo, Cc), 2, Cc, dtype=F32, device=c.device)
+    gx = torch.empty(B, H, W, Cin, dtype=BF16, device=c.device) if Cin > 0 else None
+    sp = _span("shuffle_relu_bwd", 0.0, _nb(g, y, c, dz, gx))
+    rc = lib.b200_shuffle_relu_bwd(_p(g), _p(y), _p(c), None if co is None else _p(co.scale),
+                                   None if co is None else _p(co.shift), _p(dz), _p(partial), _p(gx), B, Ho, Wo, Cin, Cc, H, W,
+                                   _stream())
+    _lib.check(rc, "b200_shuffle_relu_bwd")
+    if sp:
+        sp.end()
+    return dz, partial, gx

@@ -546,6 +546,29 @@ int b200_vgg_dropout_bwd(const void* g, const void* h, float scale, void* dx, lo
 int b200_adam(float* p, const float* g, float* m, float* v, long long n, const float* hyper, float beta1, float beta2,
               float eps, float weight_decay, float gscale, const float* clip_coef, void* stream);
 
+/* ShuffleNet v1 passes (classification/ShuffleNet/models/shufflenetv1.py ResidualBlock; csrc/shufflenet.cuh).  NHWC bf16
+ * activations, fp32 parameters / coefficients / partial rows, every sum in fp32 in a fixed order.
+ * dw_relu_*:  the 3x3 depthwise convolution (padding 1, stride 1 or 2) of relu(x * scale + shift), the previous BatchNorm +
+ *             ReLU applied on load: b200_dw_fwd / _dgrad / _wgrad with ReLU in place of SiLU (same shapes, geometry,
+ *             partial rows b200_dw_partial_rows and workspace b200_dw_wgrad_workspace_bytes with k = 3).  dgrad writes
+ *             dx = g_in [x * scale + shift > 0] and partial = {sum dx, sum dx x}
+ * shuffle_tail_s2_fwd: the stride-2 block output y [B][Ho][Wo][Cin + Cc], Ho = (H - 1) / 2 + 1:
+ *             y[..., :Cin] = relu(avg_pool3x3/2/p1(x) (divisor 9)), y[..., Cin:] = relu(c3 * scale + shift)
+ * shuffle_relu_bwd: dz [B][Ho][Wo][Cc] = g [mask] stored, partial [b200_repvgg_partial_rows(B Ho Wo, Cc)][2][Cc] =
+ *             {sum dz, sum dz c}.  With y: g and y have row pitch Cin + Cc and the mask is y[..., Cin:] > 0; with Cin > 0
+ *             gx [B][H][W][Cin] is also written (the same launch): the avg-pool backward of g [y > 0] over y's first Cin
+ *             channels, / 9.  Without y (scale, shift given, Cin == 0, no gx): the mask is c * scale + shift > 0 */
+int b200_dw_relu_fwd(const void* x, const float* w, const float* scale, const float* shift, void* d, float* stats, int B,
+                     int H, int W, int C, int stride, void* stream);
+int b200_dw_relu_dgrad(const void* dd, const float* w, const void* x, const float* scale, const float* shift, void* dx,
+                       float* partial, int B, int H, int W, int C, int stride, void* stream);
+int b200_dw_relu_wgrad(const void* dd, const void* x, const float* scale, const float* shift, float* dw, void* ws,
+                       size_t ws_bytes, int B, int H, int W, int C, int stride, void* stream);
+int b200_shuffle_tail_s2_fwd(const void* x, const void* c3, const float* scale, const float* shift, void* y, int B, int H,
+                             int W, int Cin, int Cc, void* stream);
+int b200_shuffle_relu_bwd(const void* g, const void* y, const void* c, const float* scale, const float* shift, void* dz,
+                          float* partial, void* gx, int B, int Ho, int Wo, int Cin, int Cc, int H, int W, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

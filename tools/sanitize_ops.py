@@ -1,6 +1,6 @@
 """One small launch of every wgmma / TMA kernel family, for `compute-sanitizer --tool {memcheck,racecheck,synccheck}`:
 implicit-GEMM conv (forward + statistics, dgrad + residual, affine / mask epilogues, dual-source K), the streaming 1x1 kernel
-(both modes), wgrad, ViT attention forward / backward, window attention forward / backward, BN-algebra kernels, the VGG passes.
+(both modes), wgrad, ViT attention forward / backward, window attention forward / backward, BN-algebra kernels, the VGG passes, the ShuffleNet passes.
 usage: compute-sanitizer --tool racecheck python tools/sanitize_ops.py [family ...]"""
 import os
 import sys
@@ -12,7 +12,7 @@ from deeplearning_b200 import ops
 
 dev = torch.device("cuda")
 BF = torch.bfloat16
-fam = set(sys.argv[1:]) or {"conv", "stream", "wgrad", "attn", "attn2", "ln", "wattn", "algebra", "vgg"}
+fam = set(sys.argv[1:]) or {"conv", "stream", "wgrad", "attn", "attn2", "ln", "wattn", "algebra", "vgg", "shufflenet"}
 
 
 def r(*shape, scale=1.0):
@@ -108,5 +108,23 @@ if "vgg" in fam:
     p, gg = torch.randn(1001, device=dev), torch.randn(1001, device=dev)
     ops.adam_(p, gg, torch.zeros_like(p), torch.zeros_like(p), torch.tensor([1e-3, 0, 0, 1, 1.0], device=dev), weight_decay=1e-3)
     print("vgg ok", float(d.float().abs().mean()), float(gx.float().abs().mean()), float(dh.float().abs().mean()))
+if "shufflenet" in fam:
+    # ShuffleNet passes (shufflenet.cuh, mbconv.cuh's ReLU mode): depthwise forward / dgrad / wgrad at a padded width,
+    # the stride-2 tail forward and its backward with the pool half (odd H / W), the stride-1 and stem ReLU reduces
+    c1 = r(2, 9, 7, 32)
+    co = ops.BnCoeffs(32, dev)
+    co.scale.fill_(1.0), co.shift.fill_(0.1), co.mean.zero_(), co.invstd.fill_(1.0)
+    for s in (1, 2):
+        d, _ = ops.dw_relu_fwd(c1, torch.randn(32, 1, 3, 3, device=dev), s, co, want_stats=True)
+        dz, _ = ops.dw_relu_dgrad(r(*d.shape), torch.randn(32, 1, 3, 3, device=dev), c1, s, co)
+        gw = ops.dw_relu_wgrad(r(*d.shape), c1, s, co)
+    c3 = r(2, 5, 4, 40)
+    co3 = ops.BnCoeffs(40, dev)
+    co3.scale.fill_(1.0), co3.shift.fill_(0.1), co3.mean.zero_(), co3.invstd.fill_(1.0)
+    y = ops.shuffle_tail_s2_fwd(r(2, 9, 7, 24), c3, co3)
+    dz3, _, gx = ops.shuffle_relu_bwd(r(*y.shape), c3, y=y, in_hw=(9, 7))
+    dz1, _, _ = ops.shuffle_relu_bwd(r(2, 9, 7, 32), c1, y=torch.relu(r(2, 9, 7, 32)))
+    dzs, _, _ = ops.shuffle_relu_bwd(r(2, 9, 7, 32), c1, co=co)
+    print("shufflenet ok", float(dz.float().abs().mean()), float(gw.abs().mean()), float(gx.float().abs().mean()))
 torch.cuda.synchronize()
 print("done")
