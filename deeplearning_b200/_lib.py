@@ -155,7 +155,6 @@ SIGNATURES = {
     "b200_silu_bn_bwd_reduce": (_I, [_P] * 8 + [_I] * 3 + [_P]),
     "b200_tail_apply": (_I, [_P] * 6 + [_I] * 3 + [_P]),
     "b200_tail_bwd_reduce": (_I, [_P] * 5 + [_I] * 3 + [_P]),
-    "b200_bn_bwd_apply_dz": (_I, [_P] * 5 + [_L, _I, _P]),
     "b200_dw_relu_fwd": (_I, [_P] * 6 + [_I] * 5 + [_P]),
     "b200_dw_relu_dgrad": (_I, [_P] * 7 + [_I] * 5 + [_P]),
     "b200_dw_relu_wgrad": (_I, [_P] * 6 + [c_size_t] + [_I] * 5 + [_P]),

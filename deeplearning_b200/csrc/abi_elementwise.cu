@@ -1,4 +1,5 @@
 // C-ABI entry points for the HBM-bound passes (see elementwise.cuh).
+#include <stdint.h>
 #include <string.h>
 
 #include "../../include/b200cls.h"
@@ -17,6 +18,7 @@ inline int ew_grid(long long work_items, int block = 256) {
   return static_cast<int>(blocks);
 }
 inline bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
+inline bool aligned16(const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 inline int reduce_slices(int T) {
   int s = T / 64;
   if (s < 1) s = 1;
@@ -42,7 +44,7 @@ BnBwdPlan plan_bn_bwd(long long rows, int C) {
 extern "C" {
 
 const char* b200_last_error(void) { return get_error(); }
-int b200_abi_version(void) { return 2; }
+int b200_abi_version(void) { return 3; }
 int b200_sm_count(void) { return device_sm_count(); }
 unsigned long long b200_launch_count(void) { return g_launch_count; }
 
@@ -113,11 +115,18 @@ int b200_bn_bwd_finalize(const float* partial, int T, int C, double count, float
 int b200_bn_bwd_apply(const void* g, const void* x, const void* y_out, int g_is_dz, void* dx, const float* scale,
                       const float* shift, const float* mean, const float* invstd, const float* m1, const float* m2,
                       int relu, long long rows, int C, void* stream) {
-  B200_REQUIRE(C % 8 == 0 && pow2(C / 8) && C / 8 <= 256, "bn_bwd_apply: C=%d must be 8*2^k <= 2048", C);
-  const BnBwdPlan pl = plan_bn_bwd(rows, C);
-  B200_CHECK_CUDA(launch_pdl(bn_bwd_apply_kernel, dim3(pl.blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint4*>(g), static_cast<const uint4*>(x), static_cast<const uint4*>(y_out), g_is_dz,
-      static_cast<uint4*>(dx), scale, shift, mean, invstd, m1, m2, relu, rows, C / 8, pl.rows_per_block));
+  B200_REQUIRE(rows >= 1 && C >= 8 && C % 8 == 0 && C <= kRvMaxC,
+               "bn_bwd_apply: need rows >= 1 and C a multiple of 8 in [8, 8192] (rows=%lld C=%d)", rows, C);
+  B200_REQUIRE(aligned16(g) && aligned16(x) && aligned16(dx) && aligned16(scale) && aligned16(shift) &&
+                   aligned16(mean) && aligned16(invstd) && aligned16(m1) && aligned16(m2) &&
+                   (y_out == nullptr || aligned16(y_out)),
+               "bn_bwd_apply: g, x, dx, scale, shift, mean, invstd, m1, m2 (and y_out) must be non-null and 16-byte "
+               "aligned");
+  const RvGeom gm = repvgg_geom(rows, C);
+  B200_CHECK_CUDA(launch_pdl(bn_bwd_apply_kernel, dim3(gm.blocks, gm.nchunk), dim3(256), 0,
+      static_cast<cudaStream_t>(stream), static_cast<const uint4*>(g), static_cast<const uint4*>(x),
+      static_cast<const uint4*>(y_out), g_is_dz, static_cast<uint4*>(dx), scale, shift, mean, invstd, m1, m2, relu, rows,
+      C / 8, gm.rows_per_block, gm.gpc));
   B200_LAUNCHED();
   return OK;
 }

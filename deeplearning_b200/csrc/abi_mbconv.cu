@@ -387,18 +387,4 @@ int b200_tail_bwd_reduce(const void* g, const float* rs, const void* c, void* dz
   return OK;
 }
 
-int b200_bn_bwd_apply_dz(const void* dz, const void* c, const float* co, const float* m, void* dc, long long rows, int C,
-                         void* stream) {
-  B200_REQUIRE(rows >= 1 && C >= 8 && C % 8 == 0 && C <= kRvMaxC,
-               "bn_bwd_apply_dz: need rows >= 1 and C a multiple of 8 in [8, 8192] (rows=%lld C=%d)", rows, C);
-  B200_REQUIRE(aligned16(dz) && aligned16(c) && aligned16(co) && aligned16(m) && aligned16(dc),
-               "bn_bwd_apply_dz: dz, c, co, m, dc must be non-null and 16-byte aligned");
-  const RvGeom gm = repvgg_geom(rows, C);
-  B200_CHECK_CUDA(launch_pdl(mb_bn_bwd_apply_kernel, dim3(gm.blocks, gm.nchunk), dim3(256), 0, as_stream(stream),
-                             static_cast<const uint4*>(dz), static_cast<const uint4*>(c), co, m, static_cast<uint4*>(dc),
-                             rows, C, gm.rows_per_block, gm.gpc));
-  B200_LAUNCHED();
-  return OK;
-}
-
 }  // extern "C"

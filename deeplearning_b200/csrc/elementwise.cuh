@@ -7,7 +7,7 @@
 // as used at classification/resnet/models/networks.py:45,91,134; MaxPool2d(3,2,1) :152; AdaptiveAvgPool2d(1) :160;
 // CrossEntropyLoss (classification/resnet/train.py:104); SGD momentum (classification/resnet/train.py:96).
 #pragma once
-#include "common.cuh"
+#include "row_passes.cuh"
 
 namespace b200 {
 
@@ -294,36 +294,26 @@ __global__ void bn_bwd_finalize_kernel(const float* __restrict__ partial, int T,
   }
 }
 
-// BN backward, pass 2: dx = scale * (dz - m1 - xhat * m2), dz recomputed exactly as in pass 1 (or read from dz_in).
-// Same thread mapping as pass 1 (a thread owns one 8-channel group; per-channel vectors live in registers).
+// BN backward, pass 2: dx = scale * (dz - m1 - xhat * m2), dz recomputed exactly as in pass 1 (or read from g when
+// g_is_dz).  Row geometry of row_passes.cuh (repvgg_geom): gridDim.y chunks of gpc 8-channel groups, so any C % 8 == 0 up
+// to 8192 runs; for C = 8 * 2^k <= 2048 that is pass 1's grid and thread mapping.
 __global__ void bn_bwd_apply_kernel(const uint4* __restrict__ g, const uint4* __restrict__ x,
                                     const uint4* __restrict__ y_out, int g_is_dz, uint4* __restrict__ dx,
                                     const float* __restrict__ scale, const float* __restrict__ shift,
                                     const float* __restrict__ mean, const float* __restrict__ invstd,
                                     const float* __restrict__ m1, const float* __restrict__ m2, int relu,
-                                    long long rows, int cvec, int rows_per_block) {
+                                    long long rows, int cvec, int rows_per_block, int gpc) {
   pdl_wait();
-  const int tpr = cvec, rpi = 256 / tpr;
-  const int cg = threadIdx.x % tpr, rsub = threadIdx.x / tpr;
-  float sc[8], sh[8], a[8], bq[8], cq[8];
-  {
-    float mu[8], is[8], q1[8], q2[8];
-    load8f(scale + cg * 8, sc);
-    load8f(shift + cg * 8, sh);
-    load8f(mean + cg * 8, mu);
-    load8f(invstd + cg * 8, is);
-    load8f(m1 + cg * 8, q1);
-    load8f(m2 + cg * 8, q2);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      // dx = sc*(dz - q1 - (x-mu)*is*q2) = a*dz - bq*x + cq
-      a[j] = sc[j];
-      bq[j] = sc[j] * is[j] * q2[j];
-      cq[j] = sc[j] * (mu[j] * is[j] * q2[j] - q1[j]);
-    }
-  }
+  const int rpi = 256 / gpc;
+  const int lane_g = threadIdx.x % gpc, rsub = threadIdx.x / gpc;
+  const int cg = blockIdx.y * gpc + lane_g;
+  if (rsub >= rpi || cg >= cvec) return;
+  // dx = a * dz - bq * x + cq, a = scale
+  float a[8], bq[8], cq[8], sh[8];
+  rv_bwd_coeffs(mean, invstd, scale, m1, m2, cg, a, bq, cq);
   const bool mask_from_x = relu && !g_is_dz && (y_out == nullptr);
   const bool mask_from_y = relu && !g_is_dz && (y_out != nullptr);
+  if (mask_from_x) load8f(shift + cg * 8, sh);
   const long long r0 = static_cast<long long>(blockIdx.x) * rows_per_block;
   const long long r1 = min(rows, r0 + rows_per_block);
   // four rows in flight per thread (8-12 independent 16-byte loads): the two-row version left HBM at ~4.7 TB/s
@@ -354,7 +344,7 @@ __global__ void bn_bwd_apply_kernel(const uint4* __restrict__ g, const uint4* __
         for (int j = 0; j < 8; ++j) gv[j] = yv[j] > 0.f ? gv[j] : 0.f;
       } else if (mask_from_x) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) gv[j] = fmaf(xv[j], sc[j], sh[j]) > 0.f ? gv[j] : 0.f;
+        for (int j = 0; j < 8; ++j) gv[j] = fmaf(xv[j], a[j], sh[j]) > 0.f ? gv[j] : 0.f;
       }
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = fmaf(a[j], gv[j], fmaf(-bq[j], xv[j], cq[j]));

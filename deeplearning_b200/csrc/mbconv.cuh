@@ -9,7 +9,7 @@
 //             gate reduce      S = sum_p da silu(u_d)   (u = the BatchNorm output)
 //             excite backward  dW1, db1, dW2, db2 and dpool from S
 //             SiLU-BN reduce   dz = (da gate + dpool / HW) silu'(u_d), {sum dz, sum dz d}
-//             BN apply from dz dc = scale (dz - m1 - xhat m2)
+//             BN apply from dz dc = scale (dz - m1 - xhat m2)   (b200_bn_bwd_apply, elementwise.cuh)
 //             depthwise dgrad  (+ residual) or x silu'(u_in) with the input BatchNorm's {sum dz, sum dz x}
 //             depthwise wgrad  dW [C][k*k]
 //
@@ -594,26 +594,6 @@ __global__ void __launch_bounds__(256, 2) mb_bwd_reduce_kernel(
       p[j] = acc[0][j];
       p[C + j] = acc[1][j];
     }
-  }
-}
-
-// BatchNorm backward apply from a stored dz: dc = scale (dz - m1 - (c - mean) invstd m2), co [4][C], m [2][C]
-__global__ void __launch_bounds__(256) mb_bn_bwd_apply_kernel(const uint4* __restrict__ dz, const uint4* __restrict__ c,
-                                                              const float* __restrict__ co, const float* __restrict__ m,
-                                                              uint4* __restrict__ dc, long long rows, int C,
-                                                              int rows_per_block, int gpc) {
-  pdl_wait();
-  MB_ROWS_PROLOGUE;
-  if (!live) return;
-  float a[8], bq[8], cq[8];
-  rv_bwd_coeffs(co, m, C, cg, a, bq, cq);
-  for (long long r = r0 + rsub; r < r1; r += rpi) {
-    float z[8], u[8];
-    unpack8(__ldg(dz + r * cvec + cg), z);
-    unpack8(__ldg(c + r * cvec + cg), u);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) u[j] = fmaf(a[j], z[j], fmaf(-bq[j], u[j], cq[j]));
-    dc[r * cvec + cg] = pack8(u);
   }
 }
 

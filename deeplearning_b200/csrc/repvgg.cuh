@@ -187,9 +187,9 @@ __global__ void __launch_bounds__(256) repvgg_bwd_apply_kernel(
   const int cg = blockIdx.y * gpc + lane_g;
   if (rsub >= rpi || cg >= cvec) return;
   float a3[8], b3[8], k3[8], a1[8], b1[8], k1[8], ai[8], bi[8], ki[8];
-  rv_bwd_coeffs(co3, m3, C, cg, a3, b3, k3);
-  rv_bwd_coeffs(co1, m1, C, cg, a1, b1, k1);
-  if constexpr (ID) rv_bwd_coeffs(coid, mid, C, cg, ai, bi, ki);
+  rv_bwd_coeffs(co3, co3 + C, co3 + 2 * C, m3, m3 + C, cg, a3, b3, k3);
+  rv_bwd_coeffs(co1, co1 + C, co1 + 2 * C, m1, m1 + C, cg, a1, b1, k1);
+  if constexpr (ID) rv_bwd_coeffs(coid, coid + C, coid + 2 * C, mid, mid + C, cg, ai, bi, ki);
   const long long r0 = static_cast<long long>(blockIdx.x) * rows_per_block;
   const long long r1 = min(rows, r0 + rows_per_block);
   for (long long r = r0 + rsub; r < r1; r += 2 * rpi) {

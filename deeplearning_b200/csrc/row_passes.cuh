@@ -1,6 +1,6 @@
-// Helpers of the row-streaming BatchNorm passes (repvgg.cuh, mbconv.cuh): the thread / CTA geometry over [rows][C] NHWC
-// tensors, the fixed-order CTA reduction of per-channel sums into one [2][C] partial row per CTA, and the coefficients of the
-// BatchNorm backward apply.
+// Helpers of the row-streaming BatchNorm passes (repvgg.cuh, mbconv.cuh, elementwise.cuh's BatchNorm backward apply): the
+// thread / CTA geometry over [rows][C] NHWC tensors, the fixed-order CTA reduction of per-channel sums into one [2][C]
+// partial row per CTA, and the coefficients of the BatchNorm backward apply.
 //
 // Thread mapping: a thread owns one 8-channel group (16-byte vectors) of a channel chunk (gridDim.y chunks of <= 256 groups)
 // and strides over the rows of its CTA's row range; the rpi = 256 / gpc threads of a group reduce their sums through shared
@@ -59,16 +59,18 @@ __device__ __forceinline__ bool rv_cta_reduce(float (&acc)[NS][8], int gpc, int 
   return true;
 }
 
-// dc = a * dz - bq * c + cq with a = scale, bq = scale * invstd * m2, cq = scale * (mean * invstd * m2 - m1)
-// (b200_bn_bwd_apply's algebra); co = {mean, invstd, scale, shift} [4][C], m = {m1, m2} [2][C]
-__device__ __forceinline__ void rv_bwd_coeffs(const float* __restrict__ co, const float* __restrict__ m, int C, int cg,
-                                              float (&a)[8], float (&bq)[8], float (&cq)[8]) {
+// dc = a * dz - bq * c + cq with a = scale, bq = scale * invstd * m2, cq = scale * (mean * invstd * m2 - m1): the
+// BatchNorm backward apply, dc = scale * (dz - m1 - (c - mean) * invstd * m2), for channel group cg
+__device__ __forceinline__ void rv_bwd_coeffs(const float* __restrict__ mean, const float* __restrict__ invstd,
+                                              const float* __restrict__ scale, const float* __restrict__ m1,
+                                              const float* __restrict__ m2, int cg, float (&a)[8], float (&bq)[8],
+                                              float (&cq)[8]) {
   float mu[8], is[8], q1[8], q2[8];
-  load8f(co + cg * 8, mu);
-  load8f(co + C + cg * 8, is);
-  load8f(co + 2 * C + cg * 8, a);
-  load8f(m + cg * 8, q1);
-  load8f(m + C + cg * 8, q2);
+  load8f(mean + cg * 8, mu);
+  load8f(invstd + cg * 8, is);
+  load8f(scale + cg * 8, a);
+  load8f(m1 + cg * 8, q1);
+  load8f(m2 + cg * 8, q2);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     bq[j] = a[j] * is[j] * q2[j];

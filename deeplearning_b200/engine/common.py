@@ -1,11 +1,16 @@
-"""Plumbing shared by the engine schedules (resnet, vit, swin, convnext): the class-padded classifier head, the gradient
-sink, the Linear / LayerNorm gradient helpers, the image-input prefix and the autograd entry point ``apply``.
+"""Plumbing shared by the engine schedules: the class-padded classifier head, the gradient sink, the Linear / LayerNorm
+gradient helpers, the BatchNorm admission / coefficient / backward helpers of the CNN engines, the classifier-dropout mask
+and its test hooks, the image-input prefix and the autograd entry point ``apply``.
 
 Classifier layout: the conv GEMMs take channel counts in multiples of 8, so the head runs with ``padded_classes(num_classes)``
 output columns and the fused cross-entropy writes ``dlogits`` with that row stride; the logits a schedule returns are the
 first ``num_classes`` columns of the head's output.
 """
+import contextlib
+
 import torch
+import torch.nn as nn
+import torch.nn.functional as F
 
 from .. import ops
 
@@ -27,7 +32,9 @@ class Grads(dict):
         self.sink = sink
 
     def dest(self, param):
-        return self.sink(param) if self.sink is not None else None
+        """The sink's buffer for ``param``'s gradient, viewed as the parameter's shape; None without a sink."""
+        d = self.sink(param) if self.sink is not None else None
+        return None if d is None else d.view(param.shape)
 
     def put(self, param, value):
         """Record the (final) gradient of ``param``; a sink with a ``notify`` method is told so that the data-parallel
@@ -130,6 +137,96 @@ def layernorm_backward(grads, norm, dy, x, mean, rstd, add=None):
     grads.put(norm.weight, dgamma)
     grads.put(norm.bias, dbeta)
     return dx
+
+
+def rows(t):
+    """Row count of an NHWC activation: the number of values per channel."""
+    return t.numel() // t.shape[-1]
+
+
+def bn_ok(bn, C):
+    """``bn`` is an affine BatchNorm2d / SyncBatchNorm over C channels that tracks running statistics with a momentum."""
+    return (type(bn) in (nn.BatchNorm2d, nn.SyncBatchNorm) and bn.num_features == C and bn.affine
+            and bn.track_running_stats and bn.momentum is not None)
+
+
+def bn_sync(bn):
+    """(process_group, world_size) when ``bn`` is a SyncBatchNorm in a multi-rank job (the recipe converts every BatchNorm
+    with ``nn.SyncBatchNorm.convert_sync_batchnorm``: others/train_with_DDP/train.py:190), else None.  Statistics and the
+    two backward sums are then all-reduced per layer (ops._sync_sums)."""
+    if not isinstance(bn, nn.SyncBatchNorm) or not bn.training:
+        return None
+    import torch.distributed as dist
+
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
+    world = dist.get_world_size(group)
+    return (group, world) if world > 1 else None
+
+
+def bn_coeffs(bn, stats, rows, train):
+    """BatchNorm coefficients: from the batch statistics (``rows`` values per channel, running statistics updated) in
+    train mode, from the running statistics in eval mode."""
+    if train:
+        return ops.bn_finalize(stats, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
+                               bn.num_batches_tracked, sync=bn_sync(bn))
+    return ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+
+
+def bn_backward_from_sums(grads, bn, dz, partial, c, co):
+    """dc of a train-mode BatchNorm over the raw input c from its masked gradient dz and partial sums {sum dz, sum dz * c};
+    records the bias and then the weight gradient (reverse parameter order, as the overlapped all-reduce walks the arena)."""
+    dc, dgamma, dbeta = ops.bn_backward_from_sums(dz, partial, c, co, dgamma=grads.dest(bn.weight),
+                                                  dbeta=grads.dest(bn.bias), sync=bn_sync(bn))
+    grads.put(bn.bias, dbeta)
+    grads.put(bn.weight, dgamma)
+    return dc
+
+
+# ------------------------------------------------------------------------------------------- classifier-dropout masks
+_mask_replay = None  # list of fp32 [B, F] classifier-dropout masks being consumed, or None
+_mask_record = None  # list collecting the masks drawn, or None
+
+
+@contextlib.contextmanager
+def dropout_replay(masks):
+    """Consume the given classifier-dropout masks (fp32 [B, F], already divided by 1 - p; call order) instead of drawing."""
+    global _mask_replay
+    prev, _mask_replay = _mask_replay, [m for m in masks]
+    try:
+        yield
+    finally:
+        _mask_replay = prev
+
+
+@contextlib.contextmanager
+def dropout_record():
+    """Collect the classifier-dropout masks drawn inside the context (fp32 [B, F], call order)."""
+    global _mask_record
+    prev, _mask_record = _mask_record, []
+    try:
+        yield _mask_record
+    finally:
+        _mask_record = prev
+
+
+def dropout_mask(p, B, F_, device, inplace):
+    """fp32 [B, F_] dropout mask (0 or 1 / (1 - p)) drawn with F.dropout on a tensor of ones, so that it consumes the
+    generator as the reference's nn.Dropout(p, inplace) does: the in-place path draws a Bernoulli noise tensor and
+    multiplies by it, the out-of-place one runs the fused native_dropout kernel.  Replayed / recorded under
+    dropout_replay / dropout_record."""
+    if _mask_replay is not None:
+        if not _mask_replay:
+            raise RuntimeError("dropout_replay: more classifier-dropout draws than recorded masks")
+        m = _mask_replay.pop(0).to(device=device, dtype=torch.float32).contiguous()
+        if tuple(m.shape) != (B, F_):
+            raise RuntimeError("dropout_replay: mask of the wrong shape")
+    else:
+        m = F.dropout(torch.ones(B, F_, dtype=torch.float32, device=device), p, True, inplace=inplace)
+    if _mask_record is not None:
+        _mask_record.append(m.detach().clone())
+    return m
 
 
 def image_input(model, x):

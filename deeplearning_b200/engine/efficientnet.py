@@ -19,72 +19,23 @@ bf16 [B, F] input of the shared head.
 Eval mode runs the same passes with running-statistics coefficients (bn_eval_coeffs) and records no statistics, masks or
 tape.  Drop-connect draws come from engine.droppath.sample_scale; the classifier-dropout mask is drawn with F.dropout on an
 fp32 [B, F] tensor of ones in place, which consumes the generator exactly as the reference's ``nn.Dropout(p, inplace=True)``
-on the pooled features does.  ``dropout_replay`` / ``dropout_record`` are the mask's test hooks, as droppath.replay / record are
-for the drop-connect multipliers.
+on the pooled features does.  ``dropout_replay`` / ``dropout_record`` (engine.common, shared with VGG) are the mask's test
+hooks, as droppath.replay / record are for the drop-connect multipliers.
 """
-import contextlib
 import sys
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from .. import ops
 from . import common, droppath
+from .common import dropout_record, dropout_replay  # noqa: F401  (the classifier-dropout test hooks)
 from .packing import weight_cache
-from .resnet import _bn_sync
 
 _STEM_LDK = 32     # patch-matrix width of the 3x3 x 3-channel stem (27 columns, padded to a multiple of 8)
 _MAX_CR = 256      # widest SE squeeze the excite kernels take
 
-_mask_replay = None  # list of fp32 [B, F] classifier-dropout masks being consumed, or None
-_mask_record = None  # list collecting the masks drawn, or None
-
-
-@contextlib.contextmanager
-def dropout_replay(masks):
-    """Consume the given classifier-dropout masks (fp32 [B, F], already divided by 1 - p) instead of drawing new ones."""
-    global _mask_replay
-    prev, _mask_replay = _mask_replay, [m for m in masks]
-    try:
-        yield
-    finally:
-        _mask_replay = prev
-
-
-@contextlib.contextmanager
-def dropout_record():
-    """Collect the classifier-dropout masks drawn inside the context (fp32 [B, F], call order)."""
-    global _mask_record
-    prev, _mask_record = _mask_record, []
-    try:
-        yield _mask_record
-    finally:
-        _mask_record = prev
-
-
-def _dropout_mask(p, B, F_, device):
-    if _mask_replay is not None:
-        if not _mask_replay:
-            raise RuntimeError("efficientnet.dropout_replay: more classifier-dropout draws than recorded masks")
-        m = _mask_replay.pop(0).to(device=device, dtype=torch.float32).contiguous()
-        if tuple(m.shape) != (B, F_):
-            raise RuntimeError("efficientnet.dropout_replay: mask of the wrong shape")
-    else:
-        # in place, as nn.Dropout(p, inplace=True) runs: that path draws a Bernoulli noise tensor (a different generator
-        # consumption from the fused out-of-place kernel) and multiplies by it, so ones * noise is the reference's mask
-        m = F.dropout(torch.ones(B, F_, dtype=torch.float32, device=device), p, True, inplace=True)
-    if _mask_record is not None:
-        _mask_record.append(m.detach().clone())
-    return m
-
-
 # --------------------------------------------------------------------------------------------------------- admission
-def _bn_ok(bn, C):
-    return (type(bn) in (nn.BatchNorm2d, nn.SyncBatchNorm) and bn.num_features == C and bn.affine
-            and bn.track_running_stats and bn.momentum is not None)
-
-
 def _conv_bn_act(name, seq, k, stride, cin, cout, groups, act):
     """Checks a ConvBNAction (conv, bn, act); returns (conv, bn)."""
     def no(why):
@@ -99,9 +50,9 @@ def _conv_bn_act(name, seq, k, stride, cin, cout, groups, act):
         no(f"expected a {k}x{k} convolution with stride {stride} and padding {k // 2}")
     if (cin is not None and conv.in_channels != cin) or conv.out_channels != cout or conv.groups != groups:
         no("channel counts do not follow the block structure")
-    if not _bn_ok(bn, cout):
+    if not common.bn_ok(bn, cout):
         no("expected an affine BatchNorm2d that tracks running statistics")
-    if _bn_sync(bn) is not None:
+    if common.bn_sync(bn) is not None:
         no("SyncBatchNorm in a multi-rank job is not implemented for EfficientNet")
     if type(a) is not act:
         no(f"the GPU engine runs this layer with {act.__name__}")
@@ -249,17 +200,6 @@ class _PackSpec:
 _pack_spec = _PackSpec()
 
 
-def _coeffs(bn, stats, rows, train):
-    if train:
-        return ops.bn_finalize(stats, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
-                               bn.num_batches_tracked)
-    return ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
-
-
-def _rows(t):
-    return t.numel() // t.shape[-1]
-
-
 # ---------------------------------------------------------------------------------------------------------- forward
 def forward(model, x, train, want_tape):
     """x: fp32 NCHW (or decoded uint8 NHWC) CUDA batch.  Returns (logits fp32 [B, num_classes], tape or None)."""
@@ -273,35 +213,35 @@ def forward(model, x, train, want_tape):
     a, Ho, Wo = ops.im2col_nchw(x, 3, 3, 2, 1, ldk=_STEM_LDK)
     patches = a.view(B, Ho, Wo, _STEM_LDK)
     c_s, st = ops.conv2d_fwd(patches, pack.get(stem_conv.weight, 0), 1, 1, want_stats=train)
-    co_s = _coeffs(stem_bn, st, _rows(c_s), train)
+    co_s = common.bn_coeffs(stem_bn, st, common.rows(c_s), train)
     if tape is not None:
         tape["stem"] = (patches, c_s, co_s)
     h = None
     for i, b in enumerate(blocks):
         if b.exp is not None:
             c_e, st = ops.conv2d_fwd(h, pack.get(b.exp.weight, 0), 1, 1, want_stats=train)
-            co_e = _coeffs(b.exp_bn, st, _rows(c_e), train)
+            co_e = common.bn_coeffs(b.exp_bn, st, common.rows(c_e), train)
             dw_in, dw_co = c_e, co_e
         else:
             c_e = co_e = None
             dw_in, dw_co = (c_s, co_s) if i == 0 else (h, None)
         d, st = ops.dw_fwd(dw_in, b.dw.weight, b.k, b.s, co=dw_co, want_stats=train)
-        co_d = _coeffs(b.dw_bn, st, _rows(d), train)
+        co_d = common.bn_coeffs(b.dw_bn, st, common.rows(d), train)
         pool, _ = ops.silu_bn_squeeze(d, co_d)
         hpre, gate = ops.excite_fwd(pool, b.fc1.weight, b.fc1.bias, b.fc2.weight, b.fc2.bias)
         a = ops.gate_apply(d, co_d, gate)
         c_p, st = ops.conv2d_fwd(a, pack.get(b.proj.weight, 0), 1, 1, want_stats=train)
-        co_p = _coeffs(b.proj_bn, st, _rows(c_p), train)
+        co_p = common.bn_coeffs(b.proj_bn, st, common.rows(c_p), train)
         rs = droppath.sample_scale(b.drop if train else 0.0, B, 4, x.device)
         y = ops.tail_apply(c_p, co_p, rs, residual=h if b.res else None)
         if tape is not None:
             tape["blocks"].append((b, h, dw_in, dw_co, c_e, co_e, d, co_d, pool, hpre, gate, a, c_p, co_p, rs))
         h = y
     c_t, st = ops.conv2d_fwd(h, pack.get(top_conv.weight, 0), 1, 1, want_stats=train)
-    co_t = _coeffs(top_bn, st, _rows(c_t), train)
+    co_t = common.bn_coeffs(top_bn, st, common.rows(c_t), train)
     Fc = c_t.shape[-1]
     if train and p > 0:
-        mask = _dropout_mask(p, B, Fc, x.device)
+        mask = common.dropout_mask(p, B, Fc, x.device, inplace=True)
     else:
         mask = torch.ones(B, Fc, dtype=torch.float32, device=x.device)
     _, feat = ops.silu_bn_squeeze(c_t, co_t, mask=mask)
@@ -319,32 +259,21 @@ def backward(model, tape, dlogits, sink=None):
     grads = common.Grads(sink)
     pack = tape["pack"]
 
-    def dest(p):
-        d = grads.dest(p)
-        return None if d is None else d.view(p.shape)
-
-    def bn_backward(bn, dz, partial, c, co):
-        dg, db, m = ops.bn_bwd_finalize(partial, _rows(c), co, grads.dest(bn.weight), grads.dest(bn.bias))
-        dc = ops.bn_bwd_apply_dz(dz, c, co, m)
-        grads.put(bn.bias, db)
-        grads.put(bn.weight, dg)
-        return dc
-
     h, c_t, co_t, mask, feat = tape["top"]
     dfeat = common.head_backward(grads, pack, head, feat, dlogits)
     dpool = ops.cast_f32(dfeat).mul_(mask)      # [B, F]: the classifier dropout's backward
     dz, part = ops.silu_bn_bwd_reduce(c_t, co_t, dpool)
-    dc = bn_backward(top_bn, dz, part, c_t, co_t)
-    grads.put(top_conv.weight, ops.conv2d_wgrad(dc, h, 1, 1, out=dest(top_conv.weight)))
+    dc = common.bn_backward_from_sums(grads, top_bn, dz, part, c_t, co_t)
+    grads.put(top_conv.weight, ops.conv2d_wgrad(dc, h, 1, 1, out=grads.dest(top_conv.weight)))
     g = ops.conv2d_dgrad(dc, pack.get(top_conv.weight, 1), tuple(h.shape[1:3]), 1, 1)
 
     for b, x, dw_in, dw_co, c_e, co_e, d, co_d, pool, hpre, gate, a, c_p, co_p, rs in reversed(tape["blocks"]):
         dz, part = ops.tail_bwd_reduce(g, c_p, rs)
-        dc = bn_backward(b.proj_bn, dz, part, c_p, co_p)
-        grads.put(b.proj.weight, ops.conv2d_wgrad(dc, a, 1, 1, out=dest(b.proj.weight)))
+        dc = common.bn_backward_from_sums(grads, b.proj_bn, dz, part, c_p, co_p)
+        grads.put(b.proj.weight, ops.conv2d_wgrad(dc, a, 1, 1, out=grads.dest(b.proj.weight)))
         da = ops.conv2d_dgrad(dc, pack.get(b.proj.weight, 1), tuple(a.shape[1:3]), 1, 1)
         s = ops.gate_reduce(da, d, co_d)
-        d1, d2 = dest(b.fc1.weight), dest(b.fc2.weight)
+        d1, d2 = grads.dest(b.fc1.weight), grads.dest(b.fc2.weight)
         dpool, dw1, db1, dw2, db2 = ops.excite_bwd(
             s, pool, hpre, gate, b.fc1.weight, b.fc2.weight,
             dw1=None if d1 is None else d1.view(d1.shape[0], -1), db1=grads.dest(b.fc1.bias),
@@ -354,8 +283,8 @@ def backward(model, tape, dlogits, sink=None):
         grads.put(b.fc1.bias, db1)
         grads.put(b.fc1.weight, dw1)
         dz, part = ops.silu_bn_bwd_reduce(d, co_d, dpool, da=da, gate=gate)
-        dd = bn_backward(b.dw_bn, dz, part, d, co_d)
-        grads.put(b.dw.weight, ops.dw_wgrad(dd, dw_in, b.k, b.s, co=dw_co, out=dest(b.dw.weight)))
+        dd = common.bn_backward_from_sums(grads, b.dw_bn, dz, part, d, co_d)
+        grads.put(b.dw.weight, ops.dw_wgrad(dd, dw_in, b.k, b.s, co=dw_co, out=grads.dest(b.dw.weight)))
         if dw_co is None:
             # the depthwise read the previous block's output as is
             g, _ = ops.dw_dgrad(dd, b.dw.weight, dw_in, b.k, b.s, residual=g if b.res else None)
@@ -364,13 +293,13 @@ def backward(model, tape, dlogits, sink=None):
         if b.exp is None:
             # block 1a: its input is silu(bn(stem conv)), normalised on load
             patches, c_s, co_s = tape["stem"]
-            dc = bn_backward(stem_bn, dz, part, c_s, co_s)
+            dc = common.bn_backward_from_sums(grads, stem_bn, dz, part, c_s, co_s)
             C0 = c_s.shape[-1]
             gw = ops.conv2d_wgrad(dc, patches, 1, 1).view(C0, _STEM_LDK)
-            grads.put(stem_conv.weight, ops.stem_wgrad_relayout(gw, C0, 3, 9, out=dest(stem_conv.weight)))
+            grads.put(stem_conv.weight, ops.stem_wgrad_relayout(gw, C0, 3, 9, out=grads.dest(stem_conv.weight)))
             break
-        dc = bn_backward(b.exp_bn, dz, part, c_e, co_e)
-        grads.put(b.exp.weight, ops.conv2d_wgrad(dc, x, 1, 1, out=dest(b.exp.weight)))
+        dc = common.bn_backward_from_sums(grads, b.exp_bn, dz, part, c_e, co_e)
+        grads.put(b.exp.weight, ops.conv2d_wgrad(dc, x, 1, 1, out=grads.dest(b.exp.weight)))
         g = ops.conv2d_dgrad(dc, pack.get(b.exp.weight, 1), tuple(x.shape[1:3]), 1, 1, residual=g if b.res else None)
     return grads
 

@@ -28,7 +28,6 @@ import torch.nn as nn
 from .. import ops
 from . import common
 from .packing import weight_cache
-from .resnet import _bn_sync
 
 _STEM_LDK = 32     # patch-matrix width of the 3x3 x 3-channel stem (27 columns, padded to a multiple of 8)
 _CENTRE = 12       # column of tap (1, 1), channel 0 in that matrix: what the 1x1/2 stem convolution reads
@@ -52,15 +51,10 @@ def _conv_ok(conv, k, stride, pad, bias):
             and (conv.bias is not None) == bias and conv.padding_mode == "zeros")
 
 
-def _bn_ok(bn, C):
-    return (type(bn) in (nn.BatchNorm2d, nn.SyncBatchNorm) and bn.num_features == C and bn.affine
-            and bn.track_running_stats and bn.momentum is not None)
-
-
 def _conv_bn_ok(branch, k, stride, pad, cin, cout):
     return (isinstance(branch, nn.Sequential) and list(branch._modules) == ["conv", "bn"]
             and _conv_ok(branch.conv, k, stride, pad, False) and branch.conv.in_channels == cin
-            and branch.conv.out_channels == cout and _bn_ok(branch.bn, cout))
+            and branch.conv.out_channels == cout and common.bn_ok(branch.bn, cout))
 
 
 def _check_block(name, blk, stem):
@@ -90,10 +84,10 @@ def _check_block(name, blk, stem):
     ident = getattr(blk, "rbr_identity", None)
     if not (_conv_bn_ok(blk.rbr_dense, 3, s, 1, cin, cout) and _conv_bn_ok(getattr(blk, "rbr_1x1", None), 1, s, 0, cin, cout)):
         no("branches must be conv_bn(3x3, pad 1) and conv_bn(1x1, pad 0) at the block's stride")
-    if ident is not None and not (cin == cout and s == 1 and _bn_ok(ident, cin)):
+    if ident is not None and not (cin == cout and s == 1 and common.bn_ok(ident, cin)):
         no("rbr_identity must be a BatchNorm2d of a stride-1 block with in_channels == out_channels")
     for bn in (blk.rbr_dense.bn, blk.rbr_1x1.bn) + ((ident,) if ident is not None else ()):
-        if _bn_sync(bn) is not None:
+        if common.bn_sync(bn) is not None:
             no("SyncBatchNorm in a multi-rank job is not implemented for RepVGG")
     return s
 
@@ -146,11 +140,6 @@ class _PackSpec:
 _pack_spec = _PackSpec()
 
 
-def _finalize(bn, stats, rows):
-    return ops.bn_finalize(stats, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
-                           bn.num_batches_tracked)
-
-
 def forward(model, x, train, want_tape):
     """x: fp32 NCHW (or decoded uint8 NHWC) CUDA batch.  Returns (logits fp32 [B, num_classes], tape or None)."""
     strides = check_model(model)
@@ -195,8 +184,8 @@ def forward(model, x, train, want_tape):
             c3, st3 = ops.conv2d_fwd(h, pack.get(blk.rbr_dense.conv.weight, 0), 3, s, want_stats=True)
             c1, st1 = ops.conv2d_fwd(h, pack.get(blk.rbr_1x1.conv.weight, 0), 1, s, want_stats=True)
         rows = c3.numel() // c3.shape[-1]
-        co3, co1 = _finalize(bn3, st3, rows), _finalize(bn1, st1, rows)
-        co_id = _finalize(ident, h_stats, rows) if ident is not None else None
+        co3, co1 = common.bn_coeffs(bn3, st3, rows, True), common.bn_coeffs(bn1, st1, rows, True)
+        co_id = common.bn_coeffs(ident, h_stats, rows, True) if ident is not None else None
         nxt = blocks[bi + 1][1] if bi + 1 < len(blocks) else None
         want_stats = nxt is not None and not _is_deploy(nxt) and nxt.rbr_identity is not None
         y, h_stats = ops.repvgg_apply(c3, c1, co3, co1, x=h if ident is not None else None, co_id=co_id, want_stats=want_stats)
@@ -217,10 +206,6 @@ def backward(model, tape, dlogits, sink=None):
     pack = tape["pack"]
     pooled, hw = tape["head"]
     g = ops.avgpool_bwd(common.head_backward(grads, pack, model.linear, pooled, dlogits), hw)
-
-    def dest(p):
-        d = grads.dest(p)
-        return None if d is None else d.view(p.shape)
 
     for blk, s, x, c, c3, c1, co3, co1, co_id, y in reversed(tape["blocks"]):
         stem = c is not None
@@ -249,17 +234,17 @@ def backward(model, tape, dlogits, sink=None):
             # one wgrad over [dc3 | dc1] and the patch matrix: rows 0..C-1 are the 3x3 gradient in patch layout, columns
             # 12..14 of rows C..2C-1 the 1x1 gradient
             gw = ops.conv2d_wgrad(dc, x, 1, 1).view(2 * C, _STEM_LDK)
-            d1 = dest(w1)
+            d1 = grads.dest(w1)
             g1 = gw[C:, _CENTRE:_CENTRE + 3].reshape(w1.shape)
             grads.put(w1, d1.copy_(g1) if d1 is not None else g1)
             grads.put(bn3.bias, db3)
             grads.put(bn3.weight, dg3)
-            grads.put(w3, ops.stem_wgrad_relayout(gw[:C], C, 3, 9, out=dest(w3)))
+            grads.put(w3, ops.stem_wgrad_relayout(gw[:C], C, 3, 9, out=grads.dest(w3)))
             break
-        grads.put(w1, ops.conv2d_wgrad(dc1, x, 1, s, out=dest(w1)))
+        grads.put(w1, ops.conv2d_wgrad(dc1, x, 1, s, out=grads.dest(w1)))
         grads.put(bn3.bias, db3)
         grads.put(bn3.weight, dg3)
-        grads.put(w3, ops.conv2d_wgrad(dc3, x, 3, s, out=dest(w3)))
+        grads.put(w3, ops.conv2d_wgrad(dc3, x, 3, s, out=grads.dest(w3)))
         if ident is not None:
             grads.put(ident.bias, dbi)
             grads.put(ident.weight, dgi)

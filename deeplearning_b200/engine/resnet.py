@@ -66,30 +66,6 @@ def _check_bn(bn, name):
                                   f"statistics (got {bn})")
 
 
-def _bn_sync(bn):
-    """(process_group, world_size) when ``bn`` is a SyncBatchNorm in a multi-rank job (the recipe converts every BatchNorm
-    with ``nn.SyncBatchNorm.convert_sync_batchnorm``: others/train_with_DDP/train.py:190), else None.  Statistics and the
-    two backward sums are then all-reduced per layer (ops._sync_sums); such layers stay on the plain conv -> BN schedule."""
-    if not isinstance(bn, nn.SyncBatchNorm) or not bn.training:
-        return None
-    import torch.distributed as dist
-
-    if not (dist.is_available() and dist.is_initialized()):
-        return None
-    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
-    world = dist.get_world_size(group)
-    return (group, world) if world > 1 else None
-
-
-def _bn_coeffs(bn, stats, rows, train):
-    """BatchNorm coefficients: from the batch statistics (``rows`` values per channel, running statistics updated) in
-    train mode, from the running statistics in eval mode."""
-    if train:
-        return ops.bn_finalize(stats, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
-                               bn.num_batches_tracked, sync=_bn_sync(bn))
-    return ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
-
-
 class _PackSpec:
     """Which bf16 operands a ResNet needs: forward [O][taps*I] and dgrad [I][taps*O] copies of every conv / fc weight."""
 
@@ -205,7 +181,7 @@ def _conv_bn(pack, tape, x, conv, bn, train, relu, residual=None, name=""):
         co = ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
         return ops.conv2d_bn_act(x, wp, co, k, s, relu=relu, residual=residual, groups=g)
     c, st = ops.conv2d_fwd(x, wp, k, s, want_stats=train, groups=g)
-    co = _bn_coeffs(bn, st, c.numel() // c.shape[-1], train)
+    co = common.bn_coeffs(bn, st, c.numel() // c.shape[-1], train)
     y = ops.bn_apply(c, co, relu=relu, residual=residual)
     if tape is not None:
         tape.append(_Unit(conv, bn, x, c, co, y, relu, residual is not None))
@@ -235,11 +211,11 @@ def _conv_bn_se(pack, tape, x, conv, bn, se, train, identity, name=""):
     _check_conv(conv, name)
     _check_bn(bn, name)
     _check_se(se, conv.out_channels, name)
-    if train and _bn_sync(bn) is not None:
+    if train and common.bn_sync(bn) is not None:
         raise NotImplementedError(f"{name}: SyncBatchNorm in front of a squeeze-and-excitation gate is not implemented")
     wp = pack.get(conv.weight, _pack_modes(conv)[0])
     c, st = ops.conv2d_fwd(x, wp, conv.kernel_size[0], conv.stride[0], want_stats=train, groups=conv.groups)
-    co = _bn_coeffs(bn, st, c.numel() // c.shape[-1], train)
+    co = common.bn_coeffs(bn, st, c.numel() // c.shape[-1], train)
     csum, pool = ops.se_squeeze(c, co)
     h, gate = ops.se_excite(pool, se.fc[0].weight, se.fc[2].weight)
     y = ops.se_apply(c, co, gate, identity)
@@ -289,7 +265,7 @@ def forward(model, x, train, want_tape):
     a = ops.stem_s2d_u8(x, *getattr(model, "input_norm", (ops.IMAGENET_MEAN, ops.IMAGENET_STD))) if u8 else ops.stem_s2d(x)
     Ho, Wo = a.shape[1] - 3, a.shape[2] - 3
     c1, st = ops.stem_s2d_conv_fwd(a, pack.get(conv1.weight, 2), want_stats=train)
-    co1 = _bn_coeffs(bn1, st, B * Ho * Wo, train)
+    co1 = common.bn_coeffs(bn1, st, B * Ho * Wo, train)
     h, idx = ops.bn_relu_maxpool_fwd(c1, co1)
     if want_tape:
         tape["stem"] = (a, c1, co1, idx, (Ho, Wo))
@@ -334,7 +310,7 @@ def _unit_backward(u, g, grads, want_dz=False):
     """Backward of BN(+ReLU) of unit u for upstream gradient g; returns (dc, dz) and records BN param grads."""
     dc, dgamma, dbeta, dz = ops.bn_backward(g, u.c, u.co, relu=u.relu, y_out=u.y if (u.relu and u.has_res) else None,
                                             want_dz=want_dz, dgamma=grads.dest(u.bn.weight), dbeta=grads.dest(u.bn.bias),
-                                            sync=_bn_sync(u.bn))
+                                            sync=common.bn_sync(u.bn))
     grads.put(u.bn.weight, dgamma)
     grads.put(u.bn.bias, dbeta)
     return dc, dz
@@ -359,14 +335,6 @@ def _fused_reduce_ok(u):
     """Can the dgrad GEMM that produces the gradient of unit u's output also do the reduce half of u's BN backward?
     (relu(bn(c)) without a residual, 64-channel multiples)"""
     return u.relu and not u.has_res and u.c.shape[-1] % 64 == 0
-
-
-def _unit_backward_from_sums(u, dz, sums, grads):
-    dc, dgamma, dbeta = ops.bn_backward_from_sums(dz, sums, u.c, u.co, dgamma=grads.dest(u.bn.weight), dbeta=grads.dest(u.bn.bias),
-                                                  sync=_bn_sync(u.bn))
-    grads.put(u.bn.weight, dgamma)
-    grads.put(u.bn.bias, dbeta)
-    return dc
 
 
 def _algebra_backward(u, dz, dz_stats, pack, grads):
@@ -409,7 +377,7 @@ def backward(model, tape, dlogits, sink=None):
             u2 = units[-2]
             if _fused_reduce_ok(u2):
                 dz2, sums2 = ops.gemm_dual(dz, y2, wcat, wbias, bn_mask=(u2.c, u2.co))
-                dc = _unit_backward_from_sums(u2, dz2, sums2, grads)
+                dc = common.bn_backward_from_sums(grads, u2.bn, dz2, sums2, u2.c, u2.co)
             else:
                 g_prev = ops.gemm_dual(dz, y2, wcat, wbias)
                 dc, _ = _unit_backward(u2, g_prev, grads)
@@ -437,7 +405,7 @@ def backward(model, tape, dlogits, sink=None):
             in_hw = tuple(u.x.shape[1:3])
             if j > 0 and s == 1 and _fused_reduce_ok(units[j - 1]):
                 dzj, sumsj = ops.conv2d_dgrad(dc, wd, in_hw, k, s, bn_mask=(units[j - 1].c, units[j - 1].co), groups=gr)
-                dc = _unit_backward_from_sums(units[j - 1], dzj, sumsj, grads)
+                dc = common.bn_backward_from_sums(grads, units[j - 1].bn, dzj, sumsj, units[j - 1].c, units[j - 1].co)
             elif j > 0:
                 g_prev = ops.conv2d_dgrad(dc, wd, in_hw, k, s, groups=gr)
                 dc, _ = _unit_backward(units[j - 1], g_prev, grads)
@@ -464,7 +432,7 @@ def backward(model, tape, dlogits, sink=None):
 
     a, c1, co1, idx, (Ho, Wo) = tape["stem"]
     g_act = ops.maxpool_bwd(g, idx, (Ho, Wo))
-    dc, dgamma, dbeta, _ = ops.bn_backward(g_act, c1, co1, relu=True, sync=_bn_sync(model.bn1), dgamma=grads.dest(model.bn1.weight),
+    dc, dgamma, dbeta, _ = ops.bn_backward(g_act, c1, co1, relu=True, sync=common.bn_sync(model.bn1), dgamma=grads.dest(model.bn1.weight),
                                            dbeta=grads.dest(model.bn1.bias))
     grads.put(model.bn1.weight, dgamma)
     grads.put(model.bn1.bias, dbeta)

@@ -33,7 +33,6 @@ import torch.nn as nn
 from .. import ops
 from . import common
 from .packing import weight_cache
-from .resnet import _bn_sync
 
 _STEM_LDK = 32     # patch-matrix width of the 3x3 x 3-channel stem (27 columns, padded to a multiple of 8)
 
@@ -43,16 +42,11 @@ def _pad8(n):
 
 
 # --------------------------------------------------------------------------------------------------------- admission
-def _bn_ok(bn, C):
-    return (type(bn) in (nn.BatchNorm2d, nn.SyncBatchNorm) and bn.num_features == C and bn.affine
-            and bn.track_running_stats and bn.momentum is not None)
-
-
 def _check_bn(name, bn, C):
-    if not _bn_ok(bn, C):
+    if not common.bn_ok(bn, C):
         raise NotImplementedError(f"{name}: expected an affine BatchNorm2d over {C} channels that tracks running statistics "
                                   f"(got {bn})")
-    if _bn_sync(bn) is not None:
+    if common.bn_sync(bn) is not None:
         raise NotImplementedError(f"{name}: SyncBatchNorm in a multi-rank job is not implemented for ShuffleNet")
 
 
@@ -300,17 +294,6 @@ def _dw_weight(k):
     return torch.cat([w, w.new_zeros(k.bp - k.b, 1, 3, 3)]).contiguous()
 
 
-def _coeffs(bn, stats, rows, train):
-    if train:
-        return ops.bn_finalize(stats, rows, bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean, bn.running_var,
-                               bn.num_batches_tracked)
-    return ops.bn_eval_coeffs(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
-
-
-def _rows(t):
-    return t.numel() // t.shape[-1]
-
-
 # ---------------------------------------------------------------------------------------------------------- forward
 def forward(model, x, train, want_tape):
     """x: fp32 NCHW (or decoded uint8 NHWC) CUDA batch.  Returns (logits fp32 [B, num_classes], tape or None)."""
@@ -325,7 +308,7 @@ def forward(model, x, train, want_tape):
     a, Ho, Wo = ops.im2col_nchw(x, 3, 3, 2, 1, ldk=_STEM_LDK)
     patches = a.view(B, Ho, Wo, _STEM_LDK)
     c_s, st = ops.conv2d_fwd(patches, pack.get(stem_conv.weight, 0), 1, 1, want_stats=train)
-    co_s = _coeffs(stem_bn, st, _rows(c_s), train)
+    co_s = common.bn_coeffs(stem_bn, st, common.rows(c_s), train)
     h, idx = ops.bn_relu_maxpool_fwd(c_s, co_s)
     if tape is not None:
         tape["stem"] = (patches, c_s, co_s, idx)
@@ -333,13 +316,13 @@ def forward(model, x, train, want_tape):
         w1, _ = plan.conv1[i].operands()
         w3, _ = plan.conv3[i].operands()
         c1, st = ops.conv2d_fwd(h, w1, 1, 1, want_stats=train)
-        co1 = plan.bn1[i].coeffs(st, _rows(c1), train)
+        co1 = plan.bn1[i].coeffs(st, common.rows(c1), train)
         wd = _dw_weight(k)
         d, st = ops.dw_relu_fwd(c1, wd, k.s, co1, want_stats=train)
-        co2 = plan.bn2[i].coeffs(st, _rows(d), train)
+        co2 = plan.bn2[i].coeffs(st, common.rows(d), train)
         a = ops.bn_apply(d, co2, relu=False)
         c3, st = ops.conv2d_fwd(a, w3, 1, 1, want_stats=train)
-        co3 = _coeffs(k.bn3, st, _rows(c3), train)
+        co3 = common.bn_coeffs(k.bn3, st, common.rows(c3), train)
         y = ops.bn_apply(c3, co3, relu=True, residual=h) if k.s == 1 else ops.shuffle_tail_s2_fwd(h, c3, co3)
         if tape is not None:
             tape["blocks"].append((h, c1, co1, wd, d, co2, a, c3, co3, y))
@@ -359,20 +342,8 @@ def backward(model, tape, dlogits, sink=None):
     grads = common.Grads(sink)
     pack, plan = tape["pack"], tape["plan"]
 
-    def dest(p):
-        d = grads.dest(p)
-        return None if d is None else d.view(p.shape)
-
-    def bn_backward(bn, dz, partial, c, co):
-        dg, db, m = ops.bn_bwd_finalize(partial, _rows(c), co, grads.dest(bn.weight), grads.dest(bn.bias))
-        dc = ops.bn_bwd_apply_dz(dz, c, co, m)
-        grads.put(bn.bias, db)
-        grads.put(bn.weight, dg)
-        return dc
-
     def padded_bn_backward(pbn, dz, partial, c, co):
-        dg, db, m = ops.bn_bwd_finalize(partial, _rows(c), co)
-        dc = ops.bn_bwd_apply_dz(dz, c, co, m)
+        dc, dg, db = ops.bn_backward_from_sums(dz, partial, c, co)
         grads.put(pbn.bn.bias, pbn.scatter(db, grads.dest(pbn.bn.bias)))
         grads.put(pbn.bn.weight, pbn.scatter(dg, grads.dest(pbn.bn.weight)))
         return dc
@@ -387,28 +358,28 @@ def backward(model, tape, dlogits, sink=None):
             shortcut = dz3
         else:
             dz3, part, shortcut = ops.shuffle_relu_bwd(g, c3, y=y, in_hw=tuple(x.shape[1:3]))
-        dc3 = bn_backward(k.bn3, dz3, part, c3, co3)
+        dc3 = common.bn_backward_from_sums(grads, k.bn3, dz3, part, c3, co3)
         gc3 = plan.conv3[i]
-        grads.put(k.conv3.weight, gc3.weight_grad(ops.conv2d_wgrad(dc3, a, 1, 1), dest(k.conv3.weight)))
+        grads.put(k.conv3.weight, gc3.weight_grad(ops.conv2d_wgrad(dc3, a, 1, 1), grads.dest(k.conv3.weight)))
         da = ops.conv2d_dgrad(dc3, gc3.operands()[1], tuple(a.shape[1:3]), 1, 1)
         _, part = ops.tail_bwd_reduce(da, d)
         dd = padded_bn_backward(plan.bn2[i], da, part, d, co2)
         gw = ops.dw_relu_wgrad(dd, c1, k.s, co1)
-        gwd = dest(k.dw.weight)
+        gwd = grads.dest(k.dw.weight)
         gw = gw[:k.b] if gwd is None else gwd.copy_(gw[:k.b])
         grads.put(k.dw.weight, gw)
         dz1, part = ops.dw_relu_dgrad(dd, wd, c1, k.s, co1)
         dc1 = padded_bn_backward(plan.bn1[i], dz1, part, c1, co1)
         gc1 = plan.conv1[i]
-        grads.put(k.conv1.weight, gc1.weight_grad(ops.conv2d_wgrad(dc1, x, 1, 1), dest(k.conv1.weight)))
+        grads.put(k.conv1.weight, gc1.weight_grad(ops.conv2d_wgrad(dc1, x, 1, 1), grads.dest(k.conv1.weight)))
         g = ops.conv2d_dgrad(dc1, gc1.operands()[1], tuple(x.shape[1:3]), 1, 1, residual=shortcut)
     patches, c_s, co_s, idx = tape["stem"]
     g_act = ops.maxpool_bwd(g, idx, tuple(c_s.shape[1:3]))
     dz, part, _ = ops.shuffle_relu_bwd(g_act, c_s, co=co_s)
-    dc = bn_backward(stem_bn, dz, part, c_s, co_s)
+    dc = common.bn_backward_from_sums(grads, stem_bn, dz, part, c_s, co_s)
     C0 = c_s.shape[-1]
     gw = ops.conv2d_wgrad(dc, patches, 1, 1).view(C0, _STEM_LDK)
-    grads.put(stem_conv.weight, ops.stem_wgrad_relayout(gw, C0, 3, 9, out=dest(stem_conv.weight)))
+    grads.put(stem_conv.weight, ops.stem_wgrad_relayout(gw, C0, 3, 9, out=grads.dest(stem_conv.weight)))
     return grads
 
 

@@ -17,75 +17,27 @@ The first convolution (3 input channels) is one 1x1 GEMM over the [B*H*W][32] im
 as it is.  The classifier's Linear layers are GEMMs with bias + ReLU in the epilogue; the dropout after each multiplies by a
 mask drawn with F.dropout on an fp32 tensor of ones, which consumes the generator as the reference's ``nn.Dropout()`` on
 the fp32 [B, 4096] activation does; its backward needs only the stored h = dropout(relu(pre)): dpre = h > 0 ? dh / (1 - p) : 0.
-``dropout_replay`` / ``dropout_record`` are the masks' test hooks.
+``dropout_replay`` / ``dropout_record`` (engine.common, shared with EfficientNet) are the masks' test hooks.
 
 Eval mode: plain layers run the same GEMMs and pools (without arg-max bytes); _bn layers run folded GEMMs
 relu(conv * scale + shift') with shift' = beta - (running_mean - b) * scale, dropout is the identity and no tape is recorded.
 """
-import contextlib
 import sys
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from .. import ops
 from . import common
+from .common import dropout_record, dropout_replay  # noqa: F401  (the classifier-dropout test hooks)
 from .packing import weight_cache
-from .resnet import _bn_sync
 
 _STEM_LDK = 32     # patch-matrix width of the 3x3 x 3-channel first convolution (27 columns, padded to a multiple of 8)
-
-_mask_replay = None  # list of fp32 [B, F] classifier-dropout masks being consumed, or None
-_mask_record = None  # list collecting the masks drawn, or None
-
-
-@contextlib.contextmanager
-def dropout_replay(masks):
-    """Consume the given classifier-dropout masks (fp32 [B, F], already divided by 1 - p; call order) instead of drawing."""
-    global _mask_replay
-    prev, _mask_replay = _mask_replay, [m for m in masks]
-    try:
-        yield
-    finally:
-        _mask_replay = prev
-
-
-@contextlib.contextmanager
-def dropout_record():
-    """Collect the classifier-dropout masks drawn inside the context (fp32 [B, F], call order)."""
-    global _mask_record
-    prev, _mask_record = _mask_record, []
-    try:
-        yield _mask_record
-    finally:
-        _mask_record = prev
-
-
-def _dropout_mask(p, B, F_, device):
-    if _mask_replay is not None:
-        if not _mask_replay:
-            raise RuntimeError("vgg.dropout_replay: more classifier-dropout draws than recorded masks")
-        m = _mask_replay.pop(0).to(device=device, dtype=torch.float32).contiguous()
-        if tuple(m.shape) != (B, F_):
-            raise RuntimeError("vgg.dropout_replay: mask of the wrong shape")
-    else:
-        # out of place, as nn.Dropout() runs on the classifier's fp32 activations (the fused native_dropout kernel)
-        m = F.dropout(torch.ones(B, F_, dtype=torch.float32, device=device), p, True)
-    if _mask_record is not None:
-        _mask_record.append(m.detach().clone())
-    return m
-
 
 # --------------------------------------------------------------------------------------------------------- admission
 class _Layer:
     """One convolution of ``features`` as the schedule runs it."""
     __slots__ = ("name", "conv", "bn", "pool")
-
-
-def _bn_ok(bn, C):
-    return (type(bn) in (nn.BatchNorm2d, nn.SyncBatchNorm) and bn.num_features == C and bn.affine
-            and bn.track_running_stats and bn.momentum is not None)
 
 
 def _check_features(feats):
@@ -116,10 +68,10 @@ def _check_features(feats):
         i += 1
         if i < len(mods) and type(mods[i][1]) in (nn.BatchNorm2d, nn.SyncBatchNorm):
             bn_name, bn = mods[i]
-            if not _bn_ok(bn, conv.out_channels):
+            if not common.bn_ok(bn, conv.out_channels):
                 raise NotImplementedError(f"features.{bn_name}: expected an affine BatchNorm2d that tracks running "
                                           f"statistics (got {bn})")
-            if _bn_sync(bn) is not None:
+            if common.bn_sync(bn) is not None:
                 raise NotImplementedError(f"features.{bn_name}: SyncBatchNorm in a multi-rank job is not implemented for VGG")
             lay.bn = bn
             i += 1
@@ -249,8 +201,7 @@ def forward(model, x, train, want_tape):
             c = co = None
         elif train:
             c, st = ops.conv2d_fwd(h, w, k, 1, want_stats=True, bias=conv.bias.detach())
-            co = ops.bn_finalize(st, c.numel() // c.shape[-1], bn.weight, bn.bias, bn.eps, bn.momentum, bn.running_mean,
-                                 bn.running_var, bn.num_batches_tracked)
+            co = common.bn_coeffs(bn, st, c.numel() // c.shape[-1], True)
             y = None if l.pool else ops.bn_apply(c, co, relu=True)
         else:
             # relu(bn(conv + b)) = relu(conv * scale + beta - (running_mean - b) * scale)
@@ -269,10 +220,10 @@ def forward(model, x, train, want_tape):
     feat = ops.vgg_avgpool7_fwd(h)
     d0 = _linear(pack, fc0, feat, True)
     if train and p0 > 0:
-        d0 = ops.vgg_dropout_fwd(d0, _dropout_mask(p0, B, d0.shape[1], x.device))
+        d0 = ops.vgg_dropout_fwd(d0, common.dropout_mask(p0, B, d0.shape[1], x.device, inplace=False))
     d1 = _linear(pack, fc3, d0, True)
     if train and p1 > 0:
-        d1 = ops.vgg_dropout_fwd(d1, _dropout_mask(p1, B, d1.shape[1], x.device))
+        d1 = ops.vgg_dropout_fwd(d1, common.dropout_mask(p1, B, d1.shape[1], x.device, inplace=False))
     logits = common.head_forward(pack, fc6, d1)
     if tape is not None:
         tape["head"] = (h.shape, feat, d0, d1)
@@ -286,10 +237,6 @@ def backward(model, tape, dlogits, sink=None):
     _, (fc0, fc3, fc6), (p0, p1) = check_model(model)
     grads = common.Grads(sink)
     pack = tape["pack"]
-
-    def dest(p):
-        d = grads.dest(p)
-        return None if d is None else d.view(p.shape)
 
     h_shape, feat, d0, d1 = tape["head"]
     g = ops.vgg_dropout_bwd(common.head_backward(grads, pack, fc6, d1, dlogits), d1, p1)
@@ -311,10 +258,7 @@ def backward(model, tape, dlogits, sink=None):
             g = ops.vgg_pool_bwd(g, idx, hw, y=out) if bn is None else ops.vgg_pool_bwd(g, idx, hw, c=c, co=co)
         if bn is not None:
             dz, part = g
-            dg, db, m = ops.bn_bwd_finalize(part, c.numel() // c.shape[-1], co, grads.dest(bn.weight), grads.dest(bn.bias))
-            dc = ops.bn_bwd_apply_dz(dz, c, co, m)
-            grads.put(bn.bias, db)
-            grads.put(bn.weight, dg)
+            dc = common.bn_backward_from_sums(grads, bn, dz, part, c, co)
         else:
             dc = g
         gb = grads.dest(conv.bias)
@@ -324,9 +268,9 @@ def backward(model, tape, dlogits, sink=None):
             C0 = conv.out_channels
             gw = ops.conv2d_wgrad(dc, x, 1, 1, bias_out=gb).view(C0, _STEM_LDK)
             grads.put(conv.bias, gb)
-            grads.put(conv.weight, ops.stem_wgrad_relayout(gw, C0, 3, 9, out=dest(conv.weight)))
+            grads.put(conv.weight, ops.stem_wgrad_relayout(gw, C0, 3, 9, out=grads.dest(conv.weight)))
             break
-        gw = ops.conv2d_wgrad(dc, x, 3, 1, out=dest(conv.weight), bias_out=gb)
+        gw = ops.conv2d_wgrad(dc, x, 3, 1, out=grads.dest(conv.weight), bias_out=gb)
         grads.put(conv.bias, gb)
         grads.put(conv.weight, gw)
         prev = tl[li - 1]

@@ -422,16 +422,7 @@ def bn_backward(g, x, co, relu=True, y_out=None, want_dz=False, dgamma=None, dbe
         sp.end()
     if sync is not None:
         partial = _sync_sums(partial, sync, average=True)
-        nblk = 1
-    acc = 1 if (accumulate and dgamma is not None) else 0
-    if dgamma is None:
-        dgamma = torch.empty(C, dtype=F32, device=x.device)
-        dbeta = torch.empty(C, dtype=F32, device=x.device)
-    m = torch.empty(2, C, dtype=F32, device=x.device)
-    sc = _reduce_scratch(x.device)
-    rc = lib.b200_bn_bwd_finalize(_p(partial), nblk, C, float(rows), _p(dgamma), _p(dbeta), acc, _p(m[0]), _p(m[1]),
-                                  _p(co.mean), _p(co.invstd), _p(sc), sc.numel(), _stream())
-    _lib.check(rc, "b200_bn_bwd_finalize")
+    dgamma, dbeta, m = bn_bwd_finalize(partial, rows, co, dgamma, dbeta, accumulate)
     dx = torch.empty_like(x)
     src = dz if want_dz else g
     sp = _span("bn_bwd_apply", 0.0, _nb(src, x, dx, None if want_dz else y_out))
@@ -443,22 +434,37 @@ def bn_backward(g, x, co, relu=True, y_out=None, want_dz=False, dgamma=None, dbe
     return dx, dgamma, dbeta, dz
 
 
-def bn_backward_from_sums(dz, partial, x, co, dgamma=None, dbeta=None, sync=None):
-    """Second half of bn_backward(relu=True) when the producer of the gradient already masked it (dz) and summed
-    partial[rows][2][C] = sum(dz), sum(dz * x) in its epilogue (conv2d_dgrad / gemm_dual with bn_mask=)."""
+def bn_bwd_finalize(partial, count, co, dgamma=None, dbeta=None, accumulate=False):
+    """dgamma, dbeta and m = {m1, m2} fp32 [2, C] of a train-mode BatchNorm from partial [T, 2, C] = {sum dz, sum dz * x}
+    (x the raw BatchNorm input, co its BnCoeffs).  ``accumulate`` adds onto the given dgamma / dbeta."""
     lib = _lib.load()
+    T, _, C = partial.shape
+    dev = partial.device
+    acc = 1 if (accumulate and dgamma is not None) else 0
+    if dgamma is None:
+        dgamma = torch.empty(C, dtype=F32, device=dev)
+    if dbeta is None:
+        dbeta = torch.empty(C, dtype=F32, device=dev)
+    m = torch.empty(2, C, dtype=F32, device=dev)
+    sc = _reduce_scratch(dev)
+    rc = lib.b200_bn_bwd_finalize(_p(partial), T, C, float(count), _p(dgamma), _p(dbeta), acc, _p(m[0]), _p(m[1]),
+                                  _p(co.mean), _p(co.invstd), _p(sc), sc.numel(), _stream())
+    _lib.check(rc, "b200_bn_bwd_finalize")
+    return dgamma, dbeta, m
+
+
+def bn_backward_from_sums(dz, partial, x, co, dgamma=None, dbeta=None, sync=None):
+    """Train-mode BatchNorm backward from a gradient dz that is already masked, bf16 shaped like x, and its partial sums
+    [T, 2, C] = {sum dz, sum dz * x} (a dgrad / gemm_dual epilogue with bn_mask=, or a reduce pass): finalize, then
+    dx = scale * (dz - m1 - xhat * m2) at any channel count that is a multiple of 8 up to 8192.  Returns (dx, dgamma, dbeta)."""
+    lib = _lib.load()
+    _chk_act(dz, "dz")
+    _chk_act(x, "x")
     C = x.shape[-1]
     rows = x.numel() // C
     if sync is not None:
         partial = _sync_sums(partial, sync, average=True)
-    if dgamma is None:
-        dgamma = torch.empty(C, dtype=F32, device=x.device)
-        dbeta = torch.empty(C, dtype=F32, device=x.device)
-    m = torch.empty(2, C, dtype=F32, device=x.device)
-    sc = _reduce_scratch(x.device)
-    rc = lib.b200_bn_bwd_finalize(_p(partial), partial.shape[0], C, float(rows), _p(dgamma), _p(dbeta), 0, _p(m[0]), _p(m[1]),
-                                  _p(co.mean), _p(co.invstd), _p(sc), sc.numel(), _stream())
-    _lib.check(rc, "b200_bn_bwd_finalize")
+    dgamma, dbeta, m = bn_bwd_finalize(partial, rows, co, dgamma, dbeta)
     dx = torch.empty_like(x)
     sp = _span("bn_bwd_apply", 0.0, _nb(dz, x, dx))
     rc = lib.b200_bn_bwd_apply(_p(dz), _p(x), None, 1, _p(dx), _p(co.scale), _p(co.shift), _p(co.mean), _p(co.invstd),
@@ -629,24 +635,6 @@ def repvgg_bwd_reduce(g, y, c3, c1, x=None):
     if sp:
         sp.end()
     return partial
-
-
-def bn_bwd_finalize(partial, count, co, dgamma=None, dbeta=None):
-    """dgamma, dbeta and m = {m1, m2} fp32 [2, C] of a train-mode BatchNorm from partial [T, 2, C] = {sum dz, sum dz * x}
-    (x the raw BatchNorm input, co its BnCoeffs)."""
-    lib = _lib.load()
-    T, _, C = partial.shape
-    dev = partial.device
-    if dgamma is None:
-        dgamma = torch.empty(C, dtype=F32, device=dev)
-    if dbeta is None:
-        dbeta = torch.empty(C, dtype=F32, device=dev)
-    m = torch.empty(2, C, dtype=F32, device=dev)
-    sc = _reduce_scratch(dev)
-    rc = lib.b200_bn_bwd_finalize(_p(partial), T, C, float(count), _p(dgamma), _p(dbeta), 0, _p(m[0]), _p(m[1]), _p(co.mean),
-                                  _p(co.invstd), _p(sc), sc.numel(), _stream())
-    _lib.check(rc, "b200_bn_bwd_finalize")
-    return dgamma, dbeta, m
 
 
 def repvgg_bwd_apply(g, y, c3, c1, co3, m3, co1, m1, x=None, co_id=None, m_id=None, out=None):
@@ -908,22 +896,6 @@ def tail_bwd_reduce(g, c, rs=None):
     if sp:
         sp.end()
     return (g if dz is None else dz), partial
-
-
-def bn_bwd_apply_dz(dz, c, co, m):
-    """dc = scale * (dz - m1 - (c - mean) * invstd * m2) bf16: the BatchNorm backward apply from a stored dz (m from
-    bn_bwd_finalize)."""
-    lib = _lib.load()
-    _chk_act(dz, "dz")
-    _chk_act(c, "c")
-    C = c.shape[-1]
-    dc = torch.empty_like(c)
-    sp = _span("bn_bwd_apply_dz", 0.0, _nb(dz, c, dc))
-    rc = lib.b200_bn_bwd_apply_dz(_p(dz), _p(c), _p(co.mean), _p(m), _p(dc), c.numel() // C, C, _stream())
-    _lib.check(rc, "b200_bn_bwd_apply_dz")
-    if sp:
-        sp.end()
-    return dc
 
 
 # ------------------------------------------------------------------------------ BatchNorm folded through a 1x1 convolution

@@ -268,7 +268,9 @@ int b200_bn_bwd_blocks(long long rows, int C);
 int b200_bn_bwd_finalize(const float* partial, int T, int C, double count, float* dgamma, float* dbeta, int accumulate,
                          float* m1, float* m2, const float* mean, const float* invstd, void* scratch,
                          size_t scratch_bytes, void* stream);
-/* backward pass 2: dx = scale*(dz - m1 - xhat*m2); g_is_dz != 0 means `g` already holds dz (mask applied). */
+/* backward pass 2: dx = scale*(dz - m1 - xhat*m2); g_is_dz != 0 means `g` already holds dz (mask applied), otherwise dz
+ * is g masked as in pass 1 (relu: from y_out when given, else from x). Any C multiple of 8 in [8, 8192] and rows >= 1;
+ * every pointer but y_out is required and 16-byte aligned. */
 int b200_bn_bwd_apply(const void* g, const void* x, const void* y_out, int g_is_dz, void* dx, const float* scale,
                       const float* shift, const float* mean, const float* invstd, const float* m1, const float* m2,
                       int relu, long long rows, int C, void* stream);
@@ -483,7 +485,7 @@ int b200_repvgg_fold(const float* w3, const float* w1, const float* gamma3, cons
  * tail_apply:  project BatchNorm, DropPath and shortcut (network.py:237-242): y = (c * scale + shift) * rs[b] (+ residual);
  *              rs fp32 [B] (the per-sample drop-connect multiplier) and residual optional
  * tail_bwd_reduce: dz = g * rs[b] stored bf16 (dz and rs both or neither; without them dz = g), partial = {sum dz, sum dz c}
- * bn_bwd_apply_dz: train-mode BatchNorm backward apply from a stored dz: dc = scale (dz - m1 - (c - mean) invstd m2) */
+ * The BatchNorm backward apply from a stored dz is b200_bn_bwd_apply(g_is_dz = 1) with m1 / m2 of b200_bn_bwd_finalize. */
 int b200_dw_partial_rows(long long rows, int C);
 int b200_dw_fwd(const void* x, const float* w, const float* scale, const float* shift, void* d, float* stats, int B, int H,
                 int W, int C, int k, int stride, void* stream);
@@ -509,8 +511,6 @@ int b200_silu_bn_bwd_reduce(const void* da, const float* gate, const float* dpoo
 int b200_tail_apply(const void* c, const float* scale, const float* shift, const float* rs, const void* residual, void* y,
                     int B, int HW, int C, void* stream);
 int b200_tail_bwd_reduce(const void* g, const float* rs, const void* c, void* dz, float* partial, int B, int HW, int C,
-                         void* stream);
-int b200_bn_bwd_apply_dz(const void* dz, const void* c, const float* co, const float* m, void* dc, long long rows, int C,
                          void* stream);
 
 /* ---- VGG (classification/vggNet/models/network.py) passes the convolution GEMMs do not cover, and torch.optim.Adam.

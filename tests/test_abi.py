@@ -24,11 +24,11 @@ def test_header_symbols_exported_and_bound():
     assert set(_lib.SIGNATURES) == set(names)
 
 
-def test_no_compute_calls_without_gpu_but_metadata_works():
+def test_host_metadata_without_gpu():
     from deeplearning_b200 import _lib
 
     lib = _lib.load()
-    assert lib.b200_abi_version() == 2
+    assert lib.b200_abi_version() == 3
     # pure host-side planners are usable without a device
     # BN statistics rows: (persistent CTAs / channel blocks) x 4 row quadrants (x2 when the warp pair alternates tiles);
     # without a device the planner assumes the 132 SMs of an H100 SXM; channel blocks are 64 or 128 wide

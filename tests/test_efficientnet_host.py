@@ -160,7 +160,7 @@ def _rejects(call, msg):
 
 
 @pytest.mark.parametrize("C", [0, 4, 36, 8200])
-def test_entries_reject_channel_count(C):
+def test_efficientnet_entries_reject_channel_count(C):
     m = "a multiple of 8 in [8, 8192]"
     _rejects(lambda L: L.b200_dw_fwd(F_, F_, None, None, F_, None, 2, 8, 8, C, 3, 1, None), m)
     _rejects(lambda L: L.b200_dw_dgrad(F_, F_, F_, None, None, None, F_, None, 2, 8, 8, C, 3, 1, None), m)
@@ -173,13 +173,13 @@ def test_entries_reject_channel_count(C):
     _rejects(lambda L: L.b200_silu_bn_bwd_reduce(F_, F_, F_, F_, F_, F_, F_, F_, 2, 16, C, None), m)
     _rejects(lambda L: L.b200_tail_apply(F_, F_, F_, None, None, F_, 2, 16, C, None), m)
     _rejects(lambda L: L.b200_tail_bwd_reduce(F_, None, F_, None, F_, 2, 16, C, None), m)
-    _rejects(lambda L: L.b200_bn_bwd_apply_dz(F_, F_, F_, F_, F_, 32, C, None), m)
+    _rejects(lambda L: L.b200_bn_bwd_apply(F_, F_, None, 1, *([F_] * 7), 1, 32, C, None), m)
     L = _lib().load()
     assert L.b200_dw_partial_rows(32, C) == -1
     assert L.b200_dw_wgrad_workspace_bytes(2, 8, 8, C, 3, 1) == 0
 
 
-def test_entries_reject_shapes_and_pointers():
+def test_efficientnet_entries_reject_shapes_and_pointers():
     _rejects(lambda L: L.b200_dw_fwd(F_, F_, None, None, F_, None, 2, 8, 8, 64, 7, 1, None), "k must be 3 or 5")
     _rejects(lambda L: L.b200_dw_fwd(F_, F_, None, None, F_, None, 2, 8, 8, 64, 3, 3, None), "stride must be 1 or 2")
     _rejects(lambda L: L.b200_dw_fwd(F_, F_, None, None, F_, None, 2, 0, 8, 64, 3, 1, None), "H and W must be >= 1")
@@ -199,7 +199,10 @@ def test_entries_reject_shapes_and_pointers():
     _rejects(lambda L: L.b200_silu_bn_bwd_reduce(F_, None, F_, F_, F_, F_, F_, F_, 2, 16, 64, None), "come together")
     _rejects(lambda L: L.b200_tail_apply(F_, F_, F_, None, F_ + 8, F_, 2, 16, 64, None), "16-byte aligned")
     _rejects(lambda L: L.b200_tail_bwd_reduce(F_, F_, F_, None, F_, 2, 16, 64, None), "exactly when rs is given")
-    _rejects(lambda L: L.b200_bn_bwd_apply_dz(F_, F_, F_, F_, F_, 0, 64, None), "rows >= 1")
+    _rejects(lambda L: L.b200_bn_bwd_apply(F_, F_, None, 1, *([F_] * 7), 1, 0, 64, None), "rows >= 1")
+    _rejects(lambda L: L.b200_bn_bwd_apply(F_, F_ + 8, None, 1, *([F_] * 7), 1, 32, 64, None), "16-byte aligned")
+    _rejects(lambda L: L.b200_bn_bwd_apply(F_, F_, F_ + 8, 0, *([F_] * 7), 1, 32, 64, None), "16-byte aligned")
+    _rejects(lambda L: L.b200_bn_bwd_apply(F_, F_, None, 1, F_, F_, F_, F_, F_, None, F_, 1, 32, 64, None), "non-null")
     L = _lib().load()
     assert L.b200_dw_partial_rows(1000, 64) > 0
     assert L.b200_dw_wgrad_workspace_bytes(2, 8, 8, 64, 5, 2) % (25 * 64 * 4) == 0

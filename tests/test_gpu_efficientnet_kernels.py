@@ -179,7 +179,7 @@ def test_silu_bn_bwd_reduce(shape, with_da):
 
 @pytest.mark.parametrize("shape", ROW_SHAPES)
 @pytest.mark.parametrize("rs_on,res_on", [(False, False), (True, False), (False, True), (True, True)])
-def test_tail_and_bn_apply(shape, rs_on, res_on):
+def test_tail_passes_and_bn_backward_from_sums(shape, rs_on, res_on):
     B, HW, C = shape
     c = _bf16(B, HW, 1, C, seed=12)
     co = _co(C, seed=13)
@@ -199,7 +199,37 @@ def test_tail_and_bn_apply(shape, rs_on, res_on):
     z = _d(dz).reshape(-1, C)
     _close(part.double().sum(0)[0], z.sum(0), rel=1e-5, what="sum dz")
     _close(part.double().sum(0)[1], (z * _d(c).reshape(-1, C)).sum(0), rel=1e-5, what="sum dz c")
-    m = torch.randn(2, C, device="cuda")
-    dc = ops.bn_bwd_apply_dz(dz, c, co, m)
+    dc, dgamma, dbeta = ops.bn_backward_from_sums(dz, part, c, co)
     xhat = (_d(c).reshape(-1, C) - _d(co.mean)) * _d(co.invstd)
-    _close(dc.reshape(-1, C), _d(co.scale) * (z - _d(m[0]) - xhat * _d(m[1])), what="bn_bwd_apply_dz")
+    db_ref, dg_ref = z.sum(0), (z * xhat).sum(0)
+    _close(dbeta, db_ref, rel=1e-5, what="dbeta")
+    _close(dgamma, dg_ref, rel=1e-4, what="dgamma")
+    m1, m2 = db_ref / z.shape[0], dg_ref / z.shape[0]
+    _close(dc.reshape(-1, C), _d(co.scale) * (z - m1 - xhat * m2), what="bn_backward_from_sums dx")
+
+
+@pytest.mark.parametrize("C", [240, 3840])
+@pytest.mark.parametrize("source", ["dz", "mask_x", "mask_y"])
+def test_bn_bwd_apply_sources(C, source):
+    """b200_bn_bwd_apply at widths that are not 8 * 2^k (one channel chunk, and two) for each gradient source: g is dz
+    already, or g masked where x * scale + shift > 0, or where the stored output y > 0"""
+    from deeplearning_b200 import _lib
+
+    rows = 196
+    g, x = _bf16(rows, C, seed=20), _bf16(rows, C, seed=21)
+    y = _bf16(rows, C, seed=22) if source == "mask_y" else None
+    co = _co(C, seed=23)
+    m = torch.randn(2, C, device="cuda") * 0.1
+    dx = torch.empty_like(x)
+    ptr = [t.data_ptr() for t in (co.scale, co.shift, co.mean, co.invstd, m[0], m[1])]
+    rc = _lib.load().b200_bn_bwd_apply(g.data_ptr(), x.data_ptr(), None if y is None else y.data_ptr(),
+                                       1 if source == "dz" else 0, dx.data_ptr(), *ptr, 1, rows, C,
+                                       torch.cuda.current_stream().cuda_stream)
+    _lib.check(rc, "b200_bn_bwd_apply")
+    z = _d(g)
+    if source == "mask_x":   # (exact in float64: the product of a bf16 and an fp32 value, then one rounding)
+        z = z * (_d(x) * _d(co.scale) + _d(co.shift) > 0)
+    elif source == "mask_y":
+        z = z * (_d(y) > 0)
+    xhat = (_d(x) - _d(co.mean)) * _d(co.invstd)
+    _close(dx, _d(co.scale) * (z - _d(m[0]) - xhat * _d(m[1])), what=f"bn_bwd_apply {source}")

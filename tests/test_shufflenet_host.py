@@ -9,6 +9,7 @@ import torch.nn.functional as F
 
 from deeplearning_b200.classification.ShuffleNet import models as pkg
 from deeplearning_b200.classification.ShuffleNet.models import shufflenetv1 as sn
+from deeplearning_b200.engine import common
 from deeplearning_b200.engine import shufflenet as eng
 
 WIDTHS = {"g1": (1, [144, 288, 576]), "g2": (2, [200, 400, 800]), "g3": (3, [240, 480, 960]),
@@ -97,10 +98,10 @@ def test_admission_batchnorm():
     _raises(m, r"conv1\.1: expected an affine BatchNorm2d")
 
 
-def test_admission_sync_batchnorm(monkeypatch):
+def test_admission_sync_batchnorm_multi_rank(monkeypatch):
     m = nn.SyncBatchNorm.convert_sync_batchnorm(sn.shufflenet_v1_x1_g3())
     eng.check_model(m)            # one process: admitted
-    monkeypatch.setattr(eng, "_bn_sync", lambda bn: (None, 2) if isinstance(bn, nn.SyncBatchNorm) else None)
+    monkeypatch.setattr(common, "bn_sync", lambda bn: (None, 2) if isinstance(bn, nn.SyncBatchNorm) else None)
     _raises(m, r"conv1\.1: SyncBatchNorm in a multi-rank job is not implemented")
 
 

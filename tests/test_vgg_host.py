@@ -6,6 +6,7 @@ import torch
 import torch.nn as nn
 
 from deeplearning_b200.classification.vggNet.models import network
+from deeplearning_b200.engine import common
 from deeplearning_b200.engine import vgg as engine
 from oracle.vgg import arch
 
@@ -103,12 +104,12 @@ def test_cpu_input_raises():
         m(torch.zeros(1, 3, 32, 32))
 
 
-def test_sync_batchnorm(monkeypatch):
+def test_sync_batchnorm_admission(monkeypatch):
     """a SyncBatchNorm model is admitted outside a multi-rank job and rejected, naming the layer, inside one"""
     m = nn.SyncBatchNorm.convert_sync_batchnorm(network.vgg11_bn(num_classes=3))
     assert type(m.features[1]) is nn.SyncBatchNorm
     layers, _, _ = engine.check_model(m)
     assert all(type(l.bn) is nn.SyncBatchNorm for l in layers)
-    monkeypatch.setattr(engine, "_bn_sync", lambda bn: (None, 2) if isinstance(bn, nn.SyncBatchNorm) else None)
+    monkeypatch.setattr(common, "bn_sync", lambda bn: (None, 2) if isinstance(bn, nn.SyncBatchNorm) else None)
     with pytest.raises(NotImplementedError, match=r"features\.1: SyncBatchNorm in a multi-rank job"):
         engine.check_model(m)

@@ -100,8 +100,7 @@ def pass_shapes(B):
         hpre, gate = ops.excite_fwd(pool, w1, b1, w2, b2)
         sg = ops.gate_reduce(da, d, co)
         dpool = torch.randn(B, C, device="cuda")
-        m = torch.zeros(2, C, device="cuda")
-        dz, _ = ops.silu_bn_bwd_reduce(d, co, dpool, da=da, gate=gate)
+        dz, part = ops.silu_bn_bwd_reduce(d, co, dpool, da=da, gate=gate)
         rs = torch.ones(B, device="cuda")
         name = f"{tag} {H:3d}->{Ho:<3d} C={C:4d} k{k}s{s}"
         out += [
@@ -116,7 +115,7 @@ def pass_shapes(B):
             (f"{name} silu_bn_bwd_reduce", 3 * nb(d), lambda a=(d, co, dpool, da, gate): ops.silu_bn_bwd_reduce(*a[:3], da=a[3], gate=a[4])),
             (f"{name} tail_apply (+drop-connect, residual)", 3 * nb(d), lambda a=(d, co, rs, da): ops.tail_apply(*a[:3], residual=a[3])),
             (f"{name} tail_bwd_reduce (+drop-connect)", 3 * nb(d), lambda a=(da, d, rs): ops.tail_bwd_reduce(*a)),
-            (f"{name} bn_bwd_apply_dz", 3 * nb(d), lambda a=(dz, d, co, m): ops.bn_bwd_apply_dz(*a)),
+            (f"{name} bn_bwd_apply (+finalize)", 3 * nb(d), lambda a=(dz, part, d, co): ops.bn_backward_from_sums(*a)),
         ]
     return out
 
