@@ -160,6 +160,8 @@ SIGNATURES = {
     "b200_dw_relu_wgrad": (_I, [_P] * 6 + [c_size_t] + [_I] * 5 + [_P]),
     "b200_shuffle_tail_s2_fwd": (_I, [_P] * 5 + [_I] * 5 + [_P]),
     "b200_shuffle_relu_bwd": (_I, [_P] * 8 + [_I] * 7 + [_P]),
+    "b200_shufflev2_tail_fwd": (_I, [_P] * 8 + [_L, _I, _I, _P]),
+    "b200_shufflev2_tail_bwd": (_I, [_P] * 12 + [_L, _I, _I, _P]),
     "b200_vgg_pool_partial_rows": (_I, [_I, _I, _I, _I]),
     "b200_vgg_pool_fwd": (_I, [_P] * 5 + [_I] * 4 + [_P]),
     "b200_vgg_pool_bwd": (_I, [_P] * 8 + [_I] * 4 + [_P]),

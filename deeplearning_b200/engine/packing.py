@@ -112,6 +112,9 @@ class _WeightCache:
         return pack
 
     def get(self, param, mode, ld=None, pad_rows=None, pad_cols=None):
+        """The packed bf16 operand of ``param`` (ops.pack_weight ``mode``), cached until the parameter changes.  Mode 0:
+        row pitch ``ld``, zero rows appended up to ``pad_rows`` (padded output channels).  Mode 1: row pitch ``pad_cols``
+        (else ``ld``), zero rows appended up to ``pad_rows`` (padded input channels)."""
         key = (id(param), mode, ld, pad_rows, pad_cols)
         hit = self._store.get(key)
         stamp = (param._version, param.data_ptr(), self.generation)
@@ -120,12 +123,12 @@ class _WeightCache:
         w = param.detach()
         if mode == 0:
             packed = ops.pack_weight(w, 0, ld=ld)
-            if pad_rows is not None and pad_rows != packed.shape[0]:
-                full = torch.zeros(pad_rows, packed.shape[1], dtype=packed.dtype, device=packed.device)
-                full[: packed.shape[0]] = packed
-                packed = full
         else:
             packed = ops.pack_weight(w, 1, ld=pad_cols if pad_cols is not None else ld)
+        if pad_rows is not None and pad_rows != packed.shape[0]:
+            full = torch.zeros(pad_rows, packed.shape[1], dtype=packed.dtype, device=packed.device)
+            full[: packed.shape[0]] = packed
+            packed = full
         self._store[key] = (stamp, packed, weakref.ref(param))
         if len(self._store) > 4096:
             self._store = {k: v for k, v in self._store.items() if v[2]() is not None}

@@ -20,8 +20,8 @@ Layout decisions (DESIGN.md section 3):
 - Bottleneck tensors have a channel pitch rounded up to a multiple of 8.  Pad rows / columns of the operands are zero and
   the pad channels' BatchNorm coefficients are 0, so those channels stay exactly 0 through every pass.
 
-The stem is one GEMM over the im2col patch matrix of the image, then BatchNorm + ReLU + the 3x3/2 max-pool in one pass; the
-network ends with the global mean and the shared classifier head.  Eval mode runs the same passes with running-statistics
+The stem is one GEMM over the im2col patch matrix of the image, then BatchNorm + ReLU + the 3x3/2 max-pool in one pass
+(engine/shufflenet_parts.py, shared with ShuffleNet v2); the network ends with the global mean and the shared classifier head.  Eval mode runs the same passes with running-statistics
 coefficients and records no statistics or tape.
 """
 import sys
@@ -33,31 +33,11 @@ import torch.nn as nn
 from .. import ops
 from . import common
 from .packing import weight_cache
-
-_STEM_LDK = 32     # patch-matrix width of the 3x3 x 3-channel stem (27 columns, padded to a multiple of 8)
-
-
-def _pad8(n):
-    return (n + 7) // 8 * 8
+from .shufflenet_parts import PaddedBN, check_bn as _check_bn, check_conv as _check_conv, pad8 as _pad8
+from . import shufflenet_parts as parts
 
 
 # --------------------------------------------------------------------------------------------------------- admission
-def _check_bn(name, bn, C):
-    if not common.bn_ok(bn, C):
-        raise NotImplementedError(f"{name}: expected an affine BatchNorm2d over {C} channels that tracks running statistics "
-                                  f"(got {bn})")
-    if common.bn_sync(bn) is not None:
-        raise NotImplementedError(f"{name}: SyncBatchNorm in a multi-rank job is not implemented for ShuffleNet")
-
-
-def _check_conv(name, conv, k, stride, cin, cout, groups):
-    if (type(conv) is not nn.Conv2d or conv.bias is not None or conv.dilation != (1, 1) or conv.padding_mode != "zeros"
-            or conv.kernel_size != (k, k) or conv.stride != (stride, stride) or conv.padding != (k // 2, k // 2)
-            or conv.in_channels != cin or conv.out_channels != cout or conv.groups != groups):
-        raise NotImplementedError(f"{name}: expected a bias-free {k}x{k} Conv2d {cin} -> {cout}, stride {stride}, padding "
-                                  f"{k // 2}, groups {groups} (got {conv})")
-
-
 def _widths8(name, **widths):
     bad = {k: v for k, v in widths.items() if v % 8 != 0}
     if bad:
@@ -118,17 +98,8 @@ def check_model(model):
     names = list(model._modules)
     if names != ["conv1", "maxpool", "stage2", "stage3", "stage4", "fc"]:
         raise NotImplementedError(f"ShuffleNetv1: expected the modules conv1, maxpool, stage2..4, fc (got {names})")
-    stem = model.conv1
-    if not isinstance(stem, nn.Sequential) or len(stem) != 3 or type(stem[2]) is not nn.ReLU:
-        raise NotImplementedError("conv1: expected the reference's Sequential(Conv2d, BatchNorm2d, ReLU)")
-    c0 = getattr(stem[0], "out_channels", 0)
-    _check_conv("conv1.0", stem[0], 3, 2, 3, c0, 1)
-    _check_bn("conv1.1", stem[1], c0)
+    stem_conv, stem_bn, c0 = parts.check_stem(model)
     _widths8("conv1", stem=c0)
-    mp = model.maxpool
-    if (type(mp) is not nn.MaxPool2d or mp.kernel_size not in (3, (3, 3)) or mp.stride not in (2, (2, 2))
-            or mp.padding not in (1, (1, 1)) or mp.dilation not in (1, (1, 1)) or mp.ceil_mode or mp.return_indices):
-        raise NotImplementedError(f"maxpool: expected MaxPool2d(3, 2, 1) (got {mp})")
     blocks = []
     cin = c0
     for sname in ("stage2", "stage3", "stage4"):
@@ -141,7 +112,7 @@ def check_model(model):
     fc = model.fc
     if type(fc) is not nn.Linear or fc.in_features != cin:
         raise NotImplementedError(f"fc: expected a Linear over the {cin} features of stage4 (got {fc})")
-    return stem[0], stem[1], blocks, fc
+    return stem_conv, stem_bn, blocks, fc
 
 
 # ---------------------------------------------------------------------------------------------------------- packing
@@ -153,7 +124,7 @@ class _PackSpec:
 
     def __call__(self, model):
         stem = model.conv1[0]
-        return [(stem.weight, 0, _STEM_LDK, stem.out_channels)] + common.head_pack_specs(model.fc)
+        return [parts.stem_pack_spec(stem)] + common.head_pack_specs(model.fc)
 
 
 _pack_spec = _PackSpec()
@@ -223,42 +194,6 @@ class _GroupedConv:
         return out.copy_(g)
 
 
-class _PaddedBN:
-    """A BatchNorm over a bottleneck tensor stored with channel pitch Cp: stored channel n < b is the BatchNorm's channel
-    src[n]; pad channels get gamma = beta = 0 (coefficients 0, so they stay 0).  Statistics, parameters and gradients of
-    the real channels go to and from the module in its own order."""
-
-    def __init__(self, bn, src, Cp, device):
-        b = bn.num_features
-        self.bn, self.b = bn, b
-        idx = torch.full((Cp,), b, dtype=torch.int64)
-        idx[:b] = torch.tensor(src, dtype=torch.int64)
-        self.idx = idx.to(device)
-        self.src = self.idx[:b]
-
-    def _gather(self, v, fill):
-        v = v.detach()
-        return torch.cat([v, v.new_full((1,), fill)])[self.idx]
-
-    def coeffs(self, stats, rows, train):
-        bn = self.bn
-        gamma, beta = self._gather(bn.weight, 0.0), self._gather(bn.bias, 0.0)
-        rm, rv = self._gather(bn.running_mean, 0.0), self._gather(bn.running_var, 1.0)
-        if not train:
-            return ops.bn_eval_coeffs(gamma, beta, rm, rv, bn.eps)
-        co = ops.bn_finalize(stats, rows, gamma, beta, bn.eps, bn.momentum, rm, rv, bn.num_batches_tracked)
-        with torch.no_grad():
-            bn.running_mean.index_copy_(0, self.src, rm[:self.b])
-            bn.running_var.index_copy_(0, self.src, rv[:self.b])
-        return co
-
-    def scatter(self, v, out=None):
-        """v fp32 [Cp] in stored order -> [b] in the module's order (into ``out`` when given)."""
-        if out is None:
-            out = torch.empty(self.b, dtype=v.dtype, device=v.device)
-        return out.index_copy_(0, self.src, v[:self.b])
-
-
 class _Plan:
     """Per-model device state of the schedule: the grouped convolutions and padded BatchNorms of every block."""
 
@@ -270,8 +205,8 @@ class _Plan:
             order = shuffle_order(k.b, k.g)
             self.conv1.append(_GroupedConv(k.conv1, order, k.bp, k.cin, device))
             self.conv3.append(_GroupedConv(k.conv3, list(range(k.cc)), k.cc, k.bp, device))
-            self.bn1.append(_PaddedBN(k.bn1, order, k.bp, device))
-            self.bn2.append(_PaddedBN(k.bn2, list(range(k.b)), k.bp, device))
+            self.bn1.append(PaddedBN(k.bn1, order, k.bp, device))
+            self.bn2.append(PaddedBN(k.bn2, list(range(k.b)), k.bp, device))
 
 
 _plans = weakref.WeakKeyDictionary()
@@ -286,14 +221,6 @@ def _plan(model, blocks, device):
     return plan
 
 
-def _dw_weight(k):
-    """The depthwise weight [bp, 1, 3, 3] fp32 with zero pad channels."""
-    w = k.dw.weight.detach()
-    if k.bp == k.b:
-        return w.contiguous()
-    return torch.cat([w, w.new_zeros(k.bp - k.b, 1, 3, 3)]).contiguous()
-
-
 # ---------------------------------------------------------------------------------------------------------- forward
 def forward(model, x, train, want_tape):
     """x: fp32 NCHW (or decoded uint8 NHWC) CUDA batch.  Returns (logits fp32 [B, num_classes], tape or None)."""
@@ -304,20 +231,15 @@ def forward(model, x, train, want_tape):
     pack = weight_cache.model_pack(model, _pack_spec)
     plan = _plan(model, blocks, x.device)
     tape = {"blocks": [], "pack": pack, "plan": plan} if (train and want_tape) else None
-    B = x.shape[0]
-    a, Ho, Wo = ops.im2col_nchw(x, 3, 3, 2, 1, ldk=_STEM_LDK)
-    patches = a.view(B, Ho, Wo, _STEM_LDK)
-    c_s, st = ops.conv2d_fwd(patches, pack.get(stem_conv.weight, 0), 1, 1, want_stats=train)
-    co_s = common.bn_coeffs(stem_bn, st, common.rows(c_s), train)
-    h, idx = ops.bn_relu_maxpool_fwd(c_s, co_s)
+    h, saved = parts.stem_forward(pack, stem_conv, stem_bn, x, train)
     if tape is not None:
-        tape["stem"] = (patches, c_s, co_s, idx)
+        tape["stem"] = saved
     for i, k in enumerate(blocks):
         w1, _ = plan.conv1[i].operands()
         w3, _ = plan.conv3[i].operands()
         c1, st = ops.conv2d_fwd(h, w1, 1, 1, want_stats=train)
         co1 = plan.bn1[i].coeffs(st, common.rows(c1), train)
-        wd = _dw_weight(k)
+        wd = parts.padded_dw_weight(k.dw, k.bp)
         d, st = ops.dw_relu_fwd(c1, wd, k.s, co1, want_stats=train)
         co2 = plan.bn2[i].coeffs(st, common.rows(d), train)
         a = ops.bn_apply(d, co2, relu=False)
@@ -342,12 +264,6 @@ def backward(model, tape, dlogits, sink=None):
     grads = common.Grads(sink)
     pack, plan = tape["pack"], tape["plan"]
 
-    def padded_bn_backward(pbn, dz, partial, c, co):
-        dc, dg, db = ops.bn_backward_from_sums(dz, partial, c, co)
-        grads.put(pbn.bn.bias, pbn.scatter(db, grads.dest(pbn.bn.bias)))
-        grads.put(pbn.bn.weight, pbn.scatter(dg, grads.dest(pbn.bn.weight)))
-        return dc
-
     pooled, hw = tape["head"]
     g = ops.avgpool_bwd(common.head_backward(grads, pack, fc, pooled, dlogits), hw)
     for i in range(len(blocks) - 1, -1, -1):
@@ -363,23 +279,17 @@ def backward(model, tape, dlogits, sink=None):
         grads.put(k.conv3.weight, gc3.weight_grad(ops.conv2d_wgrad(dc3, a, 1, 1), grads.dest(k.conv3.weight)))
         da = ops.conv2d_dgrad(dc3, gc3.operands()[1], tuple(a.shape[1:3]), 1, 1)
         _, part = ops.tail_bwd_reduce(da, d)
-        dd = padded_bn_backward(plan.bn2[i], da, part, d, co2)
+        dd = plan.bn2[i].backward(grads, da, part, d, co2)
         gw = ops.dw_relu_wgrad(dd, c1, k.s, co1)
         gwd = grads.dest(k.dw.weight)
         gw = gw[:k.b] if gwd is None else gwd.copy_(gw[:k.b])
         grads.put(k.dw.weight, gw)
         dz1, part = ops.dw_relu_dgrad(dd, wd, c1, k.s, co1)
-        dc1 = padded_bn_backward(plan.bn1[i], dz1, part, c1, co1)
+        dc1 = plan.bn1[i].backward(grads, dz1, part, c1, co1)
         gc1 = plan.conv1[i]
         grads.put(k.conv1.weight, gc1.weight_grad(ops.conv2d_wgrad(dc1, x, 1, 1), grads.dest(k.conv1.weight)))
         g = ops.conv2d_dgrad(dc1, gc1.operands()[1], tuple(x.shape[1:3]), 1, 1, residual=shortcut)
-    patches, c_s, co_s, idx = tape["stem"]
-    g_act = ops.maxpool_bwd(g, idx, tuple(c_s.shape[1:3]))
-    dz, part, _ = ops.shuffle_relu_bwd(g_act, c_s, co=co_s)
-    dc = common.bn_backward_from_sums(grads, stem_bn, dz, part, c_s, co_s)
-    C0 = c_s.shape[-1]
-    gw = ops.conv2d_wgrad(dc, patches, 1, 1).view(C0, _STEM_LDK)
-    grads.put(stem_conv.weight, ops.stem_wgrad_relayout(gw, C0, 3, 9, out=grads.dest(stem_conv.weight)))
+    parts.stem_backward(grads, stem_conv, stem_bn, g, tape["stem"])
     return grads
 
 

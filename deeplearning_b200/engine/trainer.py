@@ -71,6 +71,12 @@ def _engine_for(model):
         from . import shufflenet
 
         return shufflenet
+    from ..classification.ShuffleNet.models.shufflenetv2 import ShuffleNetV2
+
+    if isinstance(model, ShuffleNetV2):
+        from . import shufflenetv2
+
+        return shufflenetv2
     raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 

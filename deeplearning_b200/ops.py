@@ -1943,3 +1943,71 @@ def shuffle_relu_bwd(g, c, y=None, co=None, in_hw=None):
     if sp:
         sp.end()
     return dz, partial, gx
+
+
+# ------------------------------------------------------------------------------ ShuffleNet v2 tails (csrc/shufflenet.cuh)
+def _v2_pitch(b):
+    return (2 * b + 7) // 8 * 8
+
+
+def shufflev2_tail_fwd(u, c3, co, b, co_u=None, split=False):
+    """channel_shuffle(cat(u, v), 2) of a ShuffleNet v2 block with v = relu(c3 * scale + shift) (BnCoeffs ``co``) and u the
+    passthrough half, or relu(u * scale + shift) with BnCoeffs ``co_u`` (u then branch1's raw GEMM output).  u, c3 bf16
+    [B,H,W,bp] with b real channels.  Returns the joined output bf16 [B,H,W,J] (J = 2b rounded up to a multiple of 8), or
+    with ``split`` its two halves (P', Q') = (out[..., :b], out[..., b:2b]), each [B,H,W,bp]; pad channels are 0."""
+    lib = _lib.load()
+    _chk_act(u, "u")
+    _chk_act(c3, "c3")
+    if tuple(u.shape) != tuple(c3.shape):
+        raise ValueError(f"shufflev2_tail_fwd: u {tuple(u.shape)} and c3 {tuple(c3.shape)} differ")
+    bp = c3.shape[-1]
+    rows = c3.numel() // bp
+    if split:
+        y0, y1 = torch.empty_like(c3), torch.empty_like(c3)
+    else:
+        y0, y1 = torch.empty(*c3.shape[:-1], _v2_pitch(b), dtype=BF16, device=c3.device), None
+    sp = _span("shufflev2_tail_fwd", 0.0, _nb(u, c3, y0, y1))
+    rc = lib.b200_shufflev2_tail_fwd(_p(u), None if co_u is None else _p(co_u.scale), None if co_u is None else _p(co_u.shift),
+                                     _p(c3), _p(co.scale), _p(co.shift), _p(y0), _p(y1), rows, b, bp, _stream())
+    _lib.check(rc, "b200_shufflev2_tail_fwd")
+    if sp:
+        sp.end()
+    return (y0, y1) if split else y0
+
+
+def shufflev2_tail_bwd(g, c3, co, b, cu=None, co_u=None):
+    """Backward of shufflev2_tail_fwd for g = dL/dout: the joined gradient bf16 [B,H,W,J], or a pair (dL/dP', dL/dQ') of
+    [B,H,W,bp].  Returns (dz3, partial3, du, partial_u): dz3 = dL/dv * [c3 * scale + shift > 0] bf16 [B,H,W,bp] with
+    partial3 fp32 [T,2,bp] = {sum dz3, sum dz3 * c3}; du = dL/du (passthrough, partial_u None), or with ``cu`` / ``co_u``
+    du = dL/du * [cu * scale + shift > 0] and partial_u = {sum du, sum du * cu}."""
+    lib = _lib.load()
+    _chk_act(c3, "c3")
+    bp = c3.shape[-1]
+    rows = c3.numel() // bp
+    g0, g1 = g if isinstance(g, (tuple, list)) else (g, None)
+    _chk_act(g0, "g")
+    if g1 is not None:
+        _chk_act(g1, "g")
+        if tuple(g0.shape) != tuple(c3.shape) or tuple(g1.shape) != tuple(c3.shape):
+            raise ValueError(f"shufflev2_tail_bwd: split g {tuple(g0.shape)} / {tuple(g1.shape)} must be shaped like c3 "
+                             f"{tuple(c3.shape)}")
+    elif tuple(g0.shape) != (*c3.shape[:-1], _v2_pitch(b)):
+        raise ValueError(f"shufflev2_tail_bwd: joined g {tuple(g0.shape)} does not match c3 {tuple(c3.shape)} at b={b}")
+    if (cu is None) != (co_u is None):
+        raise ValueError("shufflev2_tail_bwd: give cu and co_u together")
+    if cu is not None:
+        _chk_act(cu, "cu")
+        if tuple(cu.shape) != tuple(c3.shape):
+            raise ValueError(f"shufflev2_tail_bwd: cu {tuple(cu.shape)} must be shaped like c3 {tuple(c3.shape)}")
+    T = repvgg_partial_rows(rows, bp)
+    dz3, du = torch.empty_like(c3), torch.empty_like(c3)
+    part3 = torch.empty(T, 2, bp, dtype=F32, device=c3.device)
+    partu = torch.empty(T, 2, bp, dtype=F32, device=c3.device) if cu is not None else None
+    sp = _span("shufflev2_tail_bwd", 0.0, _nb(g0, g1, c3, cu, dz3, du))
+    rc = lib.b200_shufflev2_tail_bwd(_p(g0), _p(g1), _p(c3), _p(co.scale), _p(co.shift), _p(dz3), _p(part3), _p(cu),
+                                     None if co_u is None else _p(co_u.scale), None if co_u is None else _p(co_u.shift),
+                                     _p(du), _p(partu), rows, b, bp, _stream())
+    _lib.check(rc, "b200_shufflev2_tail_bwd")
+    if sp:
+        sp.end()
+    return dz3, part3, du, partu

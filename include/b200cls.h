@@ -569,6 +569,24 @@ int b200_shuffle_tail_s2_fwd(const void* x, const void* c3, const float* scale, 
 int b200_shuffle_relu_bwd(const void* g, const void* y, const void* c, const float* scale, const float* shift, void* dz,
                           float* partial, void* gx, int B, int Ho, int Wo, int Cin, int Cc, int H, int W, void* stream);
 
+/* ShuffleNet v2 block tails (classification/ShuffleNet/models/shufflenetv2.py InvertedResidual; csrc/shufflenet.cuh):
+ * out = channel_shuffle(cat(u, v), 2), the interleave out[2 i] = u[i], out[2 i + 1] = v[i] (i < b), with
+ * v = relu(c3 * scale + shift) and u the passthrough half (stride 1) or relu(cu * u_scale + u_shift) (stride 2).
+ * u, c3, cu are NHWC bf16 [rows][bp], coefficients fp32 [bp]; channels b .. bp - 1 are padding.  b even >= 2, bp a multiple
+ * of 8 with b <= bp <= 8192, 2 b <= 8192, rows >= 1, every pointer 16-byte aligned; anything else returns B200_EINVAL with a
+ * message and launches nothing.  Every pad channel written is exactly 0; sums are fp32 in a fixed order (no atomics).
+ * shufflev2_tail_fwd: y1 NULL: the joined output y0 [rows][J], J = 2 b rounded up to a multiple of 8; y1 given: the split
+ *             output y0 = out[:b], y1 = out[b:2b], each [rows][bp].  u_scale / u_shift NULL: u is the passthrough
+ * shufflev2_tail_bwd: the output gradient g0 [rows][J] (g1 NULL) or g0 = dL/dy0, g1 = dL/dy1 [rows][bp] (split).  Writes
+ *             dz3 = dL/dv [c3 * scale + shift > 0] and partial3 [b200_repvgg_partial_rows(rows, bp)][2][bp] =
+ *             {sum dz3, sum dz3 c3}; du = dL/du (passthrough: cu, u_scale, u_shift, partial_u NULL) or
+ *             du = dL/du [cu * u_scale + u_shift > 0] with partial_u = {sum du, sum du cu} */
+int b200_shufflev2_tail_fwd(const void* u, const float* u_scale, const float* u_shift, const void* c3, const float* scale,
+                            const float* shift, void* y0, void* y1, long long rows, int b, int bp, void* stream);
+int b200_shufflev2_tail_bwd(const void* g0, const void* g1, const void* c3, const float* scale, const float* shift,
+                            void* dz3, float* partial3, const void* cu, const float* u_scale, const float* u_shift,
+                            void* du, float* partial_u, long long rows, int b, int bp, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,6 +1,6 @@
 """One small launch of every wgmma / TMA kernel family, for `compute-sanitizer --tool {memcheck,racecheck,synccheck}`:
 implicit-GEMM conv (forward + statistics, dgrad + residual, affine / mask epilogues, dual-source K), the streaming 1x1 kernel
-(both modes), wgrad, ViT attention forward / backward, window attention forward / backward, BN-algebra kernels, the VGG passes, the ShuffleNet passes.
+(both modes), wgrad, ViT attention forward / backward, window attention forward / backward, BN-algebra kernels, the VGG passes, the ShuffleNet v1 passes, the ShuffleNet v2 tails.
 usage: compute-sanitizer --tool racecheck python tools/sanitize_ops.py [family ...]"""
 import os
 import sys
@@ -12,7 +12,8 @@ from deeplearning_b200 import ops
 
 dev = torch.device("cuda")
 BF = torch.bfloat16
-fam = set(sys.argv[1:]) or {"conv", "stream", "wgrad", "attn", "attn2", "ln", "wattn", "algebra", "vgg", "shufflenet"}
+fam = set(sys.argv[1:]) or {"conv", "stream", "wgrad", "attn", "attn2", "ln", "wattn", "algebra", "vgg", "shufflenet",
+                               "shufflenetv2"}
 
 
 def r(*shape, scale=1.0):
@@ -126,5 +127,21 @@ if "shufflenet" in fam:
     dz1, _, _ = ops.shuffle_relu_bwd(r(2, 9, 7, 32), c1, y=torch.relu(r(2, 9, 7, 32)))
     dzs, _, _ = ops.shuffle_relu_bwd(r(2, 9, 7, 32), c1, co=co)
     print("shufflenet ok", float(dz.float().abs().mean()), float(gw.abs().mean()), float(gx.float().abs().mean()))
+if "shufflenetv2" in fam:
+    # ShuffleNet v2 tails (shufflenet.cuh shufflev2_tail_*): all four modes at b = 58 (pitch 64, joined pitch 120, the
+    # second half starting at the odd channel 29), forward and backward, joined and split gradients
+    b, bp = 58, 64
+    cos = []
+    for _ in range(2):
+        c = ops.BnCoeffs(bp, dev)
+        c.scale.fill_(1.0), c.shift.fill_(0.1), c.mean.zero_(), c.invstd.fill_(1.0)
+        cos.append(c)
+    c3, u = r(2, 5, 3, bp), r(2, 5, 3, bp)
+    for co_u in (None, cos[1]):
+        for split in (False, True):
+            y = ops.shufflev2_tail_fwd(u, c3, cos[0], b, co_u=co_u, split=split)
+            g = tuple(r(*t.shape) for t in y) if split else r(*y.shape)
+            dz3, _, du, _ = ops.shufflev2_tail_bwd(g, c3, cos[0], b, cu=None if co_u is None else u, co_u=co_u)
+    print("shufflenetv2 ok", float(dz3.float().abs().mean()), float(du.float().abs().mean()))
 torch.cuda.synchronize()
 print("done")
