@@ -170,6 +170,15 @@ SIGNATURES = {
     "b200_vgg_dropout_fwd": (_I, [_P, _P, _P, _L, _P]),
     "b200_vgg_dropout_bwd": (_I, [_P, _P, _F, _P, _L, _P]),
     "b200_adam": (_I, [_P, _P, _P, _P, _L, _P, _F, _F, _F, _F, _F, _P, _P]),
+    "b200_mae_shuffle": (_I, [_P, _P, _P, _I, _I, _P]),
+    "b200_mae_patchify": (_I, [_P, _P, _P, _P] + [_I] * 6 + [_P]),
+    "b200_mae_gather_rows": (_I, [_P, _L, _I, _P, _I, _I, _I, _I, _I, _P, _I, _P]),
+    "b200_mae_assemble_fwd": (_I, [_P] * 5 + [_I] * 4 + [_P]),
+    "b200_mae_assemble_bwd": (_I, [_P] * 4 + [_I] * 4 + [_P]),
+    "b200_mae_pos_grad": (_I, [_P] * 3 + [_I] * 4 + [_P]),
+    "b200_mae_scatter_masked": (_I, [_P] * 3 + [_I] * 4 + [_P]),
+    "b200_mae_mse_blocks": (_I, []),
+    "b200_mae_mse": (_I, [_P, _P, _L, _F, _P, _P, _P, _P]),
 }
 
 

@@ -77,6 +77,12 @@ def _engine_for(model):
         from . import shufflenetv2
 
         return shufflenetv2
+    from ..self_supervised.MAE.models.MAE import MAE
+
+    if isinstance(model, MAE):
+        from . import mae
+
+        return mae
     raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 
@@ -237,6 +243,9 @@ class TrainStep:
         added to the gradient (not AdamW's decoupled decay) - vggNet/train.py:133-136.
         clip_grad: max global L2 norm of the (all-reduced, averaged) gradient, ``clip_grad_norm_`` of the Swin recipe
         (swin_transformer/main.py:197, config TRAIN.CLIP_GRAD = 5.0); the norm of the last step is ``self.grad_norm``.
+        An engine that defines ``train_loss`` (MAE pre-training) computes its own loss and takes no labels (``labels``
+        None); ``correct`` is then None.  Parameters its ``params_without_grad`` lists stay out of the arenas: like torch's
+        optimizers over parameters whose ``.grad`` is None, they get no gradient, optimizer state, decay or all-reduce.
         label_smoothing: LabelSmoothingCrossEntropy of the Swin recipe (main.py:114-115); floating-point ``labels`` of
         shape [B, num_classes] (Mixup / CutMix targets, engine/mixup.py) select SoftTargetCrossEntropy (main.py:111-113).
         accum_steps: gradient accumulation (main.py:190-199, TRAIN.ACCUMULATION_STEPS): every call runs forward + backward of
@@ -249,7 +258,14 @@ class TrainStep:
         if optimizer not in ("sgd", "adamw", "adam"):
             raise ValueError(f"unknown optimizer {optimizer!r}")
         bucket_mb = float(os.environ.get("B200_BUCKET_MB", bucket_mb))   # tuning knob (see DESIGN.md section 5)
-        self.arena = FlatArena(model.parameters(), process_group, world_size, bucket_mb=bucket_mb)
+        params = list(model.parameters())
+        self._pidx = list(range(len(params)))   # model.parameters() index of each arena parameter (optimizer state dicts)
+        no_grad = getattr(self.engine, "params_without_grad", None)
+        if no_grad is not None:
+            skip = {id(p) for p in no_grad(model)}
+            self._pidx = [i for i, p in enumerate(params) if id(p) not in skip and p.requires_grad]
+            params = [params[i] for i in self._pidx]
+        self.arena = FlatArena(params, process_group, world_size, bucket_mb=bucket_mb)
         self.overlap = overlap   # bucketed all-reduce on a side stream during the backward pass (False: one call after it)
         if self.arena.flat_p.device.type != "cuda":
             raise RuntimeError("TrainStep needs the model on a CUDA (sm_90a) device; there is no CPU fallback")
@@ -289,8 +305,13 @@ class TrainStep:
         With gradient accumulation only the ``last`` micro-batch of a group reduces (the sum of the group's gradients)."""
         model, arena = self.model, self.arena
         logits, tape = self.engine.forward(model, images, True, True)
-        loss, dlogits, correct = ops.softmax_xent(logits, labels, want_grad=True, ld_d=padded_classes(logits.shape[1]),
-                                                  label_smoothing=self.label_smoothing, loss_scale=1.0 / self.accum_steps)
+        train_loss = getattr(self.engine, "train_loss", None)
+        if train_loss is not None:
+            loss, dlogits, correct = train_loss(logits, labels, 1.0 / self.accum_steps)
+        else:
+            loss, dlogits, correct = ops.softmax_xent(logits, labels, want_grad=True, ld_d=padded_classes(logits.shape[1]),
+                                                      label_smoothing=self.label_smoothing,
+                                                      loss_scale=1.0 / self.accum_steps)
         if self.accum_steps > 1:
             self.engine.backward(model, tape, dlogits, sink=arena.grad_view)
             if last:
@@ -342,7 +363,7 @@ class TrainStep:
     def _hyper_lr(self):
         return getattr(self, "_hyper_lr_value", self.lr)
 
-    def step_eager(self, images, labels, lr=None):
+    def step_eager(self, images, labels=None, lr=None):
         if not self.model.training:
             self.model.train()
         last = self._micro + 1 == self.accum_steps
@@ -354,7 +375,7 @@ class TrainStep:
         return loss, correct
 
     # ------------------------------------------------------------------------------------------------ CUDA-graph step
-    def capture(self, images, labels):
+    def capture(self, images, labels=None):
         """Capture fwd + loss + bwd + gradient all-reduce + update into ONE CUDA graph with static input buffers of the given
         shapes (world > 1: the NCCL collectives of the gradient buckets are graph nodes on a side stream)."""
         if not self.model.training:
@@ -362,9 +383,10 @@ class TrainStep:
         dev = self.arena.flat_p.device
         # (a decoded uint8 NHWC batch stays uint8: ToTensor + Normalize run inside the step, see ops.stem_s2d_u8)
         self._g_images = torch.empty_like(images, dtype=torch.uint8 if images.dtype == torch.uint8 else torch.float32, device=dev)
-        self._g_labels = torch.empty_like(labels, device=dev)
+        self._g_labels = None if labels is None else torch.empty_like(labels, device=dev)
         self._g_images.copy_(images)
-        self._g_labels.copy_(labels)
+        if labels is not None:
+            self._g_labels.copy_(labels)
         self._lr_dev = torch.full((1,), float(self.lr), dtype=torch.float32, device=dev)
         # The warm-up below runs two real steps (first-launch attribute calls, allocator growth).  They must not perturb
         # the caller's model: parameters, optimizer state, AdamW step counters and every buffer (BatchNorm running
@@ -411,17 +433,19 @@ class TrainStep:
         with torch.cuda.graph(self._graph_fb, capture_error_mode="thread_local"):
             self._g_loss, self._g_correct = self._fwd_bwd(self._g_images, self._g_labels, True)
             self._update(self.lr, self._lr_dev)
-        self._captured_shape = (tuple(images.shape), tuple(labels.shape))
+        self._captured_shape = (tuple(images.shape), None if labels is None else tuple(labels.shape))
         return self
 
-    def step(self, images, labels, lr=None):
-        """One training step on this rank's shard. Returns (loss [1] fp32 device tensor, correct int32 [B]).
-        Replays the captured graphs when ``capture()`` was called with matching shapes, else runs eagerly."""
-        if getattr(self, "_graph_fb", None) is None or (tuple(images.shape), tuple(labels.shape)) != self._captured_shape:
+    def step(self, images, labels=None, lr=None):
+        """One training step on this rank's shard. Returns (loss [1] fp32 device tensor, correct int32 [B], or None for a
+        model trained without labels).  Replays the captured graphs when ``capture()`` was called with matching shapes,
+        else runs eagerly."""
+        shapes = (tuple(images.shape), None if labels is None else tuple(labels.shape))
+        if getattr(self, "_graph_fb", None) is None or shapes != self._captured_shape:
             return self.step_eager(images, labels, lr)
         if images.data_ptr() != self._g_images.data_ptr():
             self._g_images.copy_(images, non_blocking=True)
-        if labels.data_ptr() != self._g_labels.data_ptr():
+        if labels is not None and labels.data_ptr() != self._g_labels.data_ptr():
             self._g_labels.copy_(labels, non_blocking=True)
         if lr is not None and lr != self.lr:
             self.lr = lr
@@ -451,7 +475,7 @@ class TrainStep:
         arena = self.arena
         state = {}
         decay, nodecay = [], []
-        for i, (prm, o) in enumerate(zip(arena.params, arena.offsets)):
+        for i, prm, o in zip(self._pidx, arena.params, arena.offsets):
             n = prm.numel()
             if self.optimizer == "sgd":
                 if self.steps > 0:
@@ -464,10 +488,10 @@ class TrainStep:
                     (decay if float(arena.flat_wd[o]) != 0.0 else nodecay).append(i)
         if self.optimizer == "sgd":
             groups = [{"lr": self.lr, "momentum": self.momentum, "dampening": 0, "weight_decay": self.weight_decay,
-                       "nesterov": False, "params": list(range(len(arena.params)))}]
+                       "nesterov": False, "params": list(self._pidx)}]
         elif self.optimizer == "adam":
             groups = [{"lr": self._hyper_lr(), "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay,
-                       "amsgrad": False, "params": list(range(len(arena.params)))}]
+                       "amsgrad": False, "params": list(self._pidx)}]
         else:
             base = {"lr": self._hyper_lr(), "betas": tuple(self.betas), "eps": self.eps, "amsgrad": False}
             groups = [dict(base, weight_decay=self.weight_decay, params=decay), dict(base, weight_decay=0.0, params=nodecay)]
@@ -482,8 +506,12 @@ class TrainStep:
             arena.flat_m.zero_()
             if hasattr(arena, "flat_v"):
                 arena.flat_v.zero_()
+            slot_of = {pi: k for k, pi in enumerate(self._pidx)}
             for i, st in sd["state"].items():
-                o, prm = arena.offsets[int(i)], arena.params[int(i)]
+                if int(i) not in slot_of:
+                    continue   # a parameter kept out of the arena (no gradient, so no state to resume)
+                k = slot_of[int(i)]
+                o, prm = arena.offsets[k], arena.params[k]
                 n = prm.numel()
                 if self.optimizer == "sgd":
                     if st.get("momentum_buffer") is not None:

@@ -3,7 +3,7 @@
 Mirrors ``VisionTransformer.forward_features`` / ``Block.forward`` / ``Attention.forward`` / ``Mlp.forward`` of the
 reference (classification/vision_transformer/vit_model.py:240-268, :158-161, :88-111, :127-133).
 
-Data flow per block (residual stream ``h`` fp32 [B,T,D], everything feeding a tensor core bf16):
+Data flow per block (residual stream ``h`` fp32 [B,T,D], everything feeding a tensor core bf16; engine/prenorm_block.py):
     LN1(h) -> qkv GEMM(+bias) -> wgmma attention -> proj GEMM(+bias, +h, fp32 out) = h2
     LN2(h2) -> fc1 GEMM(+bias, GELU; also writes GELU'(pre) for the backward) -> fc2 GEMM(+bias, +h2, fp32 out) = h3
 Residual adds, biases, GELU, GELU' (backward) and the pos-embed add of the patch embedding all live in GEMM epilogues; the
@@ -16,7 +16,7 @@ import torch
 import torch.nn as nn
 
 from .. import ops
-from . import common, droppath
+from . import common, droppath, prenorm_block
 from .common import linear_grads, layernorm_backward
 from .packing import weight_cache
 
@@ -100,22 +100,10 @@ def forward(model, x, train, want_tape):
         tape["patches"] = a
     for blk in model.blocks:
         att_m, mlp = blk.attn, blk.mlp
-        H = att_m.num_heads
-        y1, m1, r1 = ops.layernorm_fwd(h, blk.norm1.weight, blk.norm1.bias, blk.norm1.eps)
-        qkv, _ = ops.gemm(y1, pack.get(att_m.qkv.weight, 0), bias=att_m.qkv.bias)
-        att, lse = ops.attention_fwd(qkv, H, float(att_m.scale))
-        dp = droppath.drop_prob_of(blk, train)
-        dp1 = droppath.sample_scale(dp, B, 3, x.device)     # x = x + drop_path(attn(norm1(x)))   (vit_model.py:159)
-        h2, _ = ops.gemm(att, pack.get(att_m.proj.weight, 0), bias=att_m.proj.bias, residual=h, out_f32=True,
-                         rowscale=None if dp1 is None else (dp1, T))
-        y2, m2, r2 = ops.layernorm_fwd(h2, blk.norm2.weight, blk.norm2.bias, blk.norm2.eps)
-        post, dact = ops.gemm(y2, pack.get(mlp.fc1.weight, 0), bias=mlp.fc1.bias, act=2, aux_out=want_tape)
-        dp2 = droppath.sample_scale(dp, B, 3, x.device)     # x = x + drop_path(mlp(norm2(x)))    (vit_model.py:160)
-        h3, _ = ops.gemm(post, pack.get(mlp.fc2.weight, 0), bias=mlp.fc2.bias, residual=h2, out_f32=True,
-                         rowscale=None if dp2 is None else (dp2, T))
+        h, rec = prenorm_block.forward(pack, h, blk.norm1, att_m.qkv, att_m.proj, blk.norm2, mlp.fc1, mlp.fc2,
+                                       att_m.num_heads, float(att_m.scale), droppath.drop_prob_of(blk, train), want_tape)
         if want_tape:
-            tape["blocks"].append((blk, h, y1, m1, r1, qkv, att, lse, h2, y2, m2, r2, dact, post, dp1, dp2))
-        h = h3
+            tape["blocks"].append(rec)
     # ---- head: final LayerNorm on the class-token rows only, then the classifier (fp32 logits)
     cls_rows = torch.empty(B, D, dtype=F32, device=x.device)
     ops.copy_rows(h, 0, T * D, cls_rows, 0, D, B, D)
@@ -144,28 +132,8 @@ def backward(model, tape, dlogits, sink=None):
     d_cls = layernorm_backward(grads, model.norm, d_yc, cls_rows, mc, rc)
     g = torch.zeros(B, T, D, dtype=BF16, device=d_cls.device)   # gradient of the residual stream
     ops.copy_rows(d_cls, 0, D, g, 0, T * D, B, D)
-    M = B * T
-    for (blk, h, y1, m1, r1, qkv, att, lse, h2, y2, m2, r2, dact, post, dp1, dp2) in reversed(tape["blocks"]):
-        att_m, mlp = blk.attn, blk.mlp
-        H = att_m.num_heads
-        # (stochastic depth: the branch sees the per-sample scaled gradient, the identity path - `add=g` below - the full one)
-        g2 = (g if dp2 is None else ops.rowscale(g, dp2)).view(M, D)
-        # h3 = h2 + fc2(gelu(fc1(LN2(h2))))
-        linear_grads(grads, mlp.fc2, g2, post.view(M, -1))
-        # dgrad + GELU' in the epilogue, which also sums the columns of d_pre (= fc1 bias gradient) on the way out
-        d_pre, _, st_pre = ops.gemm(g2, pack.get(mlp.fc2.weight, 1), act=3, aux_in=dact.view(M, -1), want_stats=True)
-        linear_grads(grads, mlp.fc1, d_pre, y2.view(M, D), dy_stats=st_pre)
-        d_y2, _ = ops.gemm(d_pre, pack.get(mlp.fc1.weight, 1))
-        g = layernorm_backward(grads, blk.norm2, d_y2, h2, m2, r2, add=g)
-        # h2 = h + proj(attention(qkv(LN1(h))))
-        g2 = (g if dp1 is None else ops.rowscale(g, dp1)).view(M, D)
-        linear_grads(grads, att_m.proj, g2, att.view(M, D))
-        d_att, _ = ops.gemm(g2, pack.get(att_m.proj.weight, 1))
-        dqkv = ops.attention_bwd(qkv, att, d_att.view(B, T, D), lse, H, float(att_m.scale))
-        linear_grads(grads, att_m.qkv, dqkv.view(M, 3 * D), y1.view(M, D))
-        d_y1, _ = ops.gemm(dqkv.view(M, 3 * D), pack.get(att_m.qkv.weight, 1))
-        g = layernorm_backward(grads, blk.norm1, d_y1, h, m1, r1, add=g)
-        g = g.view(B, T, D)
+    for rec in reversed(tape["blocks"]):
+        g = prenorm_block.backward(grads, pack, rec, g)
     # ---- embedding: tokens = [cls ; patches W^T + b] + pos
     grads.put(model.pos_embed, ops.batch_rowsum(g, T * D, B, T * D, out=_flat(grads.dest(model.pos_embed))))
     grads.put(model.cls_token, ops.batch_rowsum(g, T * D, B, D, out=_flat(grads.dest(model.cls_token))))

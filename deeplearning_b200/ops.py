@@ -2011,3 +2011,120 @@ def shufflev2_tail_bwd(g, c3, co, b, cu=None, co_u=None):
     if sp:
         sp.end()
     return dz3, part3, du, partu
+
+
+# --------------------------------------------------------------------------------------------------------- MAE pieces
+I32 = torch.int32
+
+
+def mae_shuffle(keys):
+    """fp32 keys [B, P] -> (ids int32 [B, P], slot int32 [B, P]): ids = keys.argsort(dim=1, stable=True), slot its inverse."""
+    lib = _lib.load()
+    keys = keys.contiguous()
+    B, P = keys.shape
+    ids = torch.empty(B, P, dtype=I32, device=keys.device)
+    slot = torch.empty(B, P, dtype=I32, device=keys.device)
+    _lib.check(lib.b200_mae_shuffle(_p(keys), _p(ids), _p(slot), B, P, _stream()), "b200_mae_shuffle")
+    return ids, slot
+
+
+def mae_patchify(x, ids, p, Nm):
+    """fp32 NCHW x -> (vis bf16 [B, P - Nm, p*p*C], tgt fp32 [B, Nm, p*p*C]): (p1, p2, c)-ordered patch vectors in shuffle order."""
+    lib = _lib.load()
+    B, C, H, W = x.shape
+    P = ids.shape[1]
+    K = p * p * C
+    vis = torch.empty(B, P - Nm, K, dtype=BF16, device=x.device)
+    tgt = torch.empty(B, Nm, K, dtype=F32, device=x.device)
+    sp = _span("mae_patchify", 0.0, _nb(x, vis, tgt))
+    _lib.check(lib.b200_mae_patchify(_p(x), _p(ids), _p(vis), _p(tgt), B, C, H, W, p, Nm, _stream()), "b200_mae_patchify")
+    if sp:
+        sp.end()
+    return vis, tgt
+
+
+def mae_gather_rows(src, ids, s0, n, rows_per_sample, row_offset=0, out_dtype=F32):
+    """[B, n, D] rows src[b * rows_per_sample + ids[b, s0 + j] + row_offset] of the fp32 row matrix src (rows_per_sample 0:
+    one table shared by every sample)."""
+    lib = _lib.load()
+    B, P = ids.shape
+    D = src.shape[-1]
+    out = torch.empty(B, n, D, dtype=out_dtype, device=src.device)
+    rc = lib.b200_mae_gather_rows(_p(src), rows_per_sample, row_offset, _p(ids), B, P, s0, n, D, _p(out),
+                                  1 if out_dtype == F32 else 0, _stream())
+    _lib.check(rc, "b200_mae_gather_rows")
+    return out
+
+
+def mae_assemble_fwd(enc, mask_embed, dpos, slot, Nm):
+    """Decoder input fp32 [B, P, D] in patch order from the encoder rows fp32 [B, P - Nm, D] (shuffle order), the mask token
+    and the decoder position table fp32 [P, D]."""
+    lib = _lib.load()
+    B, P = slot.shape
+    D = enc.shape[-1]
+    dec = torch.empty(B, P, D, dtype=F32, device=enc.device)
+    sp = _span("mae_assemble_fwd", 0.0, _nb(enc, dec))
+    rc = lib.b200_mae_assemble_fwd(_p(enc), _p(mask_embed), _p(dpos), _p(slot), _p(dec), B, P, Nm, D, _stream())
+    _lib.check(rc, "b200_mae_assemble_fwd")
+    if sp:
+        sp.end()
+    return dec
+
+
+def mae_assemble_bwd(g, slot, Nm, d_dpos=None):
+    """g bf16 [B, P, D] (gradient of the decoder input) -> (encoder-row gradient bf16 [B, P - Nm, D], d_dpos fp32 [P, D])."""
+    lib = _lib.load()
+    B, P = slot.shape
+    D = g.shape[-1]
+    g_enc = torch.empty(B, P - Nm, D, dtype=BF16, device=g.device)
+    if d_dpos is None:
+        d_dpos = torch.empty(P, D, dtype=F32, device=g.device)
+    sp = _span("mae_assemble_bwd", 0.0, _nb(g, g_enc, d_dpos))
+    rc = lib.b200_mae_assemble_bwd(_p(g), _p(slot), _p(g_enc), _p(d_dpos), B, P, Nm, D, _stream())
+    _lib.check(rc, "b200_mae_assemble_bwd")
+    if sp:
+        sp.end()
+    return g_enc, d_dpos
+
+
+def mae_pos_grad(g, slot, Nm, out=None):
+    """Gradient fp32 [P + 1, D] of the encoder pos_embed from the encoder-input gradient bf16 [B, P - Nm, D]; row 0 is 0."""
+    lib = _lib.load()
+    B, P = slot.shape
+    D = g.shape[-1]
+    if out is None:
+        out = torch.empty(P + 1, D, dtype=F32, device=g.device)
+    _lib.check(lib.b200_mae_pos_grad(_p(g), _p(slot), _p(out), B, P, Nm, D, _stream()), "b200_mae_pos_grad")
+    return out
+
+
+def mae_scatter_masked(dh, slot, Nm):
+    """bf16 [B, P, D]: the rows dh bf16 [B, Nm, D] at their masked patch, zero elsewhere."""
+    lib = _lib.load()
+    B, P = slot.shape
+    D = dh.shape[-1]
+    g = torch.empty(B, P, D, dtype=BF16, device=dh.device)
+    sp = _span("mae_scatter_masked", 0.0, _nb(dh, g))
+    _lib.check(lib.b200_mae_scatter_masked(_p(dh), _p(slot), _p(g), B, P, Nm, D, _stream()), "b200_mae_scatter_masked")
+    if sp:
+        sp.end()
+    return g
+
+
+def mae_mse(pred, target, loss_scale=1.0):
+    """(loss fp32 [1] = mean((pred - target)^2), gradient bf16 of pred = loss_scale * 2 (pred - target) / numel).
+    loss_scale multiplies the gradient only (1 / accumulation steps), as in softmax_xent."""
+    lib = _lib.load()
+    if pred.shape != target.shape or pred.dtype != F32 or target.dtype != F32:
+        raise ValueError("mae_mse: pred and target must be fp32 tensors of one shape")
+    pred, target = pred.contiguous(), target.contiguous()
+    n = pred.numel()
+    grad = torch.empty(pred.shape, dtype=BF16, device=pred.device)
+    partial = torch.empty(lib.b200_mae_mse_blocks(), dtype=F32, device=pred.device)
+    loss = torch.empty(1, dtype=F32, device=pred.device)
+    sp = _span("mae_mse", 3.0 * n, _nb(pred, target, grad))
+    rc = lib.b200_mae_mse(_p(pred), _p(target), n, 2.0 * float(loss_scale) / n, _p(grad), _p(partial), _p(loss), _stream())
+    _lib.check(rc, "b200_mae_mse")
+    if sp:
+        sp.end()
+    return loss, grad

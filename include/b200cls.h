@@ -587,6 +587,38 @@ int b200_shufflev2_tail_bwd(const void* g0, const void* g1, const void* c3, cons
                             void* dz3, float* partial3, const void* cu, const float* u_scale, const float* u_shift,
                             void* du, float* partial_u, long long rows, int b, int bp, void* stream);
 
+/* Masked-autoencoder passes (self-supervised/MAE/models/MAE.py MAE.forward; csrc/mae.cuh).  Per sample b of P patches with
+ * Nm masked ones (1 <= Nm < P <= 1024, B <= 65535): ids [B][P] int32 is the shuffle order (slots [0, Nm) masked, [Nm, P)
+ * visible, Nv = P - Nm) and slot [B][P] int32 its inverse.  Every output element is written once and every sum runs in a
+ * fixed order (no atomics); invalid shapes or null pointers return B200_EINVAL with a message and launch nothing.
+ * mae_shuffle:      ids = stable argsort of each row of keys fp32 [B][P] (ties -> lower index), slot = its inverse
+ * mae_patchify:     x fp32 NCHW [B][C][H][W], P = (H / p) (W / p): patch vectors in (p1, p2, c) order, in shuffle order:
+ *                   vis bf16 [B Nv][p p C] (visible slots), tgt fp32 [B Nm][p p C] (masked slots)
+ * mae_gather_rows:  dst[b n + j] = src[b src_rows_per_sample + ids[b][s0 + j] + row_offset] (fp32 rows of width D;
+ *                   dst fp32 when dst_f32, else bf16)
+ * mae_assemble_fwd: dec fp32 [B][P][D]: mask_embed + dpos[n] for a masked patch n, else enc fp32 [B Nv][D] at its slot
+ * mae_assemble_bwd: from g bf16 [B][P][D]: g_enc bf16 [B Nv][D] (visible rows at their slot) and d_dpos fp32 [P][D] =
+ *                   per-patch sums over the batch (ascending b) of the masked rows
+ * mae_pos_grad:     d_pos fp32 [P + 1][D]: row n + 1 = sum over the batch (ascending b) of g bf16 [B Nv][D] at the slot of
+ *                   patch n when visible; row 0 = 0
+ * mae_scatter_masked: g bf16 [B][P][D] = dh bf16 [B Nm][D] at the slot of each masked patch, 0 on visible patches
+ * mae_mse:          loss fp32 [1] = mean((pred - target)^2) over n values, grad bf16 [n] = grad_scale (pred - target);
+ *                   partial fp32 [b200_mae_mse_blocks()] scratch */
+int b200_mae_shuffle(const float* keys, int* ids, int* slot, int B, int P, void* stream);
+int b200_mae_patchify(const float* x, const int* ids, void* vis, float* tgt, int B, int C, int H, int W, int p, int Nm,
+                      void* stream);
+int b200_mae_gather_rows(const float* src, long long src_rows_per_sample, int row_offset, const int* ids, int B, int P,
+                         int s0, int n, int D, void* dst, int dst_f32, void* stream);
+int b200_mae_assemble_fwd(const float* enc, const float* mask_embed, const float* dpos, const int* slot, float* dec, int B,
+                          int P, int Nm, int D, void* stream);
+int b200_mae_assemble_bwd(const void* g, const int* slot, void* g_enc, float* d_dpos, int B, int P, int Nm, int D,
+                          void* stream);
+int b200_mae_pos_grad(const void* g, const int* slot, float* d_pos, int B, int P, int Nm, int D, void* stream);
+int b200_mae_scatter_masked(const void* dh, const int* slot, void* g, int B, int P, int Nm, int D, void* stream);
+int b200_mae_mse_blocks(void);
+int b200_mae_mse(const float* pred, const float* target, long long n, float grad_scale, void* grad, float* partial,
+                 float* loss, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
