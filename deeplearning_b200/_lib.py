@@ -179,6 +179,12 @@ SIGNATURES = {
     "b200_mae_scatter_masked": (_I, [_P] * 3 + [_I] * 4 + [_P]),
     "b200_mae_mse_blocks": (_I, []),
     "b200_mae_mse": (_I, [_P, _P, _L, _F, _P, _P, _P, _P]),
+    "b200_supcon_max_dim": (_I, []),
+    "b200_supcon_normalize_fwd": (_I, [_P, _P, _P, _I, _I, _P]),
+    "b200_supcon_normalize_bwd": (_I, [_P] * 4 + [_I, _I, _P]),
+    "b200_supcon_loss_fwd": (_I, [_P, _P, _I, _I, _F, _F, _P, _P, _P, _P, _P]),
+    "b200_supcon_loss_bwd": (_I, [_P] * 5 + [_F, _I, _I, _F, _F, _P, _P]),
+    "b200_supcon_relu_bwd": (_I, [_P, _P, _P, _L, _P]),
 }
 
 

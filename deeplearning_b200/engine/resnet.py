@@ -66,6 +66,26 @@ def _check_bn(bn, name):
                                   f"statistics (got {bn})")
 
 
+def conv_pack_specs(net, stem):
+    """Forward [O][taps*I] and dgrad [I][taps*O] bf16 operands of every convolution of ``net``; ``stem`` (the 7x7/2 stem
+    convolution) gets the space-to-depth operand instead."""
+    specs = []
+    for mod in net.modules():
+        if isinstance(mod, nn.Conv2d):
+            w = mod.weight
+            O, I, kh, kw = w.shape
+            if mod is stem:
+                specs.append((w, 2, 256, O, (O, I, kh * kw)))  # space-to-depth stem operand [64][256]
+                continue
+            if mod.groups != 1:   # block-diagonal operands of a grouped 3x3 convolution
+                specs.append((w, 3, kh * kw * 64, O))
+                specs.append((w, 4, kh * kw * 64, O))
+                continue
+            specs.append((w, 0, kh * kw * I, O))
+            specs.append((w, 1, kh * kw * O, I))
+    return specs
+
+
 class _PackSpec:
     """Which bf16 operands a ResNet needs: forward [O][taps*I] and dgrad [I][taps*O] copies of every conv / fc weight."""
 
@@ -74,21 +94,7 @@ class _PackSpec:
         return (model.fc.out_features, id(model.fc))
 
     def __call__(self, model):
-        specs = []
-        for name, mod in model.named_modules():
-            if isinstance(mod, nn.Conv2d):
-                w = mod.weight
-                O, I, kh, kw = w.shape
-                if name == "conv1":
-                    specs.append((w, 2, 256, O, (O, I, kh * kw)))  # space-to-depth stem operand [64][256]
-                    continue
-                if mod.groups != 1:   # block-diagonal operands of a grouped 3x3 convolution
-                    specs.append((w, 3, kh * kw * 64, O))
-                    specs.append((w, 4, kh * kw * 64, O))
-                    continue
-                specs.append((w, 0, kh * kw * I, O))
-                specs.append((w, 1, kh * kw * O, I))
-        return specs + common.head_pack_specs(model.fc)
+        return conv_pack_specs(model, model.conv1) + common.head_pack_specs(model.fc)
 
 
 _pack_spec = _PackSpec()
@@ -236,33 +242,59 @@ def _block_units(block):
     return [(block.conv1, block.bn1), (block.conv2, block.bn2)]
 
 
-def forward(model, x, train, want_tape):
-    """x: fp32 NCHW CUDA batch. Returns (logits fp32 [B, num_classes], tape or None)."""
+class Trunk:
+    """Stem, stem BatchNorm and residual stages of a ResNet under the names its state_dict uses: the ResNet module itself
+    (conv1, bn1, layer1 .. layer4), or the ``nn.Sequential`` of its children without ``fc`` that a SupCon encoder is
+    (self-supervised/SupCon/models/model.py create_encoder: 0 = conv1, 1 = bn1, 2 = relu, 3 = maxpool, 4 .. 7 = layer1 ..
+    layer4, 8 = avgpool).  ``prefix`` is the module's own name in error messages ("" for a ResNet)."""
+    __slots__ = ("conv1", "bn1", "layers", "stem_name", "bn1_name", "layer_names")
+
+    def __init__(self, net, prefix=""):
+        if isinstance(net, nn.Sequential):
+            kinds = (nn.Conv2d, nn.Module, nn.ReLU, nn.MaxPool2d, nn.Sequential, nn.Sequential, nn.Sequential, nn.Sequential,
+                     nn.AdaptiveAvgPool2d)
+            if len(net) != len(kinds) or not all(isinstance(m, k) for m, k in zip(net, kinds)):
+                raise NotImplementedError(f"{prefix}: the GPU engine runs a ResNet trunk as the Sequential (conv1, bn1, relu, "
+                                          f"maxpool, layer1 .. layer4, avgpool) of a ResNet's children without fc")
+            self.conv1, self.bn1, self.layers = net[0], net[1], [net[i] for i in range(4, 8)]
+            self.stem_name, self.bn1_name = f"{prefix}.0", f"{prefix}.1"
+            self.layer_names = [f"{prefix}.{i}" for i in range(4, 8)]
+        else:
+            self.conv1, self.bn1 = net.conv1, net.bn1
+            self.layers = [getattr(net, f"layer{li}") for li in range(1, 5)]
+            self.stem_name, self.bn1_name = "stem", "bn1"
+            self.layer_names = [f"layer{li}" for li in range(1, 5)]
+
+
+def image_batch(x):
+    """(x, (H, W), u8) of an image batch: an fp32 NCHW batch, or a decoded uint8 NHWC batch of the GPU input pipeline."""
     u8 = x.dtype == torch.uint8     # GPU input pipeline: decoded uint8 NHWC batch, ToTensor + Normalize fused into the stem operand
     if u8:
         if x.dim() != 4 or x.shape[3] != 3:
             raise ValueError(f"uint8 input must be a decoded NHWC batch [B,H,W,3], got {tuple(x.shape)}")
         x = x.contiguous()
-        x_hw = (x.shape[1], x.shape[2])
-    else:
-        if x.dim() != 4 or x.shape[1] != 3:
-            raise ValueError(f"expected an [B,3,H,W] image batch, got {tuple(x.shape)}")
-        x = x.contiguous().float()
-        x_hw = (x.shape[2], x.shape[3])
+        return x, (x.shape[1], x.shape[2]), True
+    if x.dim() != 4 or x.shape[1] != 3:
+        raise ValueError(f"expected an [B,3,H,W] image batch, got {tuple(x.shape)}")
+    x = x.contiguous().float()
+    return x, (x.shape[2], x.shape[3]), False
+
+
+def trunk_forward(trunk, pack, x, x_hw, u8, train, want_tape, input_norm):
+    """Stem through layer4 and the global average pool of ``trunk`` (a Trunk) on a batch from image_batch.
+    Returns (pooled bf16 [B, F], tape or None).  ``train`` without ``want_tape`` runs train-mode BatchNorm (batch statistics,
+    running statistics updated) and records nothing: the frozen encoder of SupCon's second stage."""
     B = x.shape[0]
-    if not isinstance(model.fc, nn.Linear):
-        raise NotImplementedError("model.fc must be an nn.Linear")
-    pack = weight_cache.model_pack(model, _pack_spec)  # one launch repacks every bf16 operand if parameters changed
     tape = {"stem": None, "blocks": [], "head": None, "pack": pack} if want_tape else None
     # ---- stem: 7x7/2 conv as a space-to-depth implicit GEMM, BN statistics in the epilogue, BN+ReLU+max-pool in one pass
-    conv1, bn1 = model.conv1, model.bn1
-    _check_bn(bn1, "bn1")
+    conv1, bn1 = trunk.conv1, trunk.bn1
+    _check_bn(bn1, trunk.bn1_name)
     if conv1.kernel_size != (7, 7) or conv1.stride != (2, 2) or conv1.padding != (3, 3) or conv1.bias is not None:
-        raise NotImplementedError("stem must be the 7x7/2 pad-3 bias-free convolution of the reference")
+        raise NotImplementedError(f"{trunk.stem_name} must be the 7x7/2 pad-3 bias-free convolution of the reference")
     if conv1.out_channels != 64 or x_hw[0] % 2 or x_hw[1] % 2:
-        raise NotImplementedError("stem: 64 output channels and an even input size are required")
+        raise NotImplementedError(f"{trunk.stem_name}: 64 output channels and an even input size are required")
     # space-to-depth operand (108 MB at bs 256 instead of a 1 GB patch matrix); the conv reads it through overlapping TMA rows
-    a = ops.stem_s2d_u8(x, *getattr(model, "input_norm", (ops.IMAGENET_MEAN, ops.IMAGENET_STD))) if u8 else ops.stem_s2d(x)
+    a = ops.stem_s2d_u8(x, *input_norm) if u8 else ops.stem_s2d(x)
     Ho, Wo = a.shape[1] - 3, a.shape[2] - 3
     c1, st = ops.stem_s2d_conv_fwd(a, pack.get(conv1.weight, 2), want_stats=train)
     co1 = common.bn_coeffs(bn1, st, B * Ho * Wo, train)
@@ -270,10 +302,10 @@ def forward(model, x, train, want_tape):
     if want_tape:
         tape["stem"] = (a, c1, co1, idx, (Ho, Wo))
     # ---- residual stages
-    for li in range(1, 5):
-        for bi, block in enumerate(getattr(model, f"layer{li}")):
+    for layer, lname in zip(trunk.layers, trunk.layer_names):
+        for bi, block in enumerate(layer):
             units = [] if want_tape else None
-            name = f"layer{li}.{bi}"
+            name = f"{lname}.{bi}"
             x_in = h
             pairs = _block_units(block)
             for j, (conv, bn) in enumerate(pairs[:-1]):
@@ -298,11 +330,23 @@ def forward(model, x, train, want_tape):
                 h = _conv_bn(pack, units, h, conv, bn, train, relu=True, residual=identity, name=f"{name}.conv{len(pairs)}")
             if want_tape:
                 tape["blocks"].append((units, ds_units[0] if ds_units else None, x_in))
-    # ---- head: global average pool + fc (fp32 logits)
+    # ---- global average pool (bf16 features)
     pooled = ops.avgpool_fwd(h)
-    logits = common.head_forward(pack, model.fc, pooled)
     if want_tape:
         tape["head"] = (pooled, h.shape[1:3])
+    return pooled, tape
+
+
+def forward(model, x, train, want_tape):
+    """x: fp32 NCHW CUDA batch. Returns (logits fp32 [B, num_classes], tape or None)."""
+    x, x_hw, u8 = image_batch(x)
+    if not isinstance(model.fc, nn.Linear):
+        raise NotImplementedError("model.fc must be an nn.Linear")
+    pack = weight_cache.model_pack(model, _pack_spec)  # one launch repacks every bf16 operand if parameters changed
+    pooled, tape = trunk_forward(Trunk(model), pack, x, x_hw, u8, train, want_tape,
+                                 getattr(model, "input_norm", (ops.IMAGENET_MEAN, ops.IMAGENET_STD)))
+    # ---- head: fc (fp32 logits)
+    logits = common.head_forward(pack, model.fc, pooled)
     return logits, tape
 
 
@@ -355,9 +399,18 @@ def backward(model, tape, dlogits, sink=None):
     """dlogits: fp32 [B, num_classes] (or the bf16 [B, n_pad] product of ops.softmax_xent).
     Returns {parameter.data_ptr(): fp32 gradient}; with ``sink`` the gradients are written into caller-owned buffers."""
     grads = common.Grads(sink)
-    pooled, hw = tape["head"]
+    pooled, _ = tape["head"]
+    dpooled = common.head_backward(grads, tape["pack"], model.fc, pooled, dlogits)
+    trunk_backward(Trunk(model), tape, dpooled, grads)
+    return grads
+
+
+def trunk_backward(trunk, tape, dpooled, grads):
+    """Backward of trunk_forward for the gradient dpooled bf16 [B, F] of the pooled features; records every trunk
+    parameter's gradient in ``grads`` (common.Grads)."""
+    _, hw = tape["head"]
     pack = tape["pack"]
-    g = ops.avgpool_bwd(common.head_backward(grads, pack, model.fc, pooled, dlogits), hw)
+    g = ops.avgpool_bwd(dpooled, hw)
 
     # The gradient of a block output travels either as the raw gradient ``g`` (then the block masks it itself) or, when the
     # consumer's conv1 dgrad epilogue already applied this block's ReLU mask, as ``dz`` with its partial column sums.
@@ -432,12 +485,12 @@ def backward(model, tape, dlogits, sink=None):
 
     a, c1, co1, idx, (Ho, Wo) = tape["stem"]
     g_act = ops.maxpool_bwd(g, idx, (Ho, Wo))
-    dc, dgamma, dbeta, _ = ops.bn_backward(g_act, c1, co1, relu=True, sync=common.bn_sync(model.bn1), dgamma=grads.dest(model.bn1.weight),
-                                           dbeta=grads.dest(model.bn1.bias))
-    grads.put(model.bn1.weight, dgamma)
-    grads.put(model.bn1.bias, dbeta)
-    grads.put(model.conv1.weight, ops.stem_s2d_conv_wgrad(dc, a, out=grads.dest(model.conv1.weight)))
-    return grads
+    bn1, conv1 = trunk.bn1, trunk.conv1
+    dc, dgamma, dbeta, _ = ops.bn_backward(g_act, c1, co1, relu=True, sync=common.bn_sync(bn1), dgamma=grads.dest(bn1.weight),
+                                           dbeta=grads.dest(bn1.bias))
+    grads.put(bn1.weight, dgamma)
+    grads.put(bn1.bias, dbeta)
+    grads.put(conv1.weight, ops.stem_s2d_conv_wgrad(dc, a, out=grads.dest(conv1.weight)))
 
 
 def apply(model, x):

@@ -83,6 +83,12 @@ def _engine_for(model):
         from . import mae
 
         return mae
+    from ..self_supervised.SupCon.models.model import SupConModel
+
+    if isinstance(model, SupConModel):
+        from . import supcon
+
+        return supcon
     raise NotImplementedError(f"no GPU engine schedule for {type(model).__name__}")
 
 
@@ -235,7 +241,7 @@ class _GradSink:
 class TrainStep:
     def __init__(self, model, lr=0.01, momentum=0.9, weight_decay=5e-5, process_group=None, world_size=None,
                  broadcast=True, optimizer="sgd", betas=(0.9, 0.999), eps=1e-8, no_decay=None, clip_grad=None,
-                 overlap=True, bucket_mb=25.0, label_smoothing=0.0, accum_steps=1):
+                 overlap=True, bucket_mb=25.0, label_smoothing=0.0, accum_steps=1, criterion=None):
         """optimizer="sgd": torch.optim.SGD(momentum, weight_decay on every parameter) - resnet/vit train.py:96,94.
         optimizer="adamw": torch.optim.AdamW(betas, eps, weight_decay) with the reference's decay / no-decay groups
         (``no_decay(name, param) -> bool``, default ``no_decay_rule``) - convNext/train.py:96,102.
@@ -250,9 +256,18 @@ class TrainStep:
         shape [B, num_classes] (Mixup / CutMix targets, engine/mixup.py) select SoftTargetCrossEntropy (main.py:111-113).
         accum_steps: gradient accumulation (main.py:190-199, TRAIN.ACCUMULATION_STEPS): every call runs forward + backward of
         one micro-batch with the loss gradient scaled by 1/accum_steps; the all-reduce, clipping and the optimizer update
-        happen on every accum_steps-th call."""
+        happen on every accum_steps-th call.
+        criterion: the loss module of an engine that takes one (``check_criterion``), whose ``train_loss`` reads its
+        hyper-parameters: SupConLoss for a first-stage SupConModel (``step(cat(view1, view2), labels or None)``),
+        LabelSmoothingLoss for a second-stage one.  Any other engine takes None."""
         self.model = model
         self.engine = _engine_for(model)
+        check_criterion = getattr(self.engine, "check_criterion", None)
+        if check_criterion is not None:
+            check_criterion(model, criterion)
+        elif criterion is not None:
+            raise ValueError(f"{type(model).__name__} takes no criterion; its engine computes the recipe's loss")
+        self.criterion = criterion
         self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
         self.optimizer, self.betas, self.eps = optimizer, betas, eps
         if optimizer not in ("sgd", "adamw", "adam"):
@@ -306,7 +321,9 @@ class TrainStep:
         model, arena = self.model, self.arena
         logits, tape = self.engine.forward(model, images, True, True)
         train_loss = getattr(self.engine, "train_loss", None)
-        if train_loss is not None:
+        if train_loss is not None and hasattr(self.engine, "check_criterion"):
+            loss, dlogits, correct = train_loss(logits, labels, 1.0 / self.accum_steps, self.criterion)
+        elif train_loss is not None:
             loss, dlogits, correct = train_loss(logits, labels, 1.0 / self.accum_steps)
         else:
             loss, dlogits, correct = ops.softmax_xent(logits, labels, want_grad=True, ld_d=padded_classes(logits.shape[1]),

@@ -273,6 +273,11 @@ _ws_cache = {}
 
 
 def _workspace(nbytes, device):
+    """Scratch of at least ``nbytes`` for the current stream.  Inside a CUDA-graph capture it is a fresh allocation from the
+    graph's private pool: a cached buffer could be replaced (freed) by a larger request later in the same capture or in
+    another graph captured on the same stream, while the graph that recorded its address is still replayed."""
+    if torch.cuda.is_current_stream_capturing():
+        return torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8, device=device)
     key = (device, torch.cuda.current_stream().cuda_stream)
     ws = _ws_cache.get(key)
     if ws is None or ws.numel() < nbytes:
@@ -2128,3 +2133,98 @@ def mae_mse(pred, target, loss_scale=1.0):
     if sp:
         sp.end()
     return loss, grad
+
+
+# --------------------------------------------------------------------------------------------------------- SupCon pieces
+def supcon_max_dim():
+    """Widest embedding row the SupCon loss kernels take."""
+    return int(_lib.load().b200_supcon_max_dim())
+
+
+def _supcon_rows(t, name, max_dim):
+    if t.dim() != 2 or t.dtype != F32:
+        raise ValueError(f"{name}: expected an fp32 [N, D] tensor, got {t.dtype} {tuple(t.shape)}")
+    N, D = t.shape
+    if D % 4 or D > max_dim:
+        raise NotImplementedError(f"{name}: rows of width {D}; the SupCon kernels take widths that are multiples of 4 up to "
+                                  f"{max_dim}")
+    if not t.is_cuda:
+        raise ValueError(f"{name}: expected a CUDA tensor, got one on {t.device}")
+    return t.contiguous(), N, D
+
+
+def supcon_normalize(z):
+    """(e fp32 [N, D] = F.normalize(z, dim=1), norms fp32 [N]) of fp32 rows z [N, D]."""
+    lib = _lib.load()
+    z, N, D = _supcon_rows(z, "supcon_normalize", 1 << 16)
+    e = torch.empty_like(z)
+    nrm = torch.empty(N, dtype=F32, device=z.device)
+    sp = _span("supcon_normalize", 3.0 * N * D, _nb(z, e))
+    _lib.check(lib.b200_supcon_normalize_fwd(_p(z), _p(e), _p(nrm), N, D, _stream()), "b200_supcon_normalize_fwd")
+    if sp:
+        sp.end()
+    return e, nrm
+
+
+def supcon_normalize_bwd(de, e, nrm):
+    """bf16 gradient [N, D] of the rows z from the gradient de fp32 [N, D] of e = F.normalize(z, dim=1)."""
+    lib = _lib.load()
+    de, N, D = _supcon_rows(de, "supcon_normalize_bwd", 1 << 16)
+    if e.shape != de.shape or nrm.shape != (N,):
+        raise ValueError("supcon_normalize_bwd: de, e [N, D] and norms [N] must match")
+    dz = torch.empty(N, D, dtype=BF16, device=de.device)
+    sp = _span("supcon_normalize_bwd", 4.0 * N * D, _nb(de, e, dz))
+    _lib.check(lib.b200_supcon_normalize_bwd(_p(de), _p(e.contiguous()), _p(nrm), _p(dz), N, D, _stream()),
+               "b200_supcon_normalize_bwd")
+    if sp:
+        sp.end()
+    return dz
+
+
+def supcon_loss(e, labels, temperature, base_temperature):
+    """SupCon loss over the fp32 rows e [N, D] with int32 row labels [N]: (loss fp32 [1], L fp32 [N], npos fp32 [N]); L and
+    npos (the log-sum-exp and positive count of every anchor) are what supcon_loss_bwd needs."""
+    lib = _lib.load()
+    e, N, D = _supcon_rows(e, "supcon_loss", supcon_max_dim())
+    if labels.dtype != I32 or labels.shape != (N,) or not labels.is_contiguous():
+        raise ValueError(f"supcon_loss: labels must be a contiguous int32 [{N}] tensor")
+    L = torch.empty(N, dtype=F32, device=e.device)
+    npos = torch.empty(N, dtype=F32, device=e.device)
+    rows = torch.empty(N, dtype=F32, device=e.device)
+    loss = torch.empty(1, dtype=F32, device=e.device)
+    sp = _span("supcon_loss", 2.0 * N * N * D, _nb(e))
+    rc = lib.b200_supcon_loss_fwd(_p(e), _p(labels), N, D, float(temperature), float(base_temperature), _p(L), _p(npos),
+                                  _p(rows), _p(loss), _stream())
+    _lib.check(rc, "b200_supcon_loss_fwd")
+    if sp:
+        sp.end()
+    return loss, L, npos
+
+
+def supcon_loss_bwd(e, labels, L, npos, grad_out, temperature, base_temperature, grad_scale=1.0):
+    """fp32 gradient [N, D] of grad_scale * grad_out * loss with respect to e; grad_out is a device scalar read by the
+    kernel (no host synchronisation), L / npos come from supcon_loss."""
+    lib = _lib.load()
+    e, N, D = _supcon_rows(e, "supcon_loss_bwd", supcon_max_dim())
+    if grad_out.dtype != F32 or grad_out.numel() != 1 or not grad_out.is_cuda:
+        raise ValueError("supcon_loss_bwd: grad_out must be a one-element CUDA fp32 tensor")
+    de = torch.empty_like(e)
+    sp = _span("supcon_loss_bwd", 4.0 * N * N * D, _nb(e, de))
+    rc = lib.b200_supcon_loss_bwd(_p(e), _p(labels), _p(L), _p(npos), _p(grad_out.contiguous()), float(grad_scale), N, D,
+                                  float(temperature), float(base_temperature), _p(de), _stream())
+    _lib.check(rc, "b200_supcon_loss_bwd")
+    if sp:
+        sp.end()
+    return de
+
+
+def relu_bwd(dy, y):
+    """bf16 dy masked by the bf16 ReLU output y (dy where y > 0, else 0)."""
+    lib = _lib.load()
+    _chk_act(dy, "relu_bwd dy")
+    _chk_act(y, "relu_bwd y")
+    if dy.shape != y.shape:
+        raise ValueError("relu_bwd: dy and y must have one shape")
+    dx = torch.empty_like(dy)
+    _lib.check(lib.b200_supcon_relu_bwd(_p(dy), _p(y), _p(dx), dy.numel(), _stream()), "b200_supcon_relu_bwd")
+    return dx

@@ -619,6 +619,29 @@ int b200_mae_mse_blocks(void);
 int b200_mae_mse(const float* pred, const float* target, long long n, float grad_scale, void* grad, float* partial,
                  float* loss, void* stream);
 
+/* Supervised contrastive learning passes (self-supervised/SupCon: models/model.py SupConModel, losses/SupConLoss.py;
+ * csrc/supcon.cuh).  Rows are fp32 [N][D] with D a multiple of 4 and N * D < 2^31; every output element is written once
+ * and every sum runs in a fixed order (no atomics); invalid shapes or null pointers return B200_EINVAL with a message and
+ * launch nothing.
+ * supcon_normalize_fwd: e = z / max(||z||, 1e-12) per row, nrm fp32 [N] = ||z||  (D <= 65536)
+ * supcon_normalize_bwd: dz bf16 [N][D] = (de - e (e . de)) / ||z||, or de / 1e-12 where the clamp was active
+ * supcon_loss_fwd:  e fp32 [N][D] (D <= b200_supcon_max_dim()), labels int32 [N]; with l_ij = e_i . e_j / temperature,
+ *                   P_i = {j != i : labels_j == labels_i}, L_i = log sum_{j != i} exp l_ij (running maximum):
+ *                   L fp32 [N], npos fp32 [N] = |P_i|, row_loss fp32 [N] = -(temperature / base_temperature)
+ *                   (sum_{j in P_i} l_ij / |P_i| - L_i), loss fp32 [1] = mean of row_loss (NaN for an anchor without a
+ *                   positive)
+ * supcon_loss_bwd:  de fp32 [N][D] = d (grad_out[0] grad_scale loss) / de from the forward's L and npos; grad_out is a
+ *                   device scalar (the upstream gradient, read by the kernel)
+ * supcon_relu_bwd:  dx bf16 [n] = dy where the ReLU output y bf16 [n] is > 0, else 0 */
+int b200_supcon_max_dim(void);
+int b200_supcon_normalize_fwd(const float* z, float* e, float* nrm, int N, int D, void* stream);
+int b200_supcon_normalize_bwd(const float* de, const float* e, const float* nrm, void* dz, int N, int D, void* stream);
+int b200_supcon_loss_fwd(const float* e, const int* labels, int N, int D, float temperature, float base_temperature,
+                         float* L, float* npos, float* row_loss, float* loss, void* stream);
+int b200_supcon_loss_bwd(const float* e, const int* labels, const float* L, const float* npos, const float* grad_out,
+                         float grad_scale, int N, int D, float temperature, float base_temperature, float* de, void* stream);
+int b200_supcon_relu_bwd(const void* dy, const void* y, void* dx, long long n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
