@@ -233,8 +233,7 @@ int launch_conv_gemm_epi(const ConvGemmParams& q, int grid, cudaStream_t st) {
                                          Cfg::SMEM_BYTES));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(conv_gemm_kernel<BLOCK_N, EPI>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, q));
-  B200_LAUNCHED();
+  B200_LAUNCH(conv_gemm_kernel<BLOCK_N, EPI>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, q);
   return OK;
 }
 
@@ -293,8 +292,7 @@ int launch_tap64(const ConvGemmParams& q, int grid, cudaStream_t st) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(conv_tap64_kernel<kStats>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTap64SmemBytes));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(conv_tap64_kernel<kStats>, dim3(grid), dim3(384), kTap64SmemBytes, st, q));
-  B200_LAUNCHED();
+  B200_LAUNCH(conv_tap64_kernel<kStats>, dim3(grid), dim3(384), kTap64SmemBytes, st, q);
   return OK;
 }
 
@@ -342,8 +340,7 @@ int launch_stream(const StreamParams& q, int grid, cudaStream_t st) {
                                          Cfg::SMEM_BYTES));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(conv1x1_stream_kernel<KB, MODE>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, q));
-  B200_LAUNCHED();
+  B200_LAUNCH(conv1x1_stream_kernel<KB, MODE>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, q);
   return OK;
 }
 
@@ -402,12 +399,11 @@ int launch_wgrad(const WgradParams& p, cudaStream_t st) {
   q.desc_sbo = kWgDescSbo;
   q.desc_kstep = kWgDescKstep;
   if constexpr (kGrouped)
-    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, false, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
+    B200_LAUNCH(wgrad_gemm_kernel<BLOCK_NG, false, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q);
   else if (q.bias_partial != nullptr)   // + four warps that sum the dY tiles' columns (the layer's bias gradient)
-    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
+    B200_LAUNCH(wgrad_gemm_kernel<BLOCK_NG, true>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q);
   else
-    B200_CHECK_CUDA(launch_pdl(wgrad_gemm_kernel<BLOCK_NG, false>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q));
-  B200_LAUNCHED();
+    B200_LAUNCH(wgrad_gemm_kernel<BLOCK_NG, false>, dim3(grid), dim3(kWgradThreads), Cfg::SMEM_BYTES, st, q);
   return OK;
 }
 
@@ -423,13 +419,13 @@ int launch_wgrad_reduce(const float* partial, float* dw, int splits, int Cout, i
     const size_t smem = static_cast<size_t>(SL) * taps * chunk * sizeof(float);
     if (smem <= 48 * 1024 && Cout <= 65535 * 32) {
       dim3 grid(Cout, (Cin + chunk - 1) / chunk);
-      B200_CHECK_CUDA(launch_pdl(wgrad_reduce_rows_kernel, dim3(grid), dim3(256), smem, st, partial, dw, splits, Cout, Cin, taps, chunk, SL, accumulate, bias_partial, bias_out));
+      B200_LAUNCH(wgrad_reduce_rows_kernel, dim3(grid), dim3(256), smem, st, partial, dw, splits, Cout, Cin, taps, chunk, SL, accumulate, bias_partial, bias_out);
       return OK;
     }
   }
   int blocks = static_cast<int>((total + 255) / 256);
   if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
-  B200_CHECK_CUDA(launch_pdl(wgrad_reduce_flat_kernel, dim3(blocks), dim3(256), 0, st, partial, dw, splits, Cout, Cin, taps, accumulate, bias_partial, bias_out));
+  B200_LAUNCH(wgrad_reduce_flat_kernel, dim3(blocks), dim3(256), 0, st, partial, dw, splits, Cout, Cin, taps, accumulate, bias_partial, bias_out);
   return OK;
 }
 
@@ -799,7 +795,6 @@ int b200_conv2d_wgrad(const void* dy, const void* x, float* dw, void* workspace,
     rc = launch_wgrad<256>(p, st);
   if (rc) return rc;
   if ((rc = launch_wgrad_reduce(p.partial, dw, pl.splits, Cout, Cin, pl.taps, accumulate, st, bias_partial, bias_out))) return rc;
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -846,7 +841,6 @@ int b200_stem_s2d_conv_wgrad(const void* dy, const void* z, float* g, void* work
   if ((rc = launch_wgrad<256>(p, st))) return rc;  // merged-tap mode: the four y-taps are the four 64-column atoms
   // g[cout][k64][ky] (the generic "OIHW" layout of a 64-channel, 4-tap conv); b200_stem_s2d_wgrad_relayout maps it to [64,3,7,7]
   if ((rc = launch_wgrad_reduce(p.partial, g, pl.splits, Cout, Cin, taps, 0, st))) return rc;
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -1019,9 +1013,8 @@ int b200_conv2d_grouped_wgrad(const void* dy, const void* x, float* dw, void* wo
   const long long total = static_cast<long long>(C) * (C / groups) * pl.taps;
   int blocks = static_cast<int>((total + 255) / 256);
   if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
-  B200_CHECK_CUDA(launch_pdl(wgrad_reduce_grouped_kernel, dim3(blocks), dim3(256), 0, st, static_cast<const float*>(p.partial),
-                             dw, pl.splits, C, C / groups, pl.taps, accumulate));
-  B200_LAUNCHED();
+  B200_LAUNCH(wgrad_reduce_grouped_kernel, dim3(blocks), dim3(256), 0, st, static_cast<const float*>(p.partial),
+              dw, pl.splits, C, C / groups, pl.taps, accumulate);
   return OK;
 }
 

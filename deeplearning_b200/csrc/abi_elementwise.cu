@@ -10,15 +10,7 @@
 using namespace b200;
 
 namespace {
-inline int ew_grid(long long work_items, int block = 256) {
-  long long blocks = (work_items + block - 1) / block;
-  const long long cap = static_cast<long long>(device_sm_count()) * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<int>(blocks);
-}
 inline bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
-inline bool aligned16(const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 inline int reduce_slices(int T) {
   int s = T / 64;
   if (s < 1) s = 1;
@@ -59,18 +51,16 @@ int b200_bn_finalize(const float* partial, int T, int C, double count, const flo
   B200_REQUIRE(T > 0 && C > 0 && count > 0, "bn_finalize: bad sizes T=%d C=%d", T, C);
   B200_REQUIRE(C <= 256 * 32, "bn_finalize: C=%d exceeds 8192", C);
   B200_REQUIRE(scratch != nullptr && scratch_bytes >= b200_reduce_scratch_bytes(T, C), "bn_finalize: scratch too small");
-  B200_CHECK_CUDA(launch_pdl(bn_finalize_kernel, dim3(dim3((C + 31) / 32, reduce_slices(T))), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+  B200_LAUNCH(bn_finalize_kernel, dim3(dim3((C + 31) / 32, reduce_slices(T))), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       partial, T, C, count, gamma, beta, eps, momentum, running_mean, running_var, num_batches_tracked, mean, invstd,
-      scale, shift, scratch));
-  B200_LAUNCHED();
+      scale, shift, scratch);
   return OK;
 }
 
 int b200_bn_eval_coeffs(int C, const float* gamma, const float* beta, const float* running_mean,
                         const float* running_var, float eps, float* scale, float* shift, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(bn_eval_coeffs_kernel, dim3((C + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), C, gamma, beta, running_mean,
-                                                                                       running_var, eps, scale, shift));
-  B200_LAUNCHED();
+  B200_LAUNCH(bn_eval_coeffs_kernel, dim3((C + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), C, gamma, beta, running_mean,
+                                                                                       running_var, eps, scale, shift);
   return OK;
 }
 
@@ -78,15 +68,17 @@ int b200_bn_apply(const void* x, const void* residual, void* y, const float* sca
                   int C, int relu, void* stream) {
   B200_REQUIRE(C % 8 == 0, "bn_apply: C=%d must be a multiple of 8", C);
   const long long nvec = rows * (C / 8);
-  B200_CHECK_CUDA(launch_pdl(bn_apply_kernel, dim3(ew_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+  B200_LAUNCH(bn_apply_kernel, dim3(capped_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(x), static_cast<const uint4*>(residual), static_cast<uint4*>(y), scale, shift, nvec,
-      C / 8, relu));
-  B200_LAUNCHED();
+      C / 8, relu);
   return OK;
 }
 
 int b200_bn_bwd_blocks(long long rows, int C) {
-  if (C % 8 != 0 || !pow2(C / 8) || C / 8 > 256) return -1;
+  if (C % 8 != 0 || !pow2(C / 8) || C / 8 > 256) {
+    set_error("bn_bwd_blocks: C=%d must be 8*2^k <= 2048", C);
+    return -1;
+  }
   return plan_bn_bwd(rows, C).blocks;
 }
 
@@ -94,10 +86,9 @@ int b200_bn_bwd_reduce(const void* g, const void* x, const void* y_out, void* dz
                        const float* shift, int relu, long long rows, int C, float* partial, void* stream) {
   B200_REQUIRE(C % 8 == 0 && pow2(C / 8) && C / 8 <= 256, "bn_bwd_reduce: C=%d must be 8*2^k <= 2048", C);
   const BnBwdPlan pl = plan_bn_bwd(rows, C);
-  B200_CHECK_CUDA(launch_pdl(bn_bwd_reduce_kernel, dim3(pl.blocks), dim3(256), 256 * 17 * sizeof(float), static_cast<cudaStream_t>(stream), 
+  B200_LAUNCH(bn_bwd_reduce_kernel, dim3(pl.blocks), dim3(256), 256 * 17 * sizeof(float), static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(g), static_cast<const uint4*>(x), static_cast<const uint4*>(y_out),
-      static_cast<uint4*>(dz_out), scale, shift, relu, rows, C / 8, pl.rows_per_block, partial));
-  B200_LAUNCHED();
+      static_cast<uint4*>(dz_out), scale, shift, relu, rows, C / 8, pl.rows_per_block, partial);
   return OK;
 }
 
@@ -106,9 +97,8 @@ int b200_bn_bwd_finalize(const float* partial, int T, int C, double count, float
                          size_t scratch_bytes, void* stream) {
   B200_REQUIRE(T > 0 && C > 0 && C <= 256 * 32, "bn_bwd_finalize: bad sizes T=%d C=%d", T, C);
   B200_REQUIRE(scratch != nullptr && scratch_bytes >= b200_reduce_scratch_bytes(T, C), "bn_bwd_finalize: scratch too small");
-  B200_CHECK_CUDA(launch_pdl(bn_bwd_finalize_kernel, dim3(dim3((C + 31) / 32, reduce_slices(T))), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      partial, T, C, count, dgamma, dbeta, accumulate, m1, m2, mean, invstd, scratch));
-  B200_LAUNCHED();
+  B200_LAUNCH(bn_bwd_finalize_kernel, dim3(dim3((C + 31) / 32, reduce_slices(T))), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      partial, T, C, count, dgamma, dbeta, accumulate, m1, m2, mean, invstd, scratch);
   return OK;
 }
 
@@ -123,11 +113,10 @@ int b200_bn_bwd_apply(const void* g, const void* x, const void* y_out, int g_is_
                "bn_bwd_apply: g, x, dx, scale, shift, mean, invstd, m1, m2 (and y_out) must be non-null and 16-byte "
                "aligned");
   const RvGeom gm = repvgg_geom(rows, C);
-  B200_CHECK_CUDA(launch_pdl(bn_bwd_apply_kernel, dim3(gm.blocks, gm.nchunk), dim3(256), 0,
+  B200_LAUNCH(bn_bwd_apply_kernel, dim3(gm.blocks, gm.nchunk), dim3(256), 0,
       static_cast<cudaStream_t>(stream), static_cast<const uint4*>(g), static_cast<const uint4*>(x),
       static_cast<const uint4*>(y_out), g_is_dz, static_cast<uint4*>(dx), scale, shift, mean, invstd, m1, m2, relu, rows,
-      C / 8, gm.rows_per_block, gm.gpc));
-  B200_LAUNCHED();
+      C / 8, gm.rows_per_block, gm.gpc);
   return OK;
 }
 
@@ -137,10 +126,9 @@ int b200_bn_relu_maxpool_fwd(const void* x, void* y, void* idx, const float* sca
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   const long long nvec = static_cast<long long>(B) * Ho * Wo * (C / 8);
   B200_REQUIRE(static_cast<long long>(B) * H * W * (C / 8) < (1LL << 32), "maxpool: tensor too large");
-  B200_CHECK_CUDA(launch_pdl(bn_relu_maxpool_fwd_kernel, dim3(ew_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+  B200_LAUNCH(bn_relu_maxpool_fwd_kernel, dim3(capped_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(x), static_cast<uint4*>(y), static_cast<unsigned long long*>(idx), scale, shift, B, H, W,
-      C / 8));
-  B200_LAUNCHED();
+      C / 8);
   return OK;
 }
 
@@ -148,37 +136,33 @@ int b200_maxpool_bwd(const void* g_out, const void* idx, void* g_in, int B, int 
   B200_REQUIRE(C % 8 == 0, "maxpool_bwd: C=%d must be a multiple of 8", C);
   B200_REQUIRE(static_cast<long long>(B) * H * W * (C / 8) < (1LL << 32), "maxpool_bwd: tensor too large");
   const long long nvec = static_cast<long long>(B) * ((H - 1) / 2 + 1) * ((W - 1) / 2 + 1) * (C / 8);   // 2x2 input blocks
-  B200_CHECK_CUDA(launch_pdl(maxpool_bwd_kernel, dim3(ew_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+  B200_LAUNCH(maxpool_bwd_kernel, dim3(capped_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(g_out), static_cast<const unsigned long long*>(idx), static_cast<uint4*>(g_in), B, H, W,
-      C / 8));
-  B200_LAUNCHED();
+      C / 8);
   return OK;
 }
 
 int b200_avgpool_fwd(const void* x, void* y, int B, int HW, int C, void* stream) {
   B200_REQUIRE(C % 8 == 0, "avgpool: C=%d must be a multiple of 8", C);
   const long long nvec = static_cast<long long>(B) * (C / 8);
-  B200_CHECK_CUDA(launch_pdl(avgpool_fwd_kernel, dim3(ew_grid(nvec, 128)), dim3(128), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint4*>(x), static_cast<uint4*>(y), B, HW, C / 8));
-  B200_LAUNCHED();
+  B200_LAUNCH(avgpool_fwd_kernel, dim3(capped_grid(nvec, 128)), dim3(128), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const uint4*>(x), static_cast<uint4*>(y), B, HW, C / 8);
   return OK;
 }
 int b200_avgpool_bwd(const void* gy, void* gx, int B, int HW, int C, void* stream) {
   B200_REQUIRE(C % 8 == 0, "avgpool_bwd: C=%d must be a multiple of 8", C);
   const long long nvec = static_cast<long long>(B) * HW * (C / 8);
-  B200_CHECK_CUDA(launch_pdl(avgpool_bwd_kernel, dim3(ew_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint4*>(gy), static_cast<uint4*>(gx), B, HW, C / 8));
-  B200_LAUNCHED();
+  B200_LAUNCH(avgpool_bwd_kernel, dim3(capped_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const uint4*>(gy), static_cast<uint4*>(gx), B, HW, C / 8);
   return OK;
 }
 
 int b200_softmax_xent(const float* logits, long long ld, const long long* labels, int B, int N, float gscale,
                       float* loss_rows, void* dlogits, long long ld_d, int* correct, void* stream) {
   B200_REQUIRE(B > 0 && N > 0, "softmax_xent: empty input");
-  B200_CHECK_CUDA(launch_pdl(softmax_xent_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+  B200_LAUNCH(softmax_xent_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream), 
       logits, ld, labels, N, gscale, loss_rows, static_cast<__nv_bfloat16*>(dlogits), ld_d, correct,
-      static_cast<const float*>(nullptr), 0ll, 0.f));
-  B200_LAUNCHED();
+      static_cast<const float*>(nullptr), 0ll, 0.f);
   return OK;
 }
 
@@ -188,23 +172,20 @@ int b200_softmax_xent_soft(const float* logits, long long ld, const long long* l
   B200_REQUIRE(B > 0 && N > 0, "softmax_xent_soft: empty input");
   B200_REQUIRE(soft_targets != nullptr || labels != nullptr, "softmax_xent_soft: soft targets or labels are required");
   B200_REQUIRE(smoothing >= 0.f && smoothing < 1.f, "softmax_xent_soft: smoothing %f outside [0, 1)", smoothing);
-  B200_CHECK_CUDA(launch_pdl(softmax_xent_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream),
+  B200_LAUNCH(softmax_xent_kernel, dim3(B), dim3(256), 0, static_cast<cudaStream_t>(stream),
       logits, ld, labels, N, gscale, loss_rows, static_cast<__nv_bfloat16*>(dlogits), ld_d, correct, soft_targets, ld_soft,
-      smoothing));
-  B200_LAUNCHED();
+      smoothing);
   return OK;
 }
 
 int b200_mean(const float* v, int n, float* out, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(mean_kernel, dim3(1), dim3(256), 0, static_cast<cudaStream_t>(stream), v, n, out));
-  B200_LAUNCHED();
+  B200_LAUNCH(mean_kernel, dim3(1), dim3(256), 0, static_cast<cudaStream_t>(stream), v, n, out);
   return OK;
 }
 
 int b200_colsum_bf16(const void* m, long long rows, long long ld, int cols, float* out, int accumulate, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(colsum_kernel, dim3((cols + 63) / 64), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const __nv_bfloat16*>(m), rows, ld, cols, out, accumulate));
-  B200_LAUNCHED();
+  B200_LAUNCH(colsum_kernel, dim3((cols + 63) / 64), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const __nv_bfloat16*>(m), rows, ld, cols, out, accumulate);
   return OK;
 }
 
@@ -215,30 +196,26 @@ int b200_pack_weight(const float* src, void* dst, int O, int I, int taps, int mo
   const long long rows = mode == 1 ? I : O;
   const long long need = static_cast<long long>(taps) * (mode == 0 ? I : (mode == 1 ? O : 64));
   B200_REQUIRE(ld_dst >= need, "pack_weight: ld_dst %lld < %lld", ld_dst, need);
-  B200_CHECK_CUDA(launch_pdl(pack_weight_kernel, dim3(ew_grid(rows * ld_dst)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      src, static_cast<__nv_bfloat16*>(dst), O, I, taps, mode, ld_dst));
-  B200_LAUNCHED();
+  B200_LAUNCH(pack_weight_kernel, dim3(capped_grid(rows * ld_dst)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      src, static_cast<__nv_bfloat16*>(dst), O, I, taps, mode, ld_dst);
   return OK;
 }
 
 int b200_pack_weights_multi(const void* table, int n_entries, int total_blocks, void* stream) {
   B200_REQUIRE(table != nullptr && n_entries > 0 && total_blocks > 0, "pack_weights_multi: empty table");
-  B200_CHECK_CUDA(launch_pdl(pack_weights_multi_kernel, dim3(total_blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const long long*>(table), n_entries));
-  B200_LAUNCHED();
+  B200_LAUNCH(pack_weights_multi_kernel, dim3(total_blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const long long*>(table), n_entries);
   return OK;
 }
 
 int b200_cast_f32_to_bf16(const float* src, void* dst, long long n, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(cast_f32_bf16_kernel, dim3(ew_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), src, static_cast<__nv_bfloat16*>(dst),
-                                                                                  n));
-  B200_LAUNCHED();
+  B200_LAUNCH(cast_f32_bf16_kernel, dim3(capped_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), src, static_cast<__nv_bfloat16*>(dst),
+                                                                                  n);
   return OK;
 }
 int b200_cast_bf16_to_f32(const void* src, float* dst, long long n, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(cast_bf16_f32_kernel, dim3(ew_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const __nv_bfloat16*>(src), dst, n));
-  B200_LAUNCHED();
+  B200_LAUNCH(cast_bf16_f32_kernel, dim3(capped_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const __nv_bfloat16*>(src), dst, n);
   return OK;
 }
 
@@ -251,40 +228,35 @@ int b200_im2col_nchw(const float* x, void* a, int B, int Cin, int H, int W, int 
   B200_REQUIRE(smem <= 48 * 1024, "im2col: staged rows need %zu bytes of shared memory (> 48 KB)", smem);
   const int threads = (ldk / 8) * (256 / (ldk / 8) > 0 ? 256 / (ldk / 8) : 1);  // a multiple of the k-octet count
   B200_REQUIRE(ldk / 8 <= 256, "im2col: ldk=%d too large", ldk);
-  B200_CHECK_CUDA(launch_pdl(im2col_nchw_kernel, dim3(B * Ho), dim3(threads), smem, static_cast<cudaStream_t>(stream), x, static_cast<uint4*>(a), B, Cin, H, W,
-                                                                               KH, KW, stride, pad, Ho, Wo, ldk));
-  B200_LAUNCHED();
+  B200_LAUNCH(im2col_nchw_kernel, dim3(B * Ho), dim3(threads), smem, static_cast<cudaStream_t>(stream), x, static_cast<uint4*>(a), B, Cin, H, W,
+                                                                               KH, KW, stride, pad, Ho, Wo, ldk);
   return OK;
 }
 
 int b200_stem_wgrad_relayout(const float* src, float* dst, int Cout, int Cin, int taps, int ldk, int accumulate,
                               void* stream) {
   const long long total = static_cast<long long>(Cout) * Cin * taps;
-  B200_CHECK_CUDA(launch_pdl(stem_wgrad_relayout_kernel, dim3(ew_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), src, dst, Cout, Cin, taps,
-                                                                                            ldk, accumulate));
-  B200_LAUNCHED();
+  B200_LAUNCH(stem_wgrad_relayout_kernel, dim3(capped_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), src, dst, Cout, Cin, taps,
+                                                                                            ldk, accumulate);
   return OK;
 }
 
 int b200_sgd_momentum(float* p, const float* g, float* buf, long long n, float lr, const float* lr_dev, float momentum,
                       float weight_decay, float gscale, int first_step, const float* clip_coef, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(sgd_momentum_kernel, dim3(ew_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), p, g, buf, n, lr, lr_dev, momentum,
-                                                                               weight_decay, gscale, first_step, clip_coef));
-  B200_LAUNCHED();
+  B200_LAUNCH(sgd_momentum_kernel, dim3(capped_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), p, g, buf, n, lr, lr_dev, momentum,
+                                                                               weight_decay, gscale, first_step, clip_coef);
   return OK;
 }
 
 int b200_stem_s2d(const float* x, void* z, int B, int H, int W, void* stream) {
   B200_REQUIRE(B > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "stem_s2d: H=%d W=%d must be even", H, W);
   const long long total = static_cast<long long>(B) * (H / 2 + 3) * (W / 2 + 3);
-  B200_CHECK_CUDA(launch_pdl(stem_s2d_kernel, dim3(ew_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), x, static_cast<uint4*>(z), B, H, W));
-  B200_LAUNCHED();
+  B200_LAUNCH(stem_s2d_kernel, dim3(capped_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), x, static_cast<uint4*>(z), B, H, W);
   return OK;
 }
 
 int b200_stem_s2d_wgrad_relayout(const float* g, float* dw, int accumulate, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(stem_s2d_wgrad_relayout_kernel, dim3((64 * 3 * 49 + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), g, dw, accumulate));
-  B200_LAUNCHED();
+  B200_LAUNCH(stem_s2d_wgrad_relayout_kernel, dim3((64 * 3 * 49 + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), g, dw, accumulate);
   return OK;
 }
 
@@ -293,24 +265,21 @@ int b200_rowscale_bf16(const void* x, const float* scale, void* y, long long n_s
   B200_REQUIRE(n_samples > 0 && elems_per_sample > 0 && elems_per_sample % 8 == 0,
                "rowscale_bf16: elems_per_sample=%lld must be a positive multiple of 8", elems_per_sample);
   const long long nvec = n_samples * (elems_per_sample / 8);
-  B200_CHECK_CUDA(launch_pdl(rowscale_bf16_kernel, dim3(ew_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint4*>(x), scale, static_cast<uint4*>(y), nvec, elems_per_sample / 8));
-  B200_LAUNCHED();
+  B200_LAUNCH(rowscale_bf16_kernel, dim3(capped_grid(nvec)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const uint4*>(x), scale, static_cast<uint4*>(y), nvec, elems_per_sample / 8);
   return OK;
 }
 
 int b200_tanh_fwd(const float* u, float* t, void* t_bf16, long long n, void* stream) {
   B200_REQUIRE(n > 0, "tanh_fwd: empty input");
-  B200_CHECK_CUDA(launch_pdl(tanh_fwd_kernel, dim3(ew_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), u, t, static_cast<__nv_bfloat16*>(t_bf16), n));
-  B200_LAUNCHED();
+  B200_LAUNCH(tanh_fwd_kernel, dim3(capped_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), u, t, static_cast<__nv_bfloat16*>(t_bf16), n);
   return OK;
 }
 
 int b200_tanh_bwd(const void* dt_bf16, const float* t, void* du_bf16, long long n, void* stream) {
   B200_REQUIRE(n > 0, "tanh_bwd: empty input");
-  B200_CHECK_CUDA(launch_pdl(tanh_bwd_kernel, dim3(ew_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const __nv_bfloat16*>(dt_bf16), t, static_cast<__nv_bfloat16*>(du_bf16), n));
-  B200_LAUNCHED();
+  B200_LAUNCH(tanh_bwd_kernel, dim3(capped_grid(n)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const __nv_bfloat16*>(dt_bf16), t, static_cast<__nv_bfloat16*>(du_bf16), n);
   return OK;
 }
 
@@ -325,10 +294,9 @@ int b200_bn_gram_stats(const float* G, const float* s, const void* w_bf16, int N
     B200_CHECK_CUDA(cudaFuncSetAttribute(bn_conv1x1_bwd_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 40 * 256 * 4));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(bn_gram_stats_kernel, dim3((N + 7) / 8), dim3(256), smem, static_cast<cudaStream_t>(stream), 
+  B200_LAUNCH(bn_gram_stats_kernel, dim3((N + 7) / 8), dim3(256), smem, static_cast<cudaStream_t>(stream), 
       G, s, static_cast<const __nv_bfloat16*>(w_bf16), N, K, count, gamma, beta, eps, momentum, running_mean, running_var,
-      num_batches_tracked, mean, invstd, scale, shift));
-  B200_LAUNCHED();
+      num_batches_tracked, mean, invstd, scale, shift);
   return OK;
 }
 
@@ -353,14 +321,12 @@ int b200_bn_conv1x1_bwd(const float* dz_partial, int T, const float* D, const fl
   }
   float2* coef = static_cast<float2*>(scratch);
   float* partial = reinterpret_cast<float*>(static_cast<char*>(scratch) + static_cast<size_t>(2) * N * sizeof(float));
-  B200_CHECK_CUDA(launch_pdl(bn_conv1x1_bwd_rows_kernel, dim3((N + 7) / 8), dim3(256), static_cast<size_t>(32 + 8) * K * sizeof(float), st, 
+  B200_LAUNCH(bn_conv1x1_bwd_rows_kernel, dim3((N + 7) / 8), dim3(256), static_cast<size_t>(32 + 8) * K * sizeof(float), st, 
       dz_partial, T, D, G, s, static_cast<const __nv_bfloat16*>(w_bf16), w_f32, N, K, count, gamma, mean, invstd, dgamma, dbeta,
-      dW, accumulate, static_cast<__nv_bfloat16*>(wcat), coef));
-  B200_LAUNCHED();
-  B200_CHECK_CUDA(launch_pdl(bn_conv1x1_bwd_m_kernel, dim3(dim3(K / 32, K / 32, kAlgebraSlices)), dim3(256), 0, st, 
+      dW, accumulate, static_cast<__nv_bfloat16*>(wcat), coef);
+  B200_LAUNCH(bn_conv1x1_bwd_m_kernel, dim3(dim3(K / 32, K / 32, kAlgebraSlices)), dim3(256), 0, st, 
       coef, static_cast<const __nv_bfloat16*>(w_bf16), w_f32, N, K, static_cast<__nv_bfloat16*>(wcat), bias,
-      static_cast<unsigned int*>(tickets), partial));
-  B200_LAUNCHED();
+      static_cast<unsigned int*>(tickets), partial);
   return OK;
 }
 
@@ -373,9 +339,8 @@ int b200_stem_s2d_u8(const void* x_u8_nhwc, void* z, int B, int H, int W, const 
     b[c] = -mean3[c] / std3[c];
   }
   const long long total = static_cast<long long>(B) * (H / 2 + 3) * (W / 2 + 3);
-  B200_CHECK_CUDA(launch_pdl(stem_s2d_u8_kernel, dim3(ew_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const unsigned char*>(x_u8_nhwc), static_cast<uint4*>(z), B, H, W, a[0], a[1], a[2], b[0], b[1], b[2]));
-  B200_LAUNCHED();
+  B200_LAUNCH(stem_s2d_u8_kernel, dim3(capped_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const unsigned char*>(x_u8_nhwc), static_cast<uint4*>(z), B, H, W, a[0], a[1], a[2], b[0], b[1], b[2]);
   return OK;
 }
 
@@ -387,9 +352,8 @@ int b200_normalize_u8_nhwc(const void* x_u8_nhwc, float* y_nchw, int B, int H, i
     a[c] = 1.0f / (255.0f * std3[c]);
     b[c] = -mean3[c] / std3[c];
   }
-  B200_CHECK_CUDA(launch_pdl(u8_nhwc_to_f32_nchw_kernel, dim3(ew_grid(static_cast<long long>(B) * H * W)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const unsigned char*>(x_u8_nhwc), y_nchw, B, H, W, a[0], a[1], a[2], b[0], b[1], b[2]));
-  B200_LAUNCHED();
+  B200_LAUNCH(u8_nhwc_to_f32_nchw_kernel, dim3(capped_grid(static_cast<long long>(B) * H * W)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const unsigned char*>(x_u8_nhwc), y_nchw, B, H, W, a[0], a[1], a[2], b[0], b[1], b[2]);
   return OK;
 }
 
@@ -397,9 +361,8 @@ int b200_subsample2(const void* x, void* xs, int B, int H, int W, int C, void* s
   B200_REQUIRE(C % 8 == 0 && B > 0 && H > 0 && W > 0, "subsample2: C=%d must be a multiple of 8", C);
   B200_REQUIRE(static_cast<long long>(B) * H * W * (C / 8) < (1LL << 32), "subsample2: tensor too large");
   const long long total = static_cast<long long>(B) * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
-  B200_CHECK_CUDA(launch_pdl(subsample2_kernel, dim3(ew_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint4*>(x), static_cast<uint4*>(xs), B, H, W, C / 8));
-  B200_LAUNCHED();
+  B200_LAUNCH(subsample2_kernel, dim3(capped_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const uint4*>(x), static_cast<uint4*>(xs), B, H, W, C / 8);
   return OK;
 }
 
@@ -407,9 +370,8 @@ int b200_add_even_pixels(void* gx, const void* gs, int B, int H, int W, int C, v
   B200_REQUIRE(C % 8 == 0 && B > 0 && H > 0 && W > 0, "add_even_pixels: C=%d must be a multiple of 8", C);
   B200_REQUIRE(static_cast<long long>(B) * H * W * (C / 8) < (1LL << 32), "add_even_pixels: tensor too large");
   const long long total = static_cast<long long>(B) * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
-  B200_CHECK_CUDA(launch_pdl(add_even_pixels_kernel, dim3(ew_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<uint4*>(gx), static_cast<const uint4*>(gs), B, H, W, C / 8));
-  B200_LAUNCHED();
+  B200_LAUNCH(add_even_pixels_kernel, dim3(capped_grid(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<uint4*>(gx), static_cast<const uint4*>(gs), B, H, W, C / 8);
   return OK;
 }
 

@@ -9,15 +9,6 @@
 using namespace b200;
 
 namespace {
-cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
-
-int ew_blocks(long long items) {
-  long long blocks = (items + 255) / 256;
-  const long long cap = static_cast<long long>(device_sm_count()) * 16;
-  if (blocks > cap) blocks = cap;
-  return blocks < 1 ? 1 : static_cast<int>(blocks);
-}
-
 const char* mae_bad_split(int B, int P, int Nm, int D) {
   if (B < 1 || B > 65535) return "B must be in [1, 65535]";
   if (P < 2 || P > kMaeMaxP) return "P must be in [2, 1024]";
@@ -38,8 +29,7 @@ extern "C" {
 int b200_mae_shuffle(const float* keys, int* ids, int* slot, int B, int P, void* stream) {
   MAE_REQUIRE_SPLIT("mae_shuffle", B, P, 1, 1);
   B200_REQUIRE(keys != nullptr && ids != nullptr && slot != nullptr, "mae_shuffle: keys, ids, slot must be non-null");
-  B200_CHECK_CUDA(launch_pdl(mae_shuffle_kernel, dim3(B), dim3(256), 0, as_stream(stream), keys, P, ids, slot));
-  B200_LAUNCHED();
+  B200_LAUNCH(mae_shuffle_kernel, dim3(B), dim3(256), 0, as_stream(stream), keys, P, ids, slot);
   return OK;
 }
 
@@ -52,9 +42,8 @@ int b200_mae_patchify(const float* x, const int* ids, void* vis, float* tgt, int
   B200_REQUIRE(x != nullptr && ids != nullptr && vis != nullptr && tgt != nullptr,
                "mae_patchify: x, ids, vis, tgt must be non-null");
   const long long n = static_cast<long long>(B) * P * p * p * C;
-  B200_CHECK_CUDA(launch_pdl(mae_patchify_kernel, dim3(ew_blocks(n)), dim3(256), 0, as_stream(stream), x, ids, B, C, H, W, p,
-                             Nm, static_cast<__nv_bfloat16*>(vis), tgt));
-  B200_LAUNCHED();
+  B200_LAUNCH(mae_patchify_kernel, dim3(capped_grid(n)), dim3(256), 0, as_stream(stream), x, ids, B, C, H, W, p,
+              Nm, static_cast<__nv_bfloat16*>(vis), tgt);
   return OK;
 }
 
@@ -67,12 +56,11 @@ int b200_mae_gather_rows(const float* src, long long src_rows_per_sample, int ro
   B200_REQUIRE(src != nullptr && ids != nullptr && dst != nullptr, "mae_gather_rows: src, ids, dst must be non-null");
   const long long total = static_cast<long long>(B) * n * D;
   if (dst_f32)
-    B200_CHECK_CUDA(launch_pdl(mae_gather_rows_kernel<float>, dim3(ew_blocks(total)), dim3(256), 0, as_stream(stream), src,
-                               src_rows_per_sample, row_offset, ids, B, P, s0, n, D, static_cast<float*>(dst)));
+    B200_LAUNCH(mae_gather_rows_kernel<float>, dim3(capped_grid(total)), dim3(256), 0, as_stream(stream), src,
+                src_rows_per_sample, row_offset, ids, B, P, s0, n, D, static_cast<float*>(dst));
   else
-    B200_CHECK_CUDA(launch_pdl(mae_gather_rows_kernel<__nv_bfloat16>, dim3(ew_blocks(total)), dim3(256), 0, as_stream(stream),
-                               src, src_rows_per_sample, row_offset, ids, B, P, s0, n, D, static_cast<__nv_bfloat16*>(dst)));
-  B200_LAUNCHED();
+    B200_LAUNCH(mae_gather_rows_kernel<__nv_bfloat16>, dim3(capped_grid(total)), dim3(256), 0, as_stream(stream),
+                src, src_rows_per_sample, row_offset, ids, B, P, s0, n, D, static_cast<__nv_bfloat16*>(dst));
   return OK;
 }
 
@@ -82,9 +70,8 @@ int b200_mae_assemble_fwd(const float* enc, const float* mask_embed, const float
   B200_REQUIRE(enc != nullptr && mask_embed != nullptr && dpos != nullptr && slot != nullptr && dec != nullptr,
                "mae_assemble_fwd: enc, mask_embed, dpos, slot, dec must be non-null");
   const long long total = static_cast<long long>(B) * P * D;
-  B200_CHECK_CUDA(launch_pdl(mae_assemble_fwd_kernel, dim3(ew_blocks(total)), dim3(256), 0, as_stream(stream), enc,
-                             mask_embed, dpos, slot, B, P, Nm, D, dec));
-  B200_LAUNCHED();
+  B200_LAUNCH(mae_assemble_fwd_kernel, dim3(capped_grid(total)), dim3(256), 0, as_stream(stream), enc,
+              mask_embed, dpos, slot, B, P, Nm, D, dec);
   return OK;
 }
 
@@ -93,19 +80,17 @@ int b200_mae_assemble_bwd(const void* g, const int* slot, void* g_enc, float* d_
   MAE_REQUIRE_SPLIT("mae_assemble_bwd", B, P, Nm, D);
   B200_REQUIRE(g != nullptr && slot != nullptr && g_enc != nullptr && d_dpos != nullptr,
                "mae_assemble_bwd: g, slot, g_enc, d_dpos must be non-null");
-  B200_CHECK_CUDA(launch_pdl(mae_assemble_bwd_kernel, dim3(P), dim3(256), 0, as_stream(stream),
-                             static_cast<const __nv_bfloat16*>(g), slot, B, P, Nm, D, static_cast<__nv_bfloat16*>(g_enc),
-                             d_dpos));
-  B200_LAUNCHED();
+  B200_LAUNCH(mae_assemble_bwd_kernel, dim3(P), dim3(256), 0, as_stream(stream),
+              static_cast<const __nv_bfloat16*>(g), slot, B, P, Nm, D, static_cast<__nv_bfloat16*>(g_enc),
+              d_dpos);
   return OK;
 }
 
 int b200_mae_pos_grad(const void* g, const int* slot, float* d_pos, int B, int P, int Nm, int D, void* stream) {
   MAE_REQUIRE_SPLIT("mae_pos_grad", B, P, Nm, D);
   B200_REQUIRE(g != nullptr && slot != nullptr && d_pos != nullptr, "mae_pos_grad: g, slot, d_pos must be non-null");
-  B200_CHECK_CUDA(launch_pdl(mae_pos_grad_kernel, dim3(P + 1), dim3(256), 0, as_stream(stream),
-                             static_cast<const __nv_bfloat16*>(g), slot, B, P, Nm, D, d_pos));
-  B200_LAUNCHED();
+  B200_LAUNCH(mae_pos_grad_kernel, dim3(P + 1), dim3(256), 0, as_stream(stream),
+              static_cast<const __nv_bfloat16*>(g), slot, B, P, Nm, D, d_pos);
   return OK;
 }
 
@@ -113,9 +98,8 @@ int b200_mae_scatter_masked(const void* dh, const int* slot, void* g, int B, int
   MAE_REQUIRE_SPLIT("mae_scatter_masked", B, P, Nm, D);
   B200_REQUIRE(dh != nullptr && slot != nullptr && g != nullptr, "mae_scatter_masked: dh, slot, g must be non-null");
   const long long total = static_cast<long long>(B) * P * D;
-  B200_CHECK_CUDA(launch_pdl(mae_scatter_masked_kernel, dim3(ew_blocks(total)), dim3(256), 0, as_stream(stream),
-                             static_cast<const __nv_bfloat16*>(dh), slot, B, P, Nm, D, static_cast<__nv_bfloat16*>(g)));
-  B200_LAUNCHED();
+  B200_LAUNCH(mae_scatter_masked_kernel, dim3(capped_grid(total)), dim3(256), 0, as_stream(stream),
+              static_cast<const __nv_bfloat16*>(dh), slot, B, P, Nm, D, static_cast<__nv_bfloat16*>(g));
   return OK;
 }
 
@@ -126,12 +110,10 @@ int b200_mae_mse(const float* pred, const float* target, long long n, float grad
   B200_REQUIRE(n >= 1 && n <= (1ll << 40), "mae_mse: n must be in [1, 2^40] (n=%lld)", n);
   B200_REQUIRE(pred != nullptr && target != nullptr && grad != nullptr && partial != nullptr && loss != nullptr,
                "mae_mse: pred, target, grad, partial, loss must be non-null");
-  B200_CHECK_CUDA(launch_pdl(mae_mse_kernel, dim3(kMaeMseBlocks), dim3(256), 0, as_stream(stream), pred, target, n, grad_scale,
-                             static_cast<__nv_bfloat16*>(grad), partial));
-  B200_LAUNCHED();
-  B200_CHECK_CUDA(launch_pdl(mae_mse_finish_kernel, dim3(1), dim3(32), 0, as_stream(stream), static_cast<const float*>(partial),
-                             kMaeMseBlocks, 1.0 / static_cast<double>(n), loss));
-  B200_LAUNCHED();
+  B200_LAUNCH(mae_mse_kernel, dim3(kMaeMseBlocks), dim3(256), 0, as_stream(stream), pred, target, n, grad_scale,
+              static_cast<__nv_bfloat16*>(grad), partial);
+  B200_LAUNCH(mae_mse_finish_kernel, dim3(1), dim3(32), 0, as_stream(stream), static_cast<const float*>(partial),
+              kMaeMseBlocks, 1.0 / static_cast<double>(n), loss);
   return OK;
 }
 

@@ -9,9 +9,6 @@
 using namespace b200;
 
 namespace {
-bool aligned16(const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-bool opt16(const void* p) { return p == nullptr || aligned16(p); }
-
 const char* mb_bad_shape(long long B, long long HW, int C) {
   if (B < 1 || B > 65535) return "B must be in [1, 65535]";
   if (HW < 1) return "HW must be >= 1";
@@ -27,8 +24,6 @@ const char* dw_bad_shape(int B, int H, int W, int C, int k, int stride) {
 }
 
 int out_size(int n, int stride) { return (n - 1) / stride + 1; }   // pad k/2, odd k
-
-cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
 }  // namespace
 
 #define MB_REQUIRE_SHAPE(what, msg)                                                 \
@@ -53,7 +48,10 @@ cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
 extern "C" {
 
 int b200_dw_partial_rows(long long rows, int C) {
-  if (rows < 1 || C < 8 || C % 8 != 0 || C > kRvMaxC) return -1;
+  if (rows < 1 || C < 8 || C % 8 != 0 || C > kRvMaxC) {
+    set_error("dw_partial_rows: rows must be >= 1 and C a multiple of 8 in [8, 8192] (rows=%lld C=%d)", rows, C);
+    return -1;
+  }
   return dw_geom(rows, C).blocks;
 }
 
@@ -72,20 +70,19 @@ int b200_dw_fwd(const void* x, const float* w, const float* scale, const float* 
   const bool pre = scale != nullptr, st = stats != nullptr;
 #define DW_FWD(K, S)                                                                                                      \
   if (pre && st)                                                                                                          \
-    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<K, S, true, true>, grid, dim3(256), 0, as_stream(stream), px, w, scale,     \
-                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block));                                 \
+    B200_LAUNCH(dw_fwd_kernel<K, S, true, true>, grid, dim3(256), 0, as_stream(stream), px, w, scale,                    \
+                shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block);                                                 \
   else if (pre)                                                                                                           \
-    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<K, S, true, false>, grid, dim3(256), 0, as_stream(stream), px, w, scale,    \
-                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block));                                 \
+    B200_LAUNCH(dw_fwd_kernel<K, S, true, false>, grid, dim3(256), 0, as_stream(stream), px, w, scale,                   \
+                shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block);                                                 \
   else if (st)                                                                                                            \
-    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<K, S, false, true>, grid, dim3(256), 0, as_stream(stream), px, w, scale,    \
-                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block));                                 \
+    B200_LAUNCH(dw_fwd_kernel<K, S, false, true>, grid, dim3(256), 0, as_stream(stream), px, w, scale,                   \
+                shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block);                                                 \
   else                                                                                                                    \
-    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<K, S, false, false>, grid, dim3(256), 0, as_stream(stream), px, w, scale,   \
-                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block))
+    B200_LAUNCH(dw_fwd_kernel<K, S, false, false>, grid, dim3(256), 0, as_stream(stream), px, w, scale,                  \
+                shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block)
   DW_DISPATCH(k, stride, DW_FWD);
 #undef DW_FWD
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -111,17 +108,16 @@ int b200_dw_dgrad(const void* dd, const float* w, const void* x, const float* sc
   const bool res = residual != nullptr;
 #define DW_DGRAD(K, S)                                                                                                    \
   if (pre)                                                                                                                \
-    B200_CHECK_CUDA(launch_pdl(dw_dgrad_kernel<K, S, true, false>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,    \
-                               scale, shift, pr, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block));                   \
+    B200_LAUNCH(dw_dgrad_kernel<K, S, true, false>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,                   \
+                scale, shift, pr, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block);                                   \
   else if (res)                                                                                                           \
-    B200_CHECK_CUDA(launch_pdl(dw_dgrad_kernel<K, S, false, true>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,    \
-                               scale, shift, pr, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block));                   \
+    B200_LAUNCH(dw_dgrad_kernel<K, S, false, true>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,                   \
+                scale, shift, pr, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block);                                   \
   else                                                                                                                    \
-    B200_CHECK_CUDA(launch_pdl(dw_dgrad_kernel<K, S, false, false>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,   \
-                               scale, shift, pr, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block))
+    B200_LAUNCH(dw_dgrad_kernel<K, S, false, false>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,                  \
+                scale, shift, pr, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block)
   DW_DISPATCH(k, stride, DW_DGRAD);
 #undef DW_DGRAD
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -149,17 +145,16 @@ int b200_dw_wgrad(const void* dd, const void* x, const float* scale, const float
   const bool pre = scale != nullptr;
 #define DW_WGRAD(K, S)                                                                                                    \
   if (pre)                                                                                                                \
-    B200_CHECK_CUDA(launch_pdl(dw_wgrad_kernel<K, S, true>, grid, dim3(256), 0, as_stream(stream), pdd, px, scale, shift,\
-                               pws, B, H, W, Ho, Wo, C, gm.rows_per_block));                                              \
+    B200_LAUNCH(dw_wgrad_kernel<K, S, true>, grid, dim3(256), 0, as_stream(stream), pdd, px, scale, shift,               \
+                pws, B, H, W, Ho, Wo, C, gm.rows_per_block);                                                              \
   else                                                                                                                    \
-    B200_CHECK_CUDA(launch_pdl(dw_wgrad_kernel<K, S, false>, grid, dim3(256), 0, as_stream(stream), pdd, px, scale,      \
-                               shift, pws, B, H, W, Ho, Wo, C, gm.rows_per_block))
+    B200_LAUNCH(dw_wgrad_kernel<K, S, false>, grid, dim3(256), 0, as_stream(stream), pdd, px, scale,                     \
+                shift, pws, B, H, W, Ho, Wo, C, gm.rows_per_block)
   DW_DISPATCH(k, stride, DW_WGRAD);
 #undef DW_WGRAD
   const long long n = static_cast<long long>(k) * k * C;
-  B200_CHECK_CUDA(launch_pdl(dw_wgrad_reduce_kernel, dim3(static_cast<unsigned>((n + 31) / 32)), dim3(256), 0,
-                             as_stream(stream), static_cast<const float*>(pws), dw, gm.blocks, k * k, C));
-  B200_LAUNCHED();
+  B200_LAUNCH(dw_wgrad_reduce_kernel, dim3(static_cast<unsigned>((n + 31) / 32)), dim3(256), 0,
+              as_stream(stream), static_cast<const float*>(pws), dw, gm.blocks, k * k, C);
   return OK;
 }
 
@@ -176,14 +171,13 @@ int b200_dw_relu_fwd(const void* x, const float* w, const float* scale, const fl
   auto* pd = static_cast<__nv_bfloat16*>(d);
 #define DWR_FWD(S)                                                                                                        \
   if (stats != nullptr)                                                                                                   \
-    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<3, S, kDwRelu, true>, grid, dim3(256), 0, as_stream(stream), px, w, scale,  \
-                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block));                                 \
+    B200_LAUNCH(dw_fwd_kernel<3, S, kDwRelu, true>, grid, dim3(256), 0, as_stream(stream), px, w, scale,                 \
+                shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block);                                                 \
   else                                                                                                                    \
-    B200_CHECK_CUDA(launch_pdl(dw_fwd_kernel<3, S, kDwRelu, false>, grid, dim3(256), 0, as_stream(stream), px, w, scale, \
-                               shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block))
+    B200_LAUNCH(dw_fwd_kernel<3, S, kDwRelu, false>, grid, dim3(256), 0, as_stream(stream), px, w, scale,                \
+                shift, pd, stats, B, H, W, Ho, Wo, C, gm.rows_per_block)
   DW_STRIDE_DISPATCH(stride, DWR_FWD);
 #undef DWR_FWD
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -201,11 +195,10 @@ int b200_dw_relu_dgrad(const void* dd, const float* w, const void* x, const floa
   const __nv_bfloat16* none = nullptr;
   auto* pdx = static_cast<__nv_bfloat16*>(dx);
 #define DWR_DGRAD(S)                                                                                                      \
-  B200_CHECK_CUDA(launch_pdl(dw_dgrad_kernel<3, S, kDwRelu, false>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,   \
-                             scale, shift, none, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block))
+  B200_LAUNCH(dw_dgrad_kernel<3, S, kDwRelu, false>, grid, dim3(256), 0, as_stream(stream), pdd, w, px,                  \
+              scale, shift, none, pdx, partial, B, H, W, Ho, Wo, C, gm.rows_per_block)
   DW_STRIDE_DISPATCH(stride, DWR_DGRAD);
 #undef DWR_DGRAD
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -223,14 +216,13 @@ int b200_dw_relu_wgrad(const void* dd, const void* x, const float* scale, const 
   const auto* px = static_cast<const __nv_bfloat16*>(x);
   float* pws = static_cast<float*>(ws);
 #define DWR_WGRAD(S)                                                                                                      \
-  B200_CHECK_CUDA(launch_pdl(dw_wgrad_kernel<3, S, kDwRelu>, grid, dim3(256), 0, as_stream(stream), pdd, px, scale, shift,\
-                             pws, B, H, W, Ho, Wo, C, gm.rows_per_block))
+  B200_LAUNCH(dw_wgrad_kernel<3, S, kDwRelu>, grid, dim3(256), 0, as_stream(stream), pdd, px, scale, shift,               \
+              pws, B, H, W, Ho, Wo, C, gm.rows_per_block)
   DW_STRIDE_DISPATCH(stride, DWR_WGRAD);
 #undef DWR_WGRAD
   const long long n = 9ll * C;
-  B200_CHECK_CUDA(launch_pdl(dw_wgrad_reduce_kernel, dim3(static_cast<unsigned>((n + 31) / 32)), dim3(256), 0,
-                             as_stream(stream), static_cast<const float*>(pws), dw, gm.blocks, 9, C));
-  B200_LAUNCHED();
+  B200_LAUNCH(dw_wgrad_reduce_kernel, dim3(static_cast<unsigned>((n + 31) / 32)), dim3(256), 0,
+              as_stream(stream), static_cast<const float*>(pws), dw, gm.blocks, 9, C);
   return OK;
 }
 
@@ -245,12 +237,11 @@ int b200_silu_bn_squeeze(const void* d, const float* scale, const float* shift, 
   const auto* pd = static_cast<const uint4*>(d);
   auto* po = static_cast<__nv_bfloat16*>(out16);
   if (mask != nullptr)
-    B200_CHECK_CUDA(launch_pdl(mb_image_sum_kernel<false, true>, grid, dim3(256), 0, as_stream(stream),
-                               static_cast<const uint4*>(nullptr), pd, scale, shift, mask, pool, po, HW, C, gm.gpc));
+    B200_LAUNCH(mb_image_sum_kernel<false, true>, grid, dim3(256), 0, as_stream(stream),
+                static_cast<const uint4*>(nullptr), pd, scale, shift, mask, pool, po, HW, C, gm.gpc);
   else
-    B200_CHECK_CUDA(launch_pdl(mb_image_sum_kernel<false, false>, grid, dim3(256), 0, as_stream(stream),
-                               static_cast<const uint4*>(nullptr), pd, scale, shift, mask, pool, po, HW, C, gm.gpc));
-  B200_LAUNCHED();
+    B200_LAUNCH(mb_image_sum_kernel<false, false>, grid, dim3(256), 0, as_stream(stream),
+                static_cast<const uint4*>(nullptr), pd, scale, shift, mask, pool, po, HW, C, gm.gpc);
   return OK;
 }
 
@@ -260,9 +251,8 @@ int b200_excite_fwd(const float* pool, const float* w1, const float* b1, const f
   B200_REQUIRE(Cr >= 1 && Cr <= 256, "excite_fwd: Cr must be in [1, 256] (Cr=%d)", Cr);
   const void* need[] = {pool, w1, b1, w2, b2, hpre, gate};
   for (const void* p : need) B200_REQUIRE(p != nullptr, "excite_fwd: pool, w1, b1, w2, b2, hpre, gate are required");
-  B200_CHECK_CUDA(launch_pdl(mb_excite_fwd_kernel, dim3(B), dim3(256), (C + Cr) * sizeof(float), as_stream(stream), pool,
-                             w1, b1, w2, b2, hpre, gate, C, Cr));
-  B200_LAUNCHED();
+  B200_LAUNCH(mb_excite_fwd_kernel, dim3(B), dim3(256), (C + Cr) * sizeof(float), as_stream(stream), pool,
+              w1, b1, w2, b2, hpre, gate, C, Cr);
   return OK;
 }
 
@@ -273,15 +263,14 @@ int b200_excite_bwd(const float* s, const float* pool, const float* hpre, const 
   B200_REQUIRE(Cr >= 1 && Cr <= 256, "excite_bwd: Cr must be in [1, 256] (Cr=%d)", Cr);
   const void* need[] = {s, pool, hpre, gate, w1, w2, dgp, dhp, dw1, db1, dw2, db2, dpool};
   for (const void* p : need) B200_REQUIRE(p != nullptr, "excite_bwd: every pointer is required");
-  B200_CHECK_CUDA(launch_pdl(mb_excite_bwd_image_kernel, dim3(B), dim3(256), C * sizeof(float), as_stream(stream), s, gate,
-                             hpre, w2, dgp, dhp, C, Cr));
+  B200_LAUNCH(mb_excite_bwd_image_kernel, dim3(B), dim3(256), C * sizeof(float), as_stream(stream), s, gate,
+              hpre, w2, dgp, dhp, C, Cr);
   const long long total = 2ll * C * Cr + C + Cr + static_cast<long long>(B) * C;
   long long blocks = (total + 255) / 256;
   if (blocks > 4 * kNumSMs * 8) blocks = 4 * kNumSMs * 8;
-  B200_CHECK_CUDA(launch_pdl(mb_excite_bwd_params_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0,
-                             as_stream(stream), static_cast<const float*>(dgp), static_cast<const float*>(dhp), hpre, pool,
-                             w1, dw1, db1, dw2, db2, dpool, B, C, Cr));
-  B200_LAUNCHED();
+  B200_LAUNCH(mb_excite_bwd_params_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0,
+              as_stream(stream), static_cast<const float*>(dgp), static_cast<const float*>(dhp), hpre, pool,
+              w1, dw1, db1, dw2, db2, dpool, B, C, Cr);
   return OK;
 }
 
@@ -292,11 +281,10 @@ int b200_gate_apply(const void* d, const float* scale, const float* shift, const
                "gate_apply: d, scale, shift, gate, a must be non-null and 16-byte aligned");
   const long long rows = static_cast<long long>(B) * HW;
   const RvGeom gm = repvgg_geom(rows, C);
-  B200_CHECK_CUDA(launch_pdl(mb_apply_kernel<true, false, false>, dim3(gm.blocks, gm.nchunk), dim3(256), 0,
-                             as_stream(stream), static_cast<const uint4*>(d), scale, shift, gate,
-                             static_cast<const uint4*>(nullptr), static_cast<uint4*>(a), rows, HW, C, gm.rows_per_block,
-                             gm.gpc));
-  B200_LAUNCHED();
+  B200_LAUNCH(mb_apply_kernel<true, false, false>, dim3(gm.blocks, gm.nchunk), dim3(256), 0,
+              as_stream(stream), static_cast<const uint4*>(d), scale, shift, gate,
+              static_cast<const uint4*>(nullptr), static_cast<uint4*>(a), rows, HW, C, gm.rows_per_block,
+              gm.gpc);
   return OK;
 }
 
@@ -306,10 +294,9 @@ int b200_gate_reduce(const void* da, const void* d, const float* scale, const fl
   B200_REQUIRE(aligned16(da) && aligned16(d) && aligned16(scale) && aligned16(shift) && s != nullptr,
                "gate_reduce: da, d, scale, shift must be non-null and 16-byte aligned, s non-null");
   const RvGeom gm = repvgg_geom(HW, C);
-  B200_CHECK_CUDA(launch_pdl(mb_image_sum_kernel<true, false>, dim3(B, gm.nchunk), dim3(256), 0, as_stream(stream),
-                             static_cast<const uint4*>(da), static_cast<const uint4*>(d), scale, shift,
-                             static_cast<const float*>(nullptr), s, static_cast<__nv_bfloat16*>(nullptr), HW, C, gm.gpc));
-  B200_LAUNCHED();
+  B200_LAUNCH(mb_image_sum_kernel<true, false>, dim3(B, gm.nchunk), dim3(256), 0, as_stream(stream),
+              static_cast<const uint4*>(da), static_cast<const uint4*>(d), scale, shift,
+              static_cast<const float*>(nullptr), s, static_cast<__nv_bfloat16*>(nullptr), HW, C, gm.gpc);
   return OK;
 }
 
@@ -325,14 +312,13 @@ int b200_silu_bn_bwd_reduce(const void* da, const float* gate, const float* dpoo
   const RvGeom gm = repvgg_geom(rows, C);
   const dim3 grid(gm.blocks, gm.nchunk);
   if (da != nullptr)
-    B200_CHECK_CUDA(launch_pdl(mb_bwd_reduce_kernel<true, true>, grid, dim3(256), 0, as_stream(stream),
-                               static_cast<const uint4*>(da), gate, dpool, static_cast<const uint4*>(d), scale, shift,
-                               static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(mb_bwd_reduce_kernel<true, true>, grid, dim3(256), 0, as_stream(stream),
+                static_cast<const uint4*>(da), gate, dpool, static_cast<const uint4*>(d), scale, shift,
+                static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc);
   else
-    B200_CHECK_CUDA(launch_pdl(mb_bwd_reduce_kernel<true, false>, grid, dim3(256), 0, as_stream(stream),
-                               static_cast<const uint4*>(da), gate, dpool, static_cast<const uint4*>(d), scale, shift,
-                               static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc));
-  B200_LAUNCHED();
+    B200_LAUNCH(mb_bwd_reduce_kernel<true, false>, grid, dim3(256), 0, as_stream(stream),
+                static_cast<const uint4*>(da), gate, dpool, static_cast<const uint4*>(d), scale, shift,
+                static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc);
   return OK;
 }
 
@@ -349,18 +335,17 @@ int b200_tail_apply(const void* c, const float* scale, const float* shift, const
   auto* py = static_cast<uint4*>(y);
   cudaStream_t st = as_stream(stream);
   if (rs != nullptr && residual != nullptr)
-    B200_CHECK_CUDA(launch_pdl(mb_apply_kernel<false, true, true>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
-                               rows, HW, C, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(mb_apply_kernel<false, true, true>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
+                rows, HW, C, gm.rows_per_block, gm.gpc);
   else if (rs != nullptr)
-    B200_CHECK_CUDA(launch_pdl(mb_apply_kernel<false, true, false>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
-                               rows, HW, C, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(mb_apply_kernel<false, true, false>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
+                rows, HW, C, gm.rows_per_block, gm.gpc);
   else if (residual != nullptr)
-    B200_CHECK_CUDA(launch_pdl(mb_apply_kernel<false, false, true>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
-                               rows, HW, C, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(mb_apply_kernel<false, false, true>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
+                rows, HW, C, gm.rows_per_block, gm.gpc);
   else
-    B200_CHECK_CUDA(launch_pdl(mb_apply_kernel<false, false, false>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
-                               rows, HW, C, gm.rows_per_block, gm.gpc));
-  B200_LAUNCHED();
+    B200_LAUNCH(mb_apply_kernel<false, false, false>, grid, dim3(256), 0, st, pc, scale, shift, rs, pr, py,
+                rows, HW, C, gm.rows_per_block, gm.gpc);
   return OK;
 }
 
@@ -376,14 +361,13 @@ int b200_tail_bwd_reduce(const void* g, const float* rs, const void* c, void* dz
   const dim3 grid(gm.blocks, gm.nchunk);
   const float* none = nullptr;
   if (rs != nullptr)
-    B200_CHECK_CUDA(launch_pdl(mb_bwd_reduce_kernel<false, true>, grid, dim3(256), 0, as_stream(stream),
-                               static_cast<const uint4*>(g), rs, none, static_cast<const uint4*>(c), none, none,
-                               static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(mb_bwd_reduce_kernel<false, true>, grid, dim3(256), 0, as_stream(stream),
+                static_cast<const uint4*>(g), rs, none, static_cast<const uint4*>(c), none, none,
+                static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc);
   else
-    B200_CHECK_CUDA(launch_pdl(mb_bwd_reduce_kernel<false, false>, grid, dim3(256), 0, as_stream(stream),
-                               static_cast<const uint4*>(g), rs, none, static_cast<const uint4*>(c), none, none,
-                               static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc));
-  B200_LAUNCHED();
+    B200_LAUNCH(mb_bwd_reduce_kernel<false, false>, grid, dim3(256), 0, as_stream(stream),
+                static_cast<const uint4*>(g), rs, none, static_cast<const uint4*>(c), none, none,
+                static_cast<uint4*>(dz), partial, rows, HW, C, gm.rows_per_block, gm.gpc);
   return OK;
 }
 

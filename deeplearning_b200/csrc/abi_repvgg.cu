@@ -9,8 +9,6 @@
 using namespace b200;
 
 namespace {
-bool aligned16(const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 // rows, C and the row pitches (in elements) of the pitched operands; returns a message or nullptr
 const char* rv_bad_shape(long long rows, int C) {
   if (rows < 1) return "rows must be >= 1";
@@ -28,7 +26,11 @@ const char* rv_bad_pitch(long long ld, int C) {
 extern "C" {
 
 int b200_repvgg_partial_rows(long long rows, int C) {
-  if (rv_bad_shape(rows, C) != nullptr) return -1;
+  const char* bad = rv_bad_shape(rows, C);
+  if (bad != nullptr) {
+    set_error("repvgg_partial_rows: %s (rows=%lld C=%d)", bad, rows, C);
+    return -1;
+  }
   return repvgg_geom(rows, C).blocks;
 }
 
@@ -53,18 +55,17 @@ int b200_repvgg_apply(const void* c3, long long ld3, const void* c1, long long l
   const auto* px = static_cast<const __nv_bfloat16*>(x);
   uint4* py = static_cast<uint4*>(y);
   if (id && stats)
-    B200_CHECK_CUDA(launch_pdl(repvgg_apply_kernel<true, true>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3, co1,
-                               co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats));
+    B200_LAUNCH(repvgg_apply_kernel<true, true>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3, co1,
+                co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats);
   else if (id)
-    B200_CHECK_CUDA(launch_pdl(repvgg_apply_kernel<true, false>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3, co1,
-                               co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats));
+    B200_LAUNCH(repvgg_apply_kernel<true, false>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3, co1,
+                co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats);
   else if (stats)
-    B200_CHECK_CUDA(launch_pdl(repvgg_apply_kernel<false, true>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3, co1,
-                               co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats));
+    B200_LAUNCH(repvgg_apply_kernel<false, true>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3, co1,
+                co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats);
   else
-    B200_CHECK_CUDA(launch_pdl(repvgg_apply_kernel<false, false>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3,
-                               co1, co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats));
-  B200_LAUNCHED();
+    B200_LAUNCH(repvgg_apply_kernel<false, false>, grid, dim3(256), 0, st, p3, ld3, p1, ld1, px, ldx, co3,
+                co1, co_id, py, rows, C, gm.rows_per_block, gm.gpc, stats);
   return OK;
 }
 
@@ -87,12 +88,11 @@ int b200_repvgg_bwd_reduce(const void* g, const void* y, const void* c3, long lo
   const auto* p1 = static_cast<const __nv_bfloat16*>(c1);
   const auto* px = static_cast<const __nv_bfloat16*>(x);
   if (x != nullptr)
-    B200_CHECK_CUDA(launch_pdl(repvgg_bwd_reduce_kernel<true>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx, rows,
-                               C, gm.rows_per_block, gm.gpc, partial));
+    B200_LAUNCH(repvgg_bwd_reduce_kernel<true>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx, rows,
+                C, gm.rows_per_block, gm.gpc, partial);
   else
-    B200_CHECK_CUDA(launch_pdl(repvgg_bwd_reduce_kernel<false>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx,
-                               rows, C, gm.rows_per_block, gm.gpc, partial));
-  B200_LAUNCHED();
+    B200_LAUNCH(repvgg_bwd_reduce_kernel<false>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx,
+                rows, C, gm.rows_per_block, gm.gpc, partial);
   return OK;
 }
 
@@ -123,12 +123,11 @@ int b200_repvgg_bwd_apply(const void* g, const void* y, const void* c3, long lon
   auto* d1 = static_cast<__nv_bfloat16*>(dc1);
   auto* dd = static_cast<__nv_bfloat16*>(dx);
   if (id)
-    B200_CHECK_CUDA(launch_pdl(repvgg_bwd_apply_kernel<true>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx, co3,
-                               m3, co1, m1, co_id, m_id, d3, d1, dd, rows, C, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(repvgg_bwd_apply_kernel<true>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx, co3,
+                m3, co1, m1, co_id, m_id, d3, d1, dd, rows, C, gm.rows_per_block, gm.gpc);
   else
-    B200_CHECK_CUDA(launch_pdl(repvgg_bwd_apply_kernel<false>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx, co3,
-                               m3, co1, m1, co_id, m_id, d3, d1, dd, rows, C, gm.rows_per_block, gm.gpc));
-  B200_LAUNCHED();
+    B200_LAUNCH(repvgg_bwd_apply_kernel<false>, grid, dim3(256), 0, st, pg, py, p3, ld3, p1, ld1, px, ldx, co3,
+                m3, co1, m1, co_id, m_id, d3, d1, dd, rows, C, gm.rows_per_block, gm.gpc);
   return OK;
 }
 
@@ -149,10 +148,9 @@ int b200_repvgg_fold(const float* w3, const float* w1, const float* gamma3, cons
   const RvFoldBn bi{gamma_id, beta_id, mean_id, var_id, eps_id};
   long long blocks = (static_cast<long long>(O) * ldk + 255) / 256;
   if (blocks > 4 * kNumSMs * 8) blocks = 4 * kNumSMs * 8;
-  B200_CHECK_CUDA(launch_pdl(repvgg_fold_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0,
-                             static_cast<cudaStream_t>(stream), w3, w1, b3, b1, bi, O, I, ldk,
-                             static_cast<__nv_bfloat16*>(wp), bias));
-  B200_LAUNCHED();
+  B200_LAUNCH(repvgg_fold_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0,
+              static_cast<cudaStream_t>(stream), w3, w1, b3, b1, bi, O, I, ldk,
+              static_cast<__nv_bfloat16*>(wp), bias);
   return OK;
 }
 

@@ -12,8 +12,6 @@ namespace {
 constexpr int kSeMaxCr = 256;
 constexpr int kSeMaxB = 65535;   // images travel in gridDim.y / gridDim.z
 
-bool aligned16(const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-
 // B, HW, C of the streaming passes; returns a message or nullptr
 const char* se_bad_shape(int B, int HW, int C) {
   if (B < 1 || B > kSeMaxB) return "B must be in [1, 65535]";
@@ -35,9 +33,8 @@ int b200_se_squeeze(const void* c, const float* scale, const float* shift, float
   SE_REQUIRE_SHAPE("se_squeeze", bad, B, HW, C, 0);
   B200_REQUIRE(aligned16(c) && aligned16(scale) && aligned16(shift) && csum != nullptr && pool != nullptr,
                "se_squeeze: c, scale, shift must be 16-byte aligned and csum, pool non-null");
-  B200_CHECK_CUDA(launch_pdl(se_squeeze_kernel, dim3(C / 64, B), dim3(256), 0, static_cast<cudaStream_t>(stream),
-      static_cast<const uint4*>(c), scale, shift, csum, pool, HW, C / 8));
-  B200_LAUNCHED();
+  B200_LAUNCH(se_squeeze_kernel, dim3(C / 64, B), dim3(256), 0, static_cast<cudaStream_t>(stream),
+      static_cast<const uint4*>(c), scale, shift, csum, pool, HW, C / 8);
   return OK;
 }
 
@@ -49,12 +46,10 @@ int b200_se_excite(const float* pool, const float* w1, const float* w2, float* h
   B200_REQUIRE(aligned16(pool) && aligned16(w1) && w2 != nullptr && h != nullptr && gate != nullptr,
                "se_excite: pool, w1 must be 16-byte aligned and w2, h, gate non-null");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  B200_CHECK_CUDA(launch_pdl(se_fc1_kernel, dim3((Cr + 7) / 8, (B + 7) / 8), dim3(256), 0, st, pool, w1, h, B, C, Cr));
-  B200_LAUNCHED();
+  B200_LAUNCH(se_fc1_kernel, dim3((Cr + 7) / 8, (B + 7) / 8), dim3(256), 0, st, pool, w1, h, B, C, Cr);
   const size_t smem = static_cast<size_t>(32 * (Cr + 1) + 8 * Cr) * sizeof(float);   // <= 41 KB at Cr = 256
-  B200_CHECK_CUDA(launch_pdl(se_fc2_kernel, dim3(C / 32, (B + 7) / 8), dim3(256), smem, st, static_cast<const float*>(h), w2,
-      gate, B, C, Cr));
-  B200_LAUNCHED();
+  B200_LAUNCH(se_fc2_kernel, dim3(C / 32, (B + 7) / 8), dim3(256), smem, st, static_cast<const float*>(h), w2,
+      gate, B, C, Cr);
   return OK;
 }
 
@@ -64,10 +59,9 @@ int b200_se_apply(const void* c, const void* identity, void* y, const float* sca
   SE_REQUIRE_SHAPE("se_apply", bad, B, HW, C, 0);
   B200_REQUIRE(aligned16(c) && aligned16(identity) && aligned16(y) && aligned16(scale) && aligned16(shift) && aligned16(gate),
                "se_apply: c, identity, y, scale, shift, gate must be non-null and 16-byte aligned");
-  B200_CHECK_CUDA(launch_pdl(se_apply_kernel, dim3((HW + kSeApplyRows - 1) / kSeApplyRows, C / 64, B), dim3(256), 0,
+  B200_LAUNCH(se_apply_kernel, dim3((HW + kSeApplyRows - 1) / kSeApplyRows, C / 64, B), dim3(256), 0,
       static_cast<cudaStream_t>(stream), static_cast<const uint4*>(c), static_cast<const uint4*>(identity),
-      static_cast<uint4*>(y), scale, shift, gate, HW, C / 8));
-  B200_LAUNCHED();
+      static_cast<uint4*>(y), scale, shift, gate, HW, C / 8);
   return OK;
 }
 
@@ -77,10 +71,9 @@ int b200_se_bwd_reduce(const void* g, const void* y, const void* c, void* dz, fl
   SE_REQUIRE_SHAPE("se_bwd_reduce", bad, B, HW, C, 0);
   B200_REQUIRE(aligned16(g) && aligned16(y) && aligned16(c) && aligned16(dz) && A != nullptr && R != nullptr,
                "se_bwd_reduce: g, y, c, dz must be 16-byte aligned and A, R non-null");
-  B200_CHECK_CUDA(launch_pdl(se_bwd_reduce_kernel, dim3(C / 64, B), dim3(256), 0, static_cast<cudaStream_t>(stream),
+  B200_LAUNCH(se_bwd_reduce_kernel, dim3(C / 64, B), dim3(256), 0, static_cast<cudaStream_t>(stream),
       static_cast<const uint4*>(g), static_cast<const uint4*>(y), static_cast<const uint4*>(c), static_cast<uint4*>(dz), A, R,
-      HW, C / 8));
-  B200_LAUNCHED();
+      HW, C / 8);
   return OK;
 }
 
@@ -96,19 +89,17 @@ int b200_se_bwd_coeffs(const float* A, const float* R, const float* csum, const 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int nj = (Cr + 31) / 32;
   const int blocks = nj * ((B + 7) / 8) + nj * (C / 32);
-  B200_CHECK_CUDA(launch_pdl(se_bwd_gate_kernel, dim3(blocks), dim3(256), 0, st, A, R, gate, h, w2, scale, shift, dh, dw2, B, C,
-      Cr));
-  B200_LAUNCHED();
+  B200_LAUNCH(se_bwd_gate_kernel, dim3(blocks), dim3(256), 0, st, A, R, gate, h, w2, scale, shift, dh, dw2, B, C,
+      Cr);
   static bool configured = false;   // w1 columns + a chunk of dh rows: up to 64 KB at Cr = 256
   if (!configured) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(se_bwd_bn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (32 + kSeDhRows) * kSeMaxCr * static_cast<int>(sizeof(float))));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(se_bwd_bn_kernel, dim3(C / 32, 1 + (Cr + 7) / 8), dim3(256),
+  B200_LAUNCH(se_bwd_bn_kernel, dim3(C / 32, 1 + (Cr + 7) / 8), dim3(256),
       static_cast<size_t>(32 + kSeDhRows) * Cr * sizeof(float), st, A, R, csum, pool, gate, static_cast<const float*>(dh), w1,
-      mean, invstd, dp, dw1, dgamma, dbeta, m1, m2, B, HW, C, Cr));
-  B200_LAUNCHED();
+      mean, invstd, dp, dw1, dgamma, dbeta, m1, m2, B, HW, C, Cr);
   return OK;
 }
 
@@ -120,10 +111,9 @@ int b200_se_bwd_apply(const void* dz, const void* c, void* dc, const float* gate
   B200_REQUIRE(aligned16(dz) && aligned16(c) && aligned16(dc) && aligned16(gate) && aligned16(dp) && aligned16(scale) &&
                    aligned16(mean) && aligned16(invstd) && aligned16(m1) && aligned16(m2),
                "se_bwd_apply: every pointer must be non-null and 16-byte aligned");
-  B200_CHECK_CUDA(launch_pdl(se_bwd_apply_kernel, dim3((HW + kSeApplyRows - 1) / kSeApplyRows, C / 64, B), dim3(256), 0,
+  B200_LAUNCH(se_bwd_apply_kernel, dim3((HW + kSeApplyRows - 1) / kSeApplyRows, C / 64, B), dim3(256), 0,
       static_cast<cudaStream_t>(stream), static_cast<const uint4*>(dz), static_cast<const uint4*>(c), static_cast<uint4*>(dc),
-      gate, dp, scale, mean, invstd, m1, m2, HW, C / 8));
-  B200_LAUNCHED();
+      gate, dp, scale, mean, invstd, m1, m2, HW, C / 8);
   return OK;
 }
 

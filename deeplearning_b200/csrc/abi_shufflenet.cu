@@ -9,24 +9,7 @@
 using namespace b200;
 
 namespace {
-bool aligned16(const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
-cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
-
-const char* sh_bad_shape(int B, int H, int W, int C) {
-  if (B < 1 || B > 65535) return "B must be in [1, 65535]";
-  if (H < 1 || W < 1) return "H and W must be >= 1";
-  if (C < 8 || C % 8 != 0 || C > kRvMaxC) return "C must be a multiple of 8 in [8, 8192]";
-  return nullptr;
-}
-
 int pool_out(int n) { return (n - 1) / 2 + 1; }   // output extent of a 3x3 / stride 2 / pad 1 window
-
-int ew_blocks(long long items) {
-  long long blocks = (items + 255) / 256;
-  const long long cap = static_cast<long long>(device_sm_count()) * 16;
-  if (blocks > cap) blocks = cap;
-  return blocks < 1 ? 1 : static_cast<int>(blocks);
-}
 
 int pad8(int n) { return (n + 7) / 8 * 8; }
 
@@ -47,23 +30,22 @@ extern "C" {
 
 int b200_shuffle_tail_s2_fwd(const void* x, const void* c3, const float* scale, const float* shift, void* y, int B, int H,
                              int W, int Cin, int Cc, void* stream) {
-  SH_REQUIRE_SHAPE("shuffle_tail_s2_fwd", sh_bad_shape(B, H, W, Cin), B, H, W, Cin);
+  SH_REQUIRE_SHAPE("shuffle_tail_s2_fwd", nhwc_bad_shape(B, H, W, Cin), B, H, W, Cin);
   B200_REQUIRE(Cc >= 8 && Cc % 8 == 0 && Cin + Cc <= kRvMaxC,
                "shuffle_tail_s2_fwd: Cc must be a multiple of 8 with Cin + Cc <= 8192 (Cin=%d Cc=%d)", Cin, Cc);
   B200_REQUIRE(aligned16(x) && aligned16(c3) && aligned16(scale) && aligned16(shift) && aligned16(y),
                "shuffle_tail_s2_fwd: x, c3, scale, shift, y must be non-null and 16-byte aligned");
   const int Ho = pool_out(H), Wo = pool_out(W);
   const long long n = static_cast<long long>(B) * Ho * Wo * ((Cin + Cc) / 8);
-  B200_CHECK_CUDA(launch_pdl(shuffle_tail_s2_fwd_kernel, dim3(ew_blocks(n)), dim3(256), 0, as_stream(stream),
-                             static_cast<const uint4*>(x), static_cast<const uint4*>(c3), scale, shift,
-                             static_cast<uint4*>(y), B, H, W, Ho, Wo, Cin, Cc));
-  B200_LAUNCHED();
+  B200_LAUNCH(shuffle_tail_s2_fwd_kernel, dim3(capped_grid(n)), dim3(256), 0, as_stream(stream),
+              static_cast<const uint4*>(x), static_cast<const uint4*>(c3), scale, shift,
+              static_cast<uint4*>(y), B, H, W, Ho, Wo, Cin, Cc);
   return OK;
 }
 
 int b200_shuffle_relu_bwd(const void* g, const void* y, const void* c, const float* scale, const float* shift, void* dz,
                           float* partial, void* gx, int B, int Ho, int Wo, int Cin, int Cc, int H, int W, void* stream) {
-  SH_REQUIRE_SHAPE("shuffle_relu_bwd", sh_bad_shape(B, Ho, Wo, Cc), B, Ho, Wo, Cc);
+  SH_REQUIRE_SHAPE("shuffle_relu_bwd", nhwc_bad_shape(B, Ho, Wo, Cc), B, Ho, Wo, Cc);
   B200_REQUIRE(Cin >= 0 && Cin % 8 == 0 && Cin + Cc <= kRvMaxC,
                "shuffle_relu_bwd: Cin must be a multiple of 8 >= 0 with Cin + Cc <= 8192 (Cin=%d Cc=%d)", Cin, Cc);
   B200_REQUIRE(aligned16(g) && aligned16(c) && aligned16(dz) && partial != nullptr,
@@ -88,15 +70,14 @@ int b200_shuffle_relu_bwd(const void* g, const void* y, const void* c, const flo
   auto* pgx = static_cast<uint4*>(gx);
   cudaStream_t st = as_stream(stream);
   if (pool)
-    B200_CHECK_CUDA(launch_pdl(shuffle_relu_bwd_kernel<true, true>, grid, dim3(256), 0, st, pg, py, pc, scale, shift, pdz,
-                               partial, pgx, B, H, W, Ho, Wo, Cin, Cc, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(shuffle_relu_bwd_kernel<true, true>, grid, dim3(256), 0, st, pg, py, pc, scale, shift, pdz,
+                partial, pgx, B, H, W, Ho, Wo, Cin, Cc, gm.rows_per_block, gm.gpc);
   else if (mask_y)
-    B200_CHECK_CUDA(launch_pdl(shuffle_relu_bwd_kernel<true, false>, grid, dim3(256), 0, st, pg, py, pc, scale, shift, pdz,
-                               partial, pgx, B, H, W, Ho, Wo, Cin, Cc, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(shuffle_relu_bwd_kernel<true, false>, grid, dim3(256), 0, st, pg, py, pc, scale, shift, pdz,
+                partial, pgx, B, H, W, Ho, Wo, Cin, Cc, gm.rows_per_block, gm.gpc);
   else
-    B200_CHECK_CUDA(launch_pdl(shuffle_relu_bwd_kernel<false, false>, grid, dim3(256), 0, st, pg, py, pc, scale, shift,
-                               pdz, partial, pgx, B, H, W, Ho, Wo, Cin, Cc, gm.rows_per_block, gm.gpc));
-  B200_LAUNCHED();
+    B200_LAUNCH(shuffle_relu_bwd_kernel<false, false>, grid, dim3(256), 0, st, pg, py, pc, scale, shift,
+                pdz, partial, pgx, B, H, W, Ho, Wo, Cin, Cc, gm.rows_per_block, gm.gpc);
   return OK;
 }
 
@@ -117,21 +98,20 @@ int b200_shufflev2_tail_fwd(const void* u, const float* u_scale, const float* u_
   const auto* pc = static_cast<const __nv_bfloat16*>(c3);
   auto* p0 = static_cast<uint4*>(y0);
   auto* p1 = static_cast<uint4*>(y1);
-  const dim3 grid(ew_blocks(n));
+  const dim3 grid(capped_grid(n));
   cudaStream_t st = as_stream(stream);
   if (bn_u && split)
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_fwd_kernel<true, true>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc, scale,
-                               shift, p0, p1, rows, b, bp, jp));
+    B200_LAUNCH(shufflev2_tail_fwd_kernel<true, true>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc, scale,
+                shift, p0, p1, rows, b, bp, jp);
   else if (bn_u)
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_fwd_kernel<true, false>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc,
-                               scale, shift, p0, p1, rows, b, bp, jp));
+    B200_LAUNCH(shufflev2_tail_fwd_kernel<true, false>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc,
+                scale, shift, p0, p1, rows, b, bp, jp);
   else if (split)
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_fwd_kernel<false, true>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc,
-                               scale, shift, p0, p1, rows, b, bp, jp));
+    B200_LAUNCH(shufflev2_tail_fwd_kernel<false, true>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc,
+                scale, shift, p0, p1, rows, b, bp, jp);
   else
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_fwd_kernel<false, false>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc,
-                               scale, shift, p0, p1, rows, b, bp, jp));
-  B200_LAUNCHED();
+    B200_LAUNCH(shufflev2_tail_fwd_kernel<false, false>, grid, dim3(256), 0, st, pu, u_scale, u_shift, pc,
+                scale, shift, p0, p1, rows, b, bp, jp);
   return OK;
 }
 
@@ -159,19 +139,18 @@ int b200_shufflev2_tail_bwd(const void* g0, const void* g1, const void* c3, cons
   auto* pd = static_cast<uint4*>(du);
   cudaStream_t st = as_stream(stream);
   if (bn_u && split)
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_bwd_kernel<true, true>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift, pz,
-                               partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(shufflev2_tail_bwd_kernel<true, true>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift, pz,
+                partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block, gm.gpc);
   else if (bn_u)
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_bwd_kernel<true, false>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift, pz,
-                               partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(shufflev2_tail_bwd_kernel<true, false>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift, pz,
+                partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block, gm.gpc);
   else if (split)
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_bwd_kernel<false, true>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift, pz,
-                               partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block, gm.gpc));
+    B200_LAUNCH(shufflev2_tail_bwd_kernel<false, true>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift, pz,
+                partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block, gm.gpc);
   else
-    B200_CHECK_CUDA(launch_pdl(shufflev2_tail_bwd_kernel<false, false>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift,
-                               pz, partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block,
-                               gm.gpc));
-  B200_LAUNCHED();
+    B200_LAUNCH(shufflev2_tail_bwd_kernel<false, false>, grid, dim3(256), 0, st, p0, p1, pc, scale, shift,
+                pz, partial3, pu, u_scale, u_shift, pd, partial_u, rows, b, bp, jp, gm.rows_per_block,
+                gm.gpc);
   return OK;
 }
 

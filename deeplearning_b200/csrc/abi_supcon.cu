@@ -10,15 +10,6 @@
 using namespace b200;
 
 namespace {
-cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
-
-int ew_blocks(long long items) {
-  long long blocks = (items + 255) / 256;
-  const long long cap = static_cast<long long>(device_sm_count()) * 16;
-  if (blocks > cap) blocks = cap;
-  return blocks < 1 ? 1 : static_cast<int>(blocks);
-}
-
 int row_blocks(int N, int rows_per_block) { return (N + rows_per_block - 1) / rows_per_block; }
 }  // namespace
 
@@ -33,9 +24,8 @@ int b200_supcon_max_dim(void) { return kSupconMaxD; }
 int b200_supcon_normalize_fwd(const float* z, float* e, float* nrm, int N, int D, void* stream) {
   SUPCON_REQUIRE_ROWS("supcon_normalize_fwd", N, D, 1 << 16);
   B200_REQUIRE(z != nullptr && e != nullptr && nrm != nullptr, "supcon_normalize_fwd: z, e, nrm must be non-null");
-  B200_CHECK_CUDA(launch_pdl(supcon_normalize_fwd_kernel, dim3(row_blocks(N, 8)), dim3(256), 0, as_stream(stream), z, N, D,
-                             e, nrm));
-  B200_LAUNCHED();
+  B200_LAUNCH(supcon_normalize_fwd_kernel, dim3(row_blocks(N, 8)), dim3(256), 0, as_stream(stream), z, N, D,
+              e, nrm);
   return OK;
 }
 
@@ -43,9 +33,8 @@ int b200_supcon_normalize_bwd(const float* de, const float* e, const float* nrm,
   SUPCON_REQUIRE_ROWS("supcon_normalize_bwd", N, D, 1 << 16);
   B200_REQUIRE(de != nullptr && e != nullptr && nrm != nullptr && dz != nullptr,
                "supcon_normalize_bwd: de, e, nrm, dz must be non-null");
-  B200_CHECK_CUDA(launch_pdl(supcon_normalize_bwd_kernel, dim3(row_blocks(N, 8)), dim3(256), 0, as_stream(stream), de, e,
-                             nrm, N, D, static_cast<__nv_bfloat16*>(dz)));
-  B200_LAUNCHED();
+  B200_LAUNCH(supcon_normalize_bwd_kernel, dim3(row_blocks(N, 8)), dim3(256), 0, as_stream(stream), de, e,
+              nrm, N, D, static_cast<__nv_bfloat16*>(dz));
   return OK;
 }
 
@@ -57,12 +46,10 @@ int b200_supcon_loss_fwd(const float* e, const int* labels, int N, int D, float 
                base_temperature);
   B200_REQUIRE(e != nullptr && labels != nullptr && L != nullptr && npos != nullptr && row_loss != nullptr && loss != nullptr,
                "supcon_loss_fwd: e, labels, L, npos, row_loss, loss must be non-null");
-  B200_CHECK_CUDA(launch_pdl(supcon_loss_fwd_kernel, dim3(row_blocks(N, kSupconBM)), dim3(256), 0, as_stream(stream), e,
-                             labels, N, D, 1.0f / temperature, temperature / base_temperature, L, npos, row_loss));
-  B200_LAUNCHED();
-  B200_CHECK_CUDA(launch_pdl(supcon_mean_kernel, dim3(1), dim3(256), 0, as_stream(stream), static_cast<const float*>(row_loss),
-                             N, loss));
-  B200_LAUNCHED();
+  B200_LAUNCH(supcon_loss_fwd_kernel, dim3(row_blocks(N, kSupconBM)), dim3(256), 0, as_stream(stream), e,
+              labels, N, D, 1.0f / temperature, temperature / base_temperature, L, npos, row_loss);
+  B200_LAUNCH(supcon_mean_kernel, dim3(1), dim3(256), 0, as_stream(stream), static_cast<const float*>(row_loss),
+              N, loss);
   return OK;
 }
 
@@ -84,19 +71,17 @@ int b200_supcon_loss_bwd(const float* e, const int* labels, const float* L, cons
   const size_t smem = static_cast<size_t>(kSupconBM) * D * sizeof(float);
   // dloss / de_i = (1 / tau) sum_j (G_ij + G_ji) e_j with G_ij = g (tau / base_tau) / N (softmax_ij - [j in P_i] / |P_i|)
   const float c = grad_scale * (temperature / base_temperature) / static_cast<float>(N) / temperature;
-  B200_CHECK_CUDA(launch_pdl(supcon_loss_bwd_kernel, dim3(row_blocks(N, kSupconBM)), dim3(256), smem, as_stream(stream), e,
-                             labels, L, npos, grad_out, c, N, D, 1.0f / temperature, de));
-  B200_LAUNCHED();
+  B200_LAUNCH(supcon_loss_bwd_kernel, dim3(row_blocks(N, kSupconBM)), dim3(256), smem, as_stream(stream), e,
+              labels, L, npos, grad_out, c, N, D, 1.0f / temperature, de);
   return OK;
 }
 
 int b200_supcon_relu_bwd(const void* dy, const void* y, void* dx, long long n, void* stream) {
   B200_REQUIRE(n >= 1 && n <= (1ll << 40), "supcon_relu_bwd: n must be in [1, 2^40] (n=%lld)", n);
   B200_REQUIRE(dy != nullptr && y != nullptr && dx != nullptr, "supcon_relu_bwd: dy, y, dx must be non-null");
-  B200_CHECK_CUDA(launch_pdl(supcon_relu_bwd_kernel, dim3(ew_blocks(n)), dim3(256), 0, as_stream(stream),
-                             static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(y), n,
-                             static_cast<__nv_bfloat16*>(dx)));
-  B200_LAUNCHED();
+  B200_LAUNCH(supcon_relu_bwd_kernel, dim3(capped_grid(n)), dim3(256), 0, as_stream(stream),
+              static_cast<const __nv_bfloat16*>(dy), static_cast<const __nv_bfloat16*>(y), n,
+              static_cast<__nv_bfloat16*>(dx));
   return OK;
 }
 

@@ -13,13 +13,6 @@
 using namespace b200;
 
 namespace {
-inline int grid_for(long long items, int per_block, int cap_mult = 16) {
-  long long blocks = (items + per_block - 1) / per_block;
-  const long long cap = static_cast<long long>(device_sm_count()) * cap_mult;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  return static_cast<int>(blocks);
-}
 int ln_bwd_blocks(long long rows) {
   long long b = static_cast<long long>(device_sm_count()) * 3;
   if (b > (rows + 7) / 8) b = (rows + 7) / 8;
@@ -40,8 +33,8 @@ int b200_layernorm_fwd(const void* x, int x_f32, const float* gamma, const float
   B200_REQUIRE(C % 8 == 0 && C <= 3072, "layernorm_fwd: C=%d must be a multiple of 8 and <= 3072", C);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #define LN_FWD(TI, TY, MV, LPR)                                                                                      \
-  B200_CHECK_CUDA(launch_pdl(layernorm_fwd_kernel<TI, TY, MV, LPR>, dim3(grid_for((rows + 32 / LPR - 1) / (32 / LPR), 8)), dim3(256), 0, st,             \
-      static_cast<const TI*>(x), gamma, beta, static_cast<TY*>(y), mean, rstd, rows, C, eps))
+  B200_LAUNCH(layernorm_fwd_kernel<TI, TY, MV, LPR>, dim3(capped_grid((rows + 32 / LPR - 1) / (32 / LPR), 8)), dim3(256), 0, st,                            \
+      static_cast<const TI*>(x), gamma, beta, static_cast<TY*>(y), mean, rstd, rows, C, eps)
 #define LN_FWD_T(MV, LPR)                              \
   do {                                                 \
     if (x_f32 && y_f32)                                \
@@ -63,12 +56,14 @@ int b200_layernorm_fwd(const void* x, int x_f32, const float* gamma, const float
     LN_FWD_T(12, 32);
 #undef LN_FWD_T
 #undef LN_FWD
-  B200_LAUNCHED();
   return OK;
 }
 
 int b200_layernorm_bwd_blocks(long long rows, int C) {
-  if (C % 8 != 0 || C > 1024) return -1;
+  if (C % 8 != 0 || C > 1024) {
+    set_error("layernorm_bwd_blocks: C=%d must be a multiple of 8 and <= 1024", C);
+    return -1;
+  }
   return ln_bwd_blocks(rows);
 }
 
@@ -88,9 +83,9 @@ int b200_layernorm_bwd(const void* dy, const void* x, int x_f32, const float* me
       cfg = true;                                                                                                   \
     }                                                                                                               \
     const size_t smem = static_cast<size_t>(8) * (32 / LPR) * 2 * C * sizeof(float);                                \
-    B200_CHECK_CUDA(launch_pdl(layernorm_bwd_kernel<TI, TO, MV, LPR>, dim3(grid), dim3(256), smem, st, dyp,         \
-                               static_cast<const TI*>(x), mean, rstd, gamma, static_cast<const TO*>(add),          \
-                               static_cast<TO*>(dx), partial, rows, C));                                            \
+    B200_LAUNCH(layernorm_bwd_kernel<TI, TO, MV, LPR>, dim3(grid), dim3(256), smem, st, dyp,                        \
+                static_cast<const TI*>(x), mean, rstd, gamma, static_cast<const TO*>(add),                         \
+                static_cast<TO*>(dx), partial, rows, C);                                                            \
   } while (0)
 #define LN_BWD(TI, TO)                  \
   do {                                  \
@@ -115,22 +110,19 @@ int b200_layernorm_bwd(const void* dy, const void* x, int x_f32, const float* me
     LN_BWD(__nv_bfloat16, __nv_bfloat16);
 #undef LN_BWD
 #undef LN_BWD_V
-  B200_LAUNCHED();
   return OK;
 }
 
 int b200_patchify_nchw(const float* x, void* a, int B, int Cin, int H, int W, int ps, void* stream) {
   B200_REQUIRE(ps % 4 == 0 && H % ps == 0 && W % ps == 0 && W % 4 == 0, "patchify: patch %d must divide %dx%d (multiples of 4)", ps, H, W);
   const long long total = static_cast<long long>(B) * (H / ps) * (W / ps) * (Cin * ps * ps / 4);
-  B200_CHECK_CUDA(launch_pdl(patchify_nchw_kernel, dim3(grid_for(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      x, static_cast<__nv_bfloat16*>(a), B, Cin, H, W, ps));
-  B200_LAUNCHED();
+  B200_LAUNCH(patchify_nchw_kernel, dim3(capped_grid(total, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      x, static_cast<__nv_bfloat16*>(a), B, Cin, H, W, ps);
   return OK;
 }
 
 int b200_cls_row(const float* cls, const float* pos, float* tokens, int B, int T, int D, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(cls_row_kernel, dim3(grid_for(static_cast<long long>(B) * D, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), cls, pos, tokens, B, T, D));
-  B200_LAUNCHED();
+  B200_LAUNCH(cls_row_kernel, dim3(capped_grid(static_cast<long long>(B) * D, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), cls, pos, tokens, B, T, D);
   return OK;
 }
 
@@ -138,10 +130,9 @@ int b200_batch_rowsum(const void* g, int g_f32, long long stride_b, int B, int D
                       void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (g_f32)
-    B200_CHECK_CUDA(launch_pdl(batch_rowsum_kernel<float>, dim3((D + 255) / 256), dim3(256), 0, st, static_cast<const float*>(g), stride_b, B, D, out, accumulate));
+    B200_LAUNCH(batch_rowsum_kernel<float>, dim3((D + 255) / 256), dim3(256), 0, st, static_cast<const float*>(g), stride_b, B, D, out, accumulate);
   else
-    B200_CHECK_CUDA(launch_pdl(batch_rowsum_kernel<__nv_bfloat16>, dim3((D + 255) / 256), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(g), stride_b, B, D, out, accumulate));
-  B200_LAUNCHED();
+    B200_LAUNCH(batch_rowsum_kernel<__nv_bfloat16>, dim3((D + 255) / 256), dim3(256), 0, st, static_cast<const __nv_bfloat16*>(g), stride_b, B, D, out, accumulate);
   return OK;
 }
 
@@ -149,9 +140,8 @@ int b200_copy_rows(const void* src, long long src_pitch_bytes, void* dst, long l
                    long long row_bytes, void* stream) {
   B200_REQUIRE(row_bytes % 16 == 0 && src_pitch_bytes % 16 == 0 && dst_pitch_bytes % 16 == 0,
                "copy_rows: sizes must be multiples of 16 bytes");
-  B200_CHECK_CUDA(launch_pdl(copy_rows_kernel, dim3(grid_for(rows * (row_bytes / 16), 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint8_t*>(src), src_pitch_bytes, static_cast<uint8_t*>(dst), dst_pitch_bytes, rows, row_bytes));
-  B200_LAUNCHED();
+  B200_LAUNCH(copy_rows_kernel, dim3(capped_grid(rows * (row_bytes / 16), 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const uint8_t*>(src), src_pitch_bytes, static_cast<uint8_t*>(dst), dst_pitch_bytes, rows, row_bytes);
   return OK;
 }
 
@@ -166,15 +156,13 @@ int b200_colsum_partial(const void* m, long long rows, long long ld, int cols, f
   B200_REQUIRE(cols % 8 == 0 && ld % 8 == 0 && (reinterpret_cast<uintptr_t>(m) & 15) == 0,
                "colsum_partial: cols=%d / ld=%lld must be multiples of 8 and the matrix 16-byte aligned", cols, ld);
   const int S = b200_colsum_partial_slices(rows);
-  B200_CHECK_CUDA(launch_pdl(colsum_partial_kernel, dim3(dim3((cols / 8 + 255) / 256, S)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const __nv_bfloat16*>(m), rows, ld, cols, partial));
-  B200_LAUNCHED();
+  B200_LAUNCH(colsum_partial_kernel, dim3(dim3((cols / 8 + 255) / 256, S)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const __nv_bfloat16*>(m), rows, ld, cols, partial);
   return OK;
 }
 
 int b200_dwconv7_pack(const float* w, float* wt, int C, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(dwconv7_pack_kernel, dim3((49 * C + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), w, wt, C));
-  B200_LAUNCHED();
+  B200_LAUNCH(dwconv7_pack_kernel, dim3((49 * C + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), w, wt, C);
   return OK;
 }
 
@@ -185,7 +173,7 @@ int b200_dwconv7(const void* in, int in_f32, const float* wt, const float* bias,
   B200_REQUIRE(C % 4 == 0, "dwconv7: C=%d must be a multiple of 4", C);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long total = static_cast<long long>(B) * H * ((W + 3) / 4) * (C / 4);
-  const int grid = grid_for(total, 128, 32);
+  const int grid = capped_grid(total, 128, 32);
   const bool tiled = dw_tiled(H, W, C);
   const long long tgrid = tiled ? static_cast<long long>(B) * (H / kDwTile) * (W / kDwTile) * (C / kDwCh) : 0;
   B200_REQUIRE(tgrid < (1ll << 31), "dwconv7: tensor too large");
@@ -198,10 +186,10 @@ int b200_dwconv7(const void* in, int in_f32, const float* wt, const float* bias,
                                            kTileSmem));                                                                   \
       cfg = true;                                                                                                         \
     }                                                                                                                     \
-    B200_CHECK_CUDA(launch_pdl(dwconv7_tile_kernel<TI, TO, F>, dim3(static_cast<unsigned>(tgrid)), dim3(128), kTileSmem, st,                                  \
-        static_cast<const TI*>(in), wt, bias, static_cast<const TO*>(add), static_cast<TO*>(out), B, H, W, C));            \
+    B200_LAUNCH(dwconv7_tile_kernel<TI, TO, F>, dim3(static_cast<unsigned>(tgrid)), dim3(128), kTileSmem, st,                                                 \
+        static_cast<const TI*>(in), wt, bias, static_cast<const TO*>(add), static_cast<TO*>(out), B, H, W, C);             \
   } else                                                                                                                  \
-    B200_CHECK_CUDA(launch_pdl(dwconv7_kernel<TI, TO, F>, dim3(grid), dim3(128), 0, st, static_cast<const TI*>(in), wt, bias, static_cast<const TO*>(add), static_cast<TO*>(out), B, H, W, C))
+    B200_LAUNCH(dwconv7_kernel<TI, TO, F>, dim3(grid), dim3(128), 0, st, static_cast<const TI*>(in), wt, bias, static_cast<const TO*>(add), static_cast<TO*>(out), B, H, W, C)
   if (in_f32 && !out_f32 && !flip)
     DW(float, __nv_bfloat16, false);
   else if (!in_f32 && !out_f32 && flip)
@@ -215,7 +203,6 @@ int b200_dwconv7(const void* in, int in_f32, const float* wt, const float* bias,
     return EUNSUPPORTED_;
   }
 #undef DW
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -257,12 +244,10 @@ int b200_dwconv7_wgrad(const void* du, const float* x, float* dw, void* workspac
       B200_CHECK_CUDA(cudaFuncSetAttribute(dwconv7_wgrad_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
       cfg = true;
     }
-    B200_CHECK_CUDA(launch_pdl(dwconv7_wgrad_tile_kernel, dim3(dim3(C / kDwCh, pl.blocks_y)), dim3(128), kSmem, st, 
-        static_cast<const __nv_bfloat16*>(du), x, static_cast<float*>(workspace), B, H, W, C, pl.tiles_per_cta));
-    B200_LAUNCHED();
-    B200_CHECK_CUDA(launch_pdl(dwconv7_wgrad_finalize_kernel, dim3((49 * C + 255) / 256), dim3(256), 0, st, static_cast<const float*>(workspace), pl.blocks_y, C,
-                                                                        dw, accumulate));
-    B200_LAUNCHED();
+    B200_LAUNCH(dwconv7_wgrad_tile_kernel, dim3(dim3(C / kDwCh, pl.blocks_y)), dim3(128), kSmem, st, 
+        static_cast<const __nv_bfloat16*>(du), x, static_cast<float*>(workspace), B, H, W, C, pl.tiles_per_cta);
+    B200_LAUNCH(dwconv7_wgrad_finalize_kernel, dim3((49 * C + 255) / 256), dim3(256), 0, st, static_cast<const float*>(workspace), pl.blocks_y, C,
+                                                                        dw, accumulate);
     return OK;
   }
   const int by = dw_wgrad_blocks_y(B, H);
@@ -271,53 +256,46 @@ int b200_dwconv7_wgrad(const void* du, const float* x, float* dw, void* workspac
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long rows = static_cast<long long>(B) * H;
   const int rpb = static_cast<int>((rows + by - 1) / by);
-  B200_CHECK_CUDA(launch_pdl(dwconv7_wgrad_kernel, dim3(dim3((C / 4 + 31) / 32, by)), dim3(224), 0, st, static_cast<const __nv_bfloat16*>(du), x,
-                                                                    static_cast<float*>(workspace), B, H, W, C, rpb));
-  B200_LAUNCHED();
-  B200_CHECK_CUDA(launch_pdl(dwconv7_wgrad_finalize_kernel, dim3((49 * C + 255) / 256), dim3(256), 0, st, static_cast<const float*>(workspace), by, C, dw, accumulate));
-  B200_LAUNCHED();
+  B200_LAUNCH(dwconv7_wgrad_kernel, dim3(dim3((C / 4 + 31) / 32, by)), dim3(224), 0, st, static_cast<const __nv_bfloat16*>(du), x,
+                                                                    static_cast<float*>(workspace), B, H, W, C, rpb);
+  B200_LAUNCH(dwconv7_wgrad_finalize_kernel, dim3((49 * C + 255) / 256), dim3(256), 0, st, static_cast<const float*>(workspace), by, C, dw, accumulate);
   return OK;
 }
 
 int b200_avgpool_any(const void* x, int x_f32, float* y, int B, int HW, int C, void* stream) {
   B200_REQUIRE(C % 4 == 0, "avgpool_any: C=%d must be a multiple of 4", C);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int grid = grid_for(static_cast<long long>(B) * (C / 4), 128);
+  const int grid = capped_grid(static_cast<long long>(B) * (C / 4), 128);
   if (x_f32)
-    B200_CHECK_CUDA(launch_pdl(avgpool_any_fwd_kernel<float>, dim3(grid), dim3(128), 0, st, static_cast<const float*>(x), y, B, HW, C));
+    B200_LAUNCH(avgpool_any_fwd_kernel<float>, dim3(grid), dim3(128), 0, st, static_cast<const float*>(x), y, B, HW, C);
   else
-    B200_CHECK_CUDA(launch_pdl(avgpool_any_fwd_kernel<__nv_bfloat16>, dim3(grid), dim3(128), 0, st, static_cast<const __nv_bfloat16*>(x), y, B, HW, C));
-  B200_LAUNCHED();
+    B200_LAUNCH(avgpool_any_fwd_kernel<__nv_bfloat16>, dim3(grid), dim3(128), 0, st, static_cast<const __nv_bfloat16*>(x), y, B, HW, C);
   return OK;
 }
 
 int b200_colsum_prod_partial(const void* a, const void* b, long long rows, long long ld, int cols, float* partial,
                              void* stream) {
   const int S = b200_colsum_partial_slices(rows);
-  B200_CHECK_CUDA(launch_pdl(colsum_prod_partial_kernel, dim3(dim3((cols + 63) / 64, S)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const __nv_bfloat16*>(a), static_cast<const __nv_bfloat16*>(b), rows, ld, cols, partial));
-  B200_LAUNCHED();
+  B200_LAUNCH(colsum_prod_partial_kernel, dim3(dim3((cols + 63) / 64, S)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const __nv_bfloat16*>(a), static_cast<const __nv_bfloat16*>(b), rows, ld, cols, partial);
   return OK;
 }
 
 int b200_layerscale_grads(const float* G, const float* W2, const float* b2, const float* gsum, const float* gamma,
                           float* dW2, float* db2, float* dgamma, int C, int K, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(layerscale_grads_kernel, dim3(C), dim3(256), 0, static_cast<cudaStream_t>(stream), G, W2, b2, gsum, gamma, dW2, db2, dgamma, C, K));
-  B200_LAUNCHED();
+  B200_LAUNCH(layerscale_grads_kernel, dim3(C), dim3(256), 0, static_cast<cudaStream_t>(stream), G, W2, b2, gsum, gamma, dW2, db2, dgamma, C, K);
   return OK;
 }
 
 int b200_adamw_tick(float* hyper, float beta1, float beta2, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(adamw_tick_kernel, dim3(1), dim3(32), 0, static_cast<cudaStream_t>(stream), hyper, beta1, beta2));
-  B200_LAUNCHED();
+  B200_LAUNCH(adamw_tick_kernel, dim3(1), dim3(32), 0, static_cast<cudaStream_t>(stream), hyper, beta1, beta2);
   return OK;
 }
 
 int b200_adamw(float* p, const float* g, float* m, float* v, const float* wd, long long n, const float* hyper,
                float beta1, float beta2, float eps, float gscale, const float* clip_coef, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(adamw_kernel, dim3(grid_for(n, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), p, g, m, v, wd, n, hyper, beta1, beta2,
-                                                                               eps, gscale, clip_coef));
-  B200_LAUNCHED();
+  B200_LAUNCH(adamw_kernel, dim3(capped_grid(n, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), p, g, m, v, wd, n, hyper, beta1, beta2,
+                                                                               eps, gscale, clip_coef);
   return OK;
 }
 
@@ -329,10 +307,8 @@ int b200_grad_clip_coef(const float* g, long long n, float gscale, float max_nor
   B200_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "grad_clip_coef: the gradient arena must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int blocks = b200_grad_clip_blocks();
-  B200_CHECK_CUDA(launch_pdl(grad_sumsq_partial_kernel, dim3(blocks), dim3(256), 0, st, g, n, partial));
-  B200_LAUNCHED();
-  B200_CHECK_CUDA(launch_pdl(grad_clip_coef_kernel, dim3(1), dim3(256), 0, st, partial, blocks, gscale, max_norm, clip));
-  B200_LAUNCHED();
+  B200_LAUNCH(grad_sumsq_partial_kernel, dim3(blocks), dim3(256), 0, st, g, n, partial);
+  B200_LAUNCH(grad_clip_coef_kernel, dim3(1), dim3(256), 0, st, partial, blocks, gscale, max_norm, clip);
   return OK;
 }
 
@@ -363,8 +339,7 @@ int b200_window_attention_fwd(const void* qkv, void* out, const float* bias_tab,
   if (grid < nH) grid = nH;
   const int total = B * (H / 7) * (W / 7);
   if (grid > (total + 1) / 2 * nH) grid = (total + 1) / 2 * nH;
-  B200_CHECK_CUDA(launch_pdl(wattn_fwd_kernel, dim3(grid), dim3(kWAttnFwdThreads), kWAttnFwdSmem, static_cast<cudaStream_t>(stream), p));
-  B200_LAUNCHED();
+  B200_LAUNCH(wattn_fwd_kernel, dim3(grid), dim3(kWAttnFwdThreads), kWAttnFwdSmem, static_cast<cudaStream_t>(stream), p);
   return OK;
 }
 
@@ -390,8 +365,7 @@ int b200_window_attention_bwd(const void* qkv, const void* out, const void* dout
   if (grid < nH) grid = nH;
   const int total = B * (H / 7) * (W / 7);
   if (grid > (total + 1) / 2 * nH) grid = (total + 1) / 2 * nH;
-  B200_CHECK_CUDA(launch_pdl(wattn_bwd_kernel, dim3(grid), dim3(kWAttnFwdThreads), kWAttnBwdSmem, static_cast<cudaStream_t>(stream), p));
-  B200_LAUNCHED();
+  B200_LAUNCH(wattn_bwd_kernel, dim3(grid), dim3(kWAttnFwdThreads), kWAttnBwdSmem, static_cast<cudaStream_t>(stream), p);
   return OK;
 }
 
@@ -400,14 +374,12 @@ int b200_window_bias_gather(const float* table, const long long* index, const fl
   const int nWm = mask != nullptr ? nW : 1;
   B200_REQUIRE(nH > 0 && nWm > 0, "window_bias_gather: bad sizes nH=%d nW=%d", nH, nW);
   const long long n = static_cast<long long>(nH) * nWm * 49 * 64;
-  B200_CHECK_CUDA(launch_pdl(wattn_bias_gather_kernel, dim3(grid_for(n, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), table, index, mask, nWm, bias_tab,
-                                                                                           nH));
-  B200_LAUNCHED();
+  B200_LAUNCH(wattn_bias_gather_kernel, dim3(capped_grid(n, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), table, index, mask, nWm, bias_tab,
+                                                                                           nH);
   return OK;
 }
 int b200_window_bias_scatter(const float* dbias, const long long* index, float* dtable, int nH, void* stream) {
-  B200_CHECK_CUDA(launch_pdl(wattn_bias_scatter_kernel, dim3((nH * 49 * 49 + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), dbias, index, dtable, nH));
-  B200_LAUNCHED();
+  B200_LAUNCH(wattn_bias_scatter_kernel, dim3((nH * 49 * 49 + 255) / 256), dim3(256), 0, static_cast<cudaStream_t>(stream), dbias, index, dtable, nH);
   return OK;
 }
 
@@ -418,9 +390,8 @@ int b200_window_partition(const void* in, void* out, int B, int H, int W, int C,
   const int cvec = C * elem_bytes / 16;
   const long long nvec = static_cast<long long>(B) * H * W * cvec;
   B200_REQUIRE(nvec < (1LL << 31), "window_partition: tensor too large (%lld 16-byte vectors)", nvec);
-  B200_CHECK_CUDA(launch_pdl(window_permute_kernel<false>, dim3(grid_for((nvec + 3) / 4, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint4*>(in), static_cast<uint4*>(out), B, H, W, cvec, shift, ws));
-  B200_LAUNCHED();
+  B200_LAUNCH(window_permute_kernel<false>, dim3(capped_grid((nvec + 3) / 4, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const uint4*>(in), static_cast<uint4*>(out), B, H, W, cvec, shift, ws);
   return OK;
 }
 int b200_window_merge(const void* in, void* out, int B, int H, int W, int C, int shift, int ws, int elem_bytes,
@@ -430,9 +401,8 @@ int b200_window_merge(const void* in, void* out, int B, int H, int W, int C, int
   const int cvec = C * elem_bytes / 16;
   const long long nvec = static_cast<long long>(B) * H * W * cvec;
   B200_REQUIRE(nvec < (1LL << 31), "window_merge: tensor too large (%lld 16-byte vectors)", nvec);
-  B200_CHECK_CUDA(launch_pdl(window_permute_kernel<true>, dim3(grid_for((nvec + 3) / 4, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      static_cast<const uint4*>(in), static_cast<uint4*>(out), B, H, W, cvec, shift, ws));
-  B200_LAUNCHED();
+  B200_LAUNCH(window_permute_kernel<true>, dim3(capped_grid((nvec + 3) / 4, 256)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      static_cast<const uint4*>(in), static_cast<uint4*>(out), B, H, W, cvec, shift, ws);
   return OK;
 }
 
@@ -440,9 +410,8 @@ int b200_patch_merge_ln_fwd(const float* x, const float* gamma, const float* bet
                             int B, int H, int W, int C, float eps, void* stream) {
   B200_REQUIRE(C % 8 == 0 && 4 * C <= 2048 && H % 2 == 0 && W % 2 == 0, "patch_merge_ln: C=%d H=%d W=%d unsupported", C, H, W);
   const long long rows = static_cast<long long>(B) * (H / 2) * (W / 2);
-  B200_CHECK_CUDA(launch_pdl(patch_merge_ln_fwd_kernel<8>, dim3(grid_for(rows, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
-      x, gamma, beta, static_cast<__nv_bfloat16*>(y), mean, rstd, B, H, W, C, eps));
-  B200_LAUNCHED();
+  B200_LAUNCH(patch_merge_ln_fwd_kernel<8>, dim3(capped_grid(rows, 8)), dim3(256), 0, static_cast<cudaStream_t>(stream), 
+      x, gamma, beta, static_cast<__nv_bfloat16*>(y), mean, rstd, B, H, W, C, eps);
   return OK;
 }
 int b200_patch_merge_ln_bwd_blocks(long long rows) { return ln_bwd_blocks(rows); }
@@ -456,9 +425,8 @@ int b200_patch_merge_ln_bwd(const void* dy, const float* x, const float* mean, c
     B200_CHECK_CUDA(cudaFuncSetAttribute(patch_merge_ln_bwd_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 2048 * 4));
     cfg = true;
   }
-  B200_CHECK_CUDA(launch_pdl(patch_merge_ln_bwd_kernel<8>, dim3(ln_bwd_blocks(rows)), dim3(256), smem, static_cast<cudaStream_t>(stream), 
-      static_cast<const __nv_bfloat16*>(dy), x, mean, rstd, gamma, static_cast<__nv_bfloat16*>(dx), partial, B, H, W, C));
-  B200_LAUNCHED();
+  B200_LAUNCH(patch_merge_ln_bwd_kernel<8>, dim3(ln_bwd_blocks(rows)), dim3(256), smem, static_cast<cudaStream_t>(stream), 
+      static_cast<const __nv_bfloat16*>(dy), x, mean, rstd, gamma, static_cast<__nv_bfloat16*>(dx), partial, B, H, W, C);
   return OK;
 }
 
@@ -472,7 +440,7 @@ int launch_attn_fwd(const AttnFwdParams& p, int grid, cudaStream_t st) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd2_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttn2SmemBytes));
     configured = true;
   }
-  B200_CHECK_CUDA(launch_pdl(attn_fwd2_kernel<NT>, dim3(grid), dim3(kAttn2Threads), kAttn2SmemBytes, st, p));
+  B200_LAUNCH(attn_fwd2_kernel<NT>, dim3(grid), dim3(kAttn2Threads), kAttn2SmemBytes, st, p);
   return OK;
 }
 }  // namespace
@@ -505,7 +473,6 @@ int b200_attention_fwd(const void* qkv, void* out, float* lse, int B, int T, int
     default: rc = launch_attn_fwd<256>(p, grid, st); break;
   }
   if (rc) return rc;
-  B200_LAUNCHED();
   return OK;
 }
 
@@ -515,9 +482,8 @@ int b200_attention_bwd(const void* qkv, const void* out, const void* dout, const
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   {
     const long long rows = static_cast<long long>(B) * T * H;
-    B200_CHECK_CUDA(launch_pdl(attn_delta_kernel, dim3(grid_for(rows, 128)), dim3(256), 0, st, 
-        static_cast<const __nv_bfloat16*>(dout), static_cast<const __nv_bfloat16*>(out), delta, B, T, H));
-    B200_LAUNCHED();
+    B200_LAUNCH(attn_delta_kernel, dim3(capped_grid(rows, 128)), dim3(256), 0, st, 
+        static_cast<const __nv_bfloat16*>(dout), static_cast<const __nv_bfloat16*>(out), delta, B, T, H);
   }
   AttnBwdParams p;
   memset(&p, 0, sizeof(p));
@@ -537,8 +503,7 @@ int b200_attention_bwd(const void* qkv, const void* out, const void* dout, const
     B200_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnBwdSmemBytes));
     cfg = true;
   }
-  B200_CHECK_CUDA(launch_pdl(attn_bwd_kernel, dim3(B * H), dim3(kAttnBwdThreads), kAttnBwdSmemBytes, st, p));
-  B200_LAUNCHED();
+  B200_LAUNCH(attn_bwd_kernel, dim3(B * H), dim3(kAttnBwdThreads), kAttnBwdSmemBytes, st, p);
   return OK;
 }
 

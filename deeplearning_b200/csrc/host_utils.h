@@ -42,18 +42,35 @@ int encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t
 
 int device_sm_count();
 
+// Blocks of a grid-stride pass over `items` work items: ceil(items / per_block), at least 1 and at most cap_mult blocks
+// per SM. The fixed-order reductions sum per block, so their results depend on this count.
+inline int capped_grid(long long items, int per_block = 256, int cap_mult = 16) {
+  long long blocks = (items + per_block - 1) / per_block;
+  const long long cap = static_cast<long long>(device_sm_count()) * cap_mult;
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  return static_cast<int>(blocks);
+}
+
+inline bool aligned16(const void* p) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+inline bool opt16(const void* p) { return p == nullptr || aligned16(p); }   // optional operand: NULL or 16-byte aligned
+inline cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
+
+// B, H, W, C of an NHWC bf16 map that the row passes read 8 channels at a time (C <= kRvMaxC of row_passes.cuh);
+// returns a message or nullptr
+inline const char* nhwc_bad_shape(int B, int H, int W, int C) {
+  if (B < 1 || B > 65535) return "B must be in [1, 65535]";
+  if (H < 1 || W < 1) return "H and W must be >= 1";
+  if (C < 8 || C % 8 != 0 || C > 8192) return "C must be a multiple of 8 in [8, 8192]";
+  return nullptr;
+}
+
 // Number of kernels this library has launched (process-wide); see b200_launch_count().
 extern unsigned long long g_launch_count;
 
-#define B200_LAUNCHED()                                   \
-  do {                                                    \
-    ++::b200::g_launch_count;                             \
-    B200_CHECK_CUDA(cudaPeekAtLastError());               \
-  } while (0)
-
 // Launch with programmatic stream serialization (see common.cuh pdl_wait): the kernel may be scheduled while its
 // predecessor in the stream drains; every kernel of the library waits for that predecessor (griddepcontrol.wait) before it
-// touches global memory.
+// touches global memory. Called only through B200_LAUNCH.
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg;
@@ -69,5 +86,15 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
   cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
+
+// B200_LAUNCH(kernel, grid, block, smem, stream, args...): every kernel launch of the library. Launches with launch_pdl,
+// counts the kernel in g_launch_count and checks the launch; on failure the enclosing entry returns ECUDA_. (Variadic, so
+// that a kernel's template argument list needs no parentheses.)
+#define B200_LAUNCH(...)                                   \
+  do {                                                     \
+    B200_CHECK_CUDA(::b200::launch_pdl(__VA_ARGS__));      \
+    ++::b200::g_launch_count;                              \
+    B200_CHECK_CUDA(cudaPeekAtLastError());                \
+  } while (0)
 
 }  // namespace b200

@@ -10,7 +10,7 @@ import weakref
 
 import torch
 
-from .. import _lib, ops
+from .. import ops
 
 
 class ModelPack:
@@ -77,10 +77,7 @@ class ModelPack:
         if stamp == self.stamp:
             return
         self._build_table()
-        lib = _lib.load()
-        rc = lib.b200_pack_weights_multi(self.table.data_ptr(), len(self._rows), self.total_blocks,
-                                         torch.cuda.current_stream().cuda_stream)
-        _lib.check(rc, "b200_pack_weights_multi")
+        ops._call("pack_weights_multi", self.table.data_ptr(), len(self._rows), self.total_blocks)
         self.stamp = stamp
 
     def get(self, param, mode):

@@ -93,9 +93,7 @@ def _engine_for(model):
 
 
 def ops_clip_blocks():
-    from .. import _lib
-
-    return _lib.load().b200_grad_clip_blocks()
+    return ops._query("grad_clip_blocks")
 
 
 class FlatArena:
